@@ -152,7 +152,9 @@ static int launch_pass(wf_ctx* ctx, int mode, NttPassParams& p, u32 n_segments, 
             CKI(get_pow_table(ctx, p.logM, p.tw_split, &p.tw_lo));
             CKI(get_pow_table(ctx, p.logM - p.tw_split, p.logM - p.tw_split, &p.tw_hi));
         }
-        p.vec_in = p.vec_out = (p.W >= 2 || mode == NTT_STRIDED) ? 1 : 0;
+        // a lane pair of a one-column segment spans two tile columns: adjacent words only in the plain strided layout
+        p.vec_in = (p.W >= 2 || mode == NTT_STRIDED) ? 1 : 0;
+        p.vec_out = (p.W >= 2 || (mode == NTT_STRIDED && !p.y_in_out)) ? 1 : 0;
         CK(ntt2_launch_pass(mode, p, n_segments, n_batch, ctx->st));
     } else {
         CKI(wf_get_twiddles(ctx, std::max((u32)p.logS, 1u), &p.sub_tw));
@@ -350,39 +352,36 @@ static int run_lde(wf_ctx* ctx, const SegMatrix& polys, SegMatrix& out, u32 log_
         if (sc) CKI(set_scatter(ctx, p, *sc, log_b, k0));
         return launch_pass(ctx, NTT_CONTIG, p, polys.nseg(), k1 - k0);
     }
-    // Cosets per launch (grid.z = coset). The scratch Y of one coset is as large as the polynomials; while
-    // it fits in half of the L2 the contiguous pass finds most of it there, so cosets are processed
-    // kb at a time with kb chosen to keep kb * |polys| <= L2 / 2 (never less than one coset; narrow matrices
-    // whose tiles would not fill the SMs, two blocks resident on each, take all cosets at once).
-    const size_t poly_bytes = polys.words() * 8;
-    const size_t tiles_per_coset = (((size_t)1 << logC) * polys.nseg());  // strided-pass blocks (x chunks)
-    u32 kb = b;
-    while (kb > 1 && poly_bytes * kb > ctx->l2_bytes / 2 && tiles_per_coset * (kb / 2) >= 4 * 2 * (size_t)ctx->sms) kb >>= 1;
-    while (kb > 1 && poly_bytes * kb > ((size_t)1 << 30)) kb >>= 1;
-    while (kb > k1 - k0 || (k1 - k0) % kb) kb >>= 1;
+    // Two passes, one launch each for all cosets [k0, k1) (batch z = coset k0 + z): Y_k is written into the rows of `out` that
+    // X_k will occupy and pass 2 transforms it in place, so the polynomials are read once and no scratch is needed. A
+    // scattered output is not written locally: there Y goes to a scratch as large as the polynomials, one coset at a time.
     SegMatrix y = polys;
-    void* yp;
-    CKI(wf_dev_alloc(ctx, poly_bytes * kb, &yp));
-    y.base = (u64*)yp;
+    void* yp = nullptr;
+    if (sc) {
+        CKI(wf_dev_alloc(ctx, polys.words() * 8, &yp));
+        y.base = (u64*)yp;
+    }
+    const u32 kb = sc ? 1 : k1 - k0;
     int rc = WF_OK;
     for (u32 k = k0; k < k1 && rc == WF_OK; k += kb) {
         // pass 1: Y_k[j1][m2] = 7^m2 w_N^((b j1 + k) m2) sum_m1 a[C m1 + m2] (s_k^C)^m1 w_R^(j1 m1)
-        pass_defaults(p, polys, y);
+        pass_defaults(p, polys, sc ? y : out);
         p.logS = (int)logR; p.logR = logR; p.logC = logC;
         p.pre_tab = tabs.pre + ((size_t)k << logR); p.pre_batch_stride = (size_t)1 << logR;
-        p.out_batch_stride = polys.words();
         // exponent (b*j1 + k)*m2 = (j1*a_mul + (batch0 + z)*b_mul)*m2
         p.has_post = 1; p.logM = log_n + log_b; p.a_mul = b; p.b_mul = 1; p.batch0 = k;
         p.ctab = tabs.pow7;
+        if (!sc) { p.y_in_out = 1; p.out_row_mul = row_mul; p.out_row_add = row_add; p.out_col0 = out_col0; }
         rc = launch_pass(ctx, NTT_STRIDED, p, polys.nseg(), kb);
         if (rc != WF_OK) break;
         // pass 2: X_k[j1 + R j2] = sum_m2 Y_k[j1][m2] w_C^(j2 m2)  -> row b*(j1 + R j2) + k
-        pass_defaults(p, y, out);
+        pass_defaults(p, polys, out);
+        p.in = sc ? y.base : out.base;
+        p.in_seg_stride = sc ? y.seg_stride : out.seg_stride;
         p.logS = (int)logC; p.logR = logR; p.logC = logC;
-        p.in_batch_stride = polys.words();
         p.out_row_mul = row_mul; p.out_row_add = row_add; p.out_col0 = out_col0;
-        p.out = out.base + (size_t)(k - k0) * row_add * out.W;  // first coset of the launch; the launch's coset z adds z * row_add rows
         if (sc) { rc = set_scatter(ctx, p, *sc, log_b, k); if (rc != WF_OK) break; }
+        else p.y_in_out = 1;
         rc = launch_pass(ctx, NTT_CONTIG, p, polys.nseg(), kb);
     }
     wf_dev_free(ctx, yp);
@@ -444,14 +443,8 @@ int wf_ctx_create(wf_ctx** out, int device, void* stream) {
     if (e != cudaSuccess || n == 0) return WF_ERR_CUDA;  // no CPU fallback
     if (device < 0 || device >= n) return WF_ERR_INVALID;
     if (cudaSetDevice(device) != cudaSuccess) return WF_ERR_CUDA;
-    int sms = 0, l2 = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess ||
-        cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, device) != cudaSuccess)
-        return WF_ERR_CUDA;
     wf_ctx* ctx = new wf_ctx();
     ctx->device = device;
-    ctx->sms = sms;
-    ctx->l2_bytes = (size_t)l2;
     ctx->st = (cudaStream_t)stream;
     ctx->launches = 0;
     ctx->pinned = nullptr;

@@ -26,8 +26,6 @@ struct LdeTables {
 
 struct wf_ctx {
     int device;
-    int sms;                                 // streaming multiprocessors of the device
-    size_t l2_bytes;                         // L2 cache size of the device
     cudaStream_t st;
     std::string err;
     uint64_t launches;

@@ -53,6 +53,13 @@ struct NttPassParams {
     int inverse;                               // 1: inverse sub-transform (index-reversed output)
     // CONTIG output row mapping: out_row = row * out_row_mul + batch * out_row_add
     u32 out_row_mul, out_row_add;
+    // y_in_out = 1 (two-pass LDE): the intermediate Y[j1][m2] of the four-step schedule lives in the output matrix, in the
+    // row that X[j1 + R m2] will occupy, (j1 + R m2) * out_row_mul + batch * out_row_add at out_col0 of the out_W-wide rows.
+    // The STRIDED pass writes it there and the CONTIG pass reads it from there (in == out: in place; every block reads
+    // exactly the rows and lanes it writes). The batch index is then blockIdx.x, so that the cosets of one tile run side
+    // by side: the STRIDED pass reads each input tile from HBM once and every 512-byte group of output rows is written
+    // while it is in L2. ntt2 kernels only.
+    int y_in_out;
     // CONTIG output segment geometry: the output matrix may be wider than the input segment (a column
     // chunk of W columns lands at column offset out_col0 of an out_W-wide segment row)
     u32 out_W, out_col0;

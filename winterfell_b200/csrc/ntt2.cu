@@ -168,7 +168,8 @@ __device__ __forceinline__ void tile_round(u64* __restrict__ s, const u64* __res
 }
 
 // ---- the pass kernel ------------------------------------------------------------------------------------
-// grid = (tile columns x chunks per row, segments, batch). Shared memory:
+// grid = (tile columns x chunks per row, segments, batch), or (batch, tile columns x chunks per row, segments) with
+// y_in_out. Shared memory:
 //   tile [S][LANES] | round twiddles [tw_entries] | post twiddles [S][T] (STRIDED with has_post) | mbarrier
 template <int MODE, int LOGS>
 __global__ void __launch_bounds__(NTT2_THREADS, NTT2_MINB) ntt2_pass_kernel(const NttPassParams p) {
@@ -184,8 +185,10 @@ __global__ void __launch_bounds__(NTT2_THREADS, NTT2_MINB) ntt2_pass_kernel(cons
     u64* ctw = rtw + Plan<LOGS>::tw_entries;
     u64* mbar = ctw + (p.has_post ? (size_t)S * T : 0);
 
-    const u32 tile = blockIdx.x / chunks, q0 = (blockIdx.x % chunks) * LANES;
-    const u32 g = blockIdx.y, b = blockIdx.z;
+    const bool ymap = p.y_in_out;
+    const u32 tc = ymap ? blockIdx.y : blockIdx.x;
+    const u32 tile = tc / chunks, q0 = (tc % chunks) * LANES;
+    const u32 g = ymap ? blockIdx.z : blockIdx.y, b = ymap ? blockIdx.x : blockIdx.z;
     const u32 R = 1u << p.logR, C = 1u << p.logC;
     const u32 ncols = MODE == NTT_STRIDED ? C : R;
 
@@ -242,10 +245,16 @@ __global__ void __launch_bounds__(NTT2_THREADS, NTT2_MINB) ntt2_pass_kernel(cons
         const u32 w0 = W >= LANES ? q0 + l0 : (l0 & (W - 1)), w1 = W >= LANES ? q0 + l0 + 1 : ((l0 + 1) & (W - 1));
         const u32 c0 = tile * T + t0, c1 = tile * T + t1;
         const bool ok0 = c0 < ncols, ok1 = c1 < ncols;
-        // element (i, col c, word w): STRIDED row C*i + c; CONTIG row c*C + i
-        const u64 istride = MODE == NTT_STRIDED ? ((u64)W << p.logC) : (u64)W;
-        const u64* a0 = MODE == NTT_STRIDED ? in + (size_t)c0 * W + w0 : in + (((size_t)c0 << p.logC) * W + w0);
-        const u64* a1 = MODE == NTT_STRIDED ? in + (size_t)c1 * W + w1 : in + (((size_t)c1 << p.logC) * W + w1);
+        // element (i, col c, word w): STRIDED row C*i + c; CONTIG row c*C + i, or with y_in_out the row it is written back
+        // to, (c + R*i)*mul + b*add of the output geometry
+        const bool yin = MODE == NTT_CONTIG && ymap;
+        const u64 istride = MODE == NTT_STRIDED ? ((u64)W << p.logC) : (yin ? ((u64)p.out_row_mul << p.logR) * p.out_W : (u64)W);
+        const u64* a0 = MODE == NTT_STRIDED ? in + (size_t)c0 * W + w0
+                        : yin ? in + ((size_t)c0 * p.out_row_mul + (size_t)b * p.out_row_add) * p.out_W + p.out_col0 + w0
+                              : in + (((size_t)c0 << p.logC) * W + w0);
+        const u64* a1 = MODE == NTT_STRIDED ? in + (size_t)c1 * W + w1
+                        : yin ? in + ((size_t)c1 * p.out_row_mul + (size_t)b * p.out_row_add) * p.out_W + p.out_col0 + w1
+                              : in + (((size_t)c1 << p.logC) * W + w1);
         const bool vec = p.vec_in;
         constexpr u32 ROWS_PER_IT = NTT2_THREADS / LP;
         constexpr int LDB = 8;
@@ -300,7 +309,11 @@ __global__ void __launch_bounds__(NTT2_THREADS, NTT2_MINB) ntt2_pass_kernel(cons
         const u32 c0 = tile * T + t0, c1 = tile * T + t1;
         const bool ok0 = c0 < ncols, ok1 = c1 < ncols;
         u64 *o0, *o1, jstride;
-        if (MODE == NTT_STRIDED) {  // Y[j][m2] = row j*C + col
+        if (MODE == NTT_STRIDED && ymap) {  // Y[j][m2] -> out row (j + R*col)*mul + b*add, where X[j + R*col] goes
+            o0 = out + (((size_t)c0 << p.logR) * p.out_row_mul + (size_t)b * p.out_row_add) * p.out_W + p.out_col0 + w0;
+            o1 = out + (((size_t)c1 << p.logR) * p.out_row_mul + (size_t)b * p.out_row_add) * p.out_W + p.out_col0 + w1;
+            jstride = (u64)p.out_row_mul * p.out_W;
+        } else if (MODE == NTT_STRIDED) {  // Y[j][m2] = row j*C + col
             o0 = out + (size_t)c0 * W + w0;
             o1 = out + (size_t)c1 * W + w1;
             jstride = (u64)W << p.logC;
@@ -374,7 +387,8 @@ static cudaError_t launch_t(const NttPassParams& p, u32 n_segments, u32 n_batch,
     const u32 T = p.W >= lanes ? 1 : lanes / p.W, chunks = p.W >= lanes ? p.W / lanes : 1;
     const u32 ncols = MODE == NTT_STRIDED ? (1u << p.logC) : (1u << p.logR);
     const size_t smem = smem_bytes_t<LOGS>(p);
-    dim3 grid(((ncols + T - 1) / T) * chunks, n_segments, n_batch);
+    const u32 tiles = ((ncols + T - 1) / T) * chunks;
+    const dim3 grid = p.y_in_out ? dim3(n_batch, tiles, n_segments) : dim3(tiles, n_segments, n_batch);
     cudaError_t e = cudaFuncSetAttribute(ntt2_pass_kernel<MODE, LOGS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     ntt2_pass_kernel<MODE, LOGS><<<grid, NTT2_THREADS, smem, st>>>(p);
