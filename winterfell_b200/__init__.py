@@ -79,6 +79,10 @@ _SIGS = [
                                    u8p, C.POINTER(C.c_size_t)]),
         ("wf_prove_air_aux_dyn", C.c_int, [vp, u64p, C.c_size_t, C.POINTER(u64p), C.c_int, C.c_uint32, C.POINTER(C.c_uint32), AUX_BUILDER, AUX_BUILDER, vp,
                                    u8p, C.POINTER(C.c_size_t)]),
+    ("wf_aux_build_check", C.c_int, [u64p, C.c_size_t, u64p, C.c_size_t, C.c_uint32, C.c_char_p, C.c_size_t]),
+    ("wf_aux_build", C.c_int, [vp, u64p, C.c_size_t, u64p, C.c_size_t, vp, u64p, C.c_uint32, C.POINTER(vp)]),
+    ("wf_prove_air_aux_built", C.c_int, [vp, u64p, C.c_size_t, u64p, C.c_size_t, C.POINTER(u64p), vp, C.c_int, C.c_uint32,
+                                         C.POINTER(C.c_uint32), AUX_BUILDER, vp, u8p, C.POINTER(C.c_size_t)]),
     ("wf_eval_constraints", C.c_int, [vp, u64p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, u64p, u64p, C.POINTER(vp)]),
     ("wf_composition_commit", C.c_int, [vp, C.c_int, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
     ("wf_composition_commit_partitioned", C.c_int, [vp, C.c_int, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(vp),
@@ -376,6 +380,56 @@ class Context:
                                                o_.ctypes.data_as(C.POINTER(C.c_uint32)), f1, f2, None, buf.ctypes.data_as(u8p), C.byref(ln)))
         return buf[: ln.value].tobytes()
 
+    def aux_build(self, desc, build, main_evals, rand, ext):
+        """wf_aux_build: the aux segment of AIR `desc` built on the device from the build description `build`, reading the main
+        trace's evaluations `main_evals` (Mat, n x width) and the random elements rand [num_rands, ext]. Returns a Mat of
+        n x aux_width*ext base columns (component q of aux column j is base column j*ext + q)."""
+        d_, dp = _u64(desc)
+        b_, bp = _u64(build)
+        r_, rp = _u64(np.asarray(rand, dtype=np.uint64).reshape(-1))
+        h = vp()
+        self.check(self.L.wf_aux_build(self.h, dp, d_.size, bp, b_.size, main_evals.h, rp, ext, C.byref(h)))
+        return Mat(self, h)
+
+    def prove_air_aux_built(self, desc, build, trace, opts, n=None, mont=False, values_fn=None, num_rands=0, num_values=0):
+        """wf_prove_air_aux_built: a two-segment proof whose aux segment is built on the device from `build`.
+        trace: [width, n] uint64 host array, or an integer device pointer to column-major [width][n] canonical words (then
+        `n` is required). values_fn(rand [num_rands, d], values [num_values, d]) -> values: optional
+        Air::get_aux_assertions(aux_rand_elements), as in prove_air_aux_dyn. Returns proof bytes."""
+        d_, dp = _u64(desc)
+        b_, bp = _u64(build)
+        o_ = np.ascontiguousarray(opts, dtype=np.uint32)
+        d = int(o_[3])
+        ptrs, dev = None, None
+        if isinstance(trace, int):
+            if n is None:
+                raise ValueError("n is required with a device trace pointer")
+            dev = vp(trace)
+        else:
+            a = np.ascontiguousarray(trace, dtype=np.uint64)
+            c, n = a.shape
+            ptrs = (u64p * c)(*[a[j].ctypes.data_as(u64p) for j in range(c)])
+        cv = AUX_BUILDER()  # NULL: no aux assertion callback
+        if values_fn is not None:
+            def cb_values(_user, rand_p, val_p):
+                try:
+                    rand = np.ctypeslib.as_array(rand_p, shape=(num_rands, d)).copy()
+                    vals = np.ctypeslib.as_array(val_p, shape=(num_values, d))
+                    vals[:] = np.ascontiguousarray(values_fn(rand, vals.copy()), dtype=np.uint64).reshape(num_values, d)
+                    return 0
+                except Exception:  # must not unwind through the C caller
+                    import traceback
+                    traceback.print_exc()
+                    return 1
+            cv = AUX_BUILDER(cb_values)
+        cap = 1 << 23
+        buf = np.zeros(cap, dtype=np.uint8)
+        ln = C.c_size_t(cap)
+        self.check(self.L.wf_prove_air_aux_built(self.h, dp, d_.size, bp, b_.size, ptrs, dev, int(mont), int(n).bit_length() - 1,
+                                                 o_.ctypes.data_as(C.POINTER(C.c_uint32)), cv, None, buf.ctypes.data_as(u8p),
+                                                 C.byref(ln)))
+        return buf[: ln.value].tobytes()
+
     def prove_fib_dev(self, d_trace, k, log_n, results, opts, out_buf=None):
         """trace resident on the device: column-major [2k][n] at raw pointer d_trace."""
         r_, rp = _u64(results)
@@ -606,6 +660,15 @@ def air_check(desc, log_n, blowup):
     d_, dp = _u64(desc)
     msg = C.create_string_buffer(512)
     rc = lib().wf_air_check(dp, d_.size, log_n, blowup, msg, 512)
+    return rc, msg.value.decode(errors="replace")
+
+
+def aux_build_check(desc, build, log_n):
+    """The checks of an aux build description against its AIR (wf_aux_build_check), without a device. Returns (status, reason)."""
+    d_, dp = _u64(desc)
+    b_, bp = _u64(build)
+    msg = C.create_string_buffer(512)
+    rc = lib().wf_aux_build_check(dp, d_.size, bp, b_.size, log_n, msg, 512)
     return rc, msg.value.decode(errors="replace")
 
 

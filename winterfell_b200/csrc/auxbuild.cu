@@ -1,0 +1,352 @@
+// auxbuild.cu — the auxiliary trace segment built on the device from a column-program description (the described
+// alternative to Prover::build_aux_trace, prover/src/lib.rs:236-247; format and semantics at wf_aux_build in
+// include/winterfell_b200.h). Every column is "a per-row term from a straight-line program, then a prefix scan":
+//   aux_term_kernel    interprets the column's program for a run of AUX_TERM_ROWS consecutive rows per thread, registers in a
+//                      local array as in the interpreted generic_constraints_kernel; the run's denominators share one extension
+//                      field inversion (Montgomery's trick). POINTWISE columns are written straight into the aux matrix, the
+//                      running kinds into a term buffer [n][D].
+//   aux_scan_reduce    per tile of AUX_SCAN_TILE rows: the product / sum of its terms;
+//   aux_scan_carry     one block: exclusive scan of the tile aggregates, seeded with the column's init;
+//   aux_scan_apply     per tile: block-wide exclusive scan with the tile's carry-in, written into the aux matrix.
+// Field arithmetic is exact, so the association order of the scan does not change a bit of the result.
+#include "internal.hpp"
+#include "constraints_generic.cuh"  // ld_ext, seg_at, AUX_MAX_REGS
+
+#define AUX_TERM_ROWS 4
+#define AUX_TERM_THREADS 128
+#define AUX_SCAN_THREADS 256
+#define AUX_SCAN_ITEMS 8
+#define AUX_SCAN_TILE (AUX_SCAN_THREADS * AUX_SCAN_ITEMS)
+
+struct AuxTermParams {
+    SegMatrix main;        // n x w evaluations of the main segment
+    SegMatrix aux;         // n x aw*D, columns < col already built
+    u32 w, aw, np, nr, col, log_n;
+    const u32* prog;       // [len][4] op, dst, a, b
+    u32 prog_len;
+    const u64* consts;
+    const u64* ptab;       // periodic columns over the trace domain, concatenated
+    const u32* ptab_off;
+    const u32* ptab_len;   // powers of two
+    const u64* rnd;        // [nr][D]
+    u64* terms;            // [n][D] running kinds; nullptr: POINTWISE, written into aux column `col`
+};
+
+template <int D>
+__device__ __forceinline__ void st_aux(const SegMatrix& m, size_t row, u32 col, const GlExt<D>& v) {
+#pragma unroll
+    for (int q = 0; q < D; q++) {
+        const u32 c = col * D + q;
+        m.base[(size_t)(c / m.W) * m.seg_stride + row * m.W + (c % m.W)] = v.v[q];
+    }
+}
+
+template <int D>
+__global__ void __launch_bounds__(AUX_TERM_THREADS) aux_term_kernel(AuxTermParams p) {
+    const size_t n = (size_t)1 << p.log_n;
+    const size_t row0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * AUX_TERM_ROWS;
+    if (row0 >= n) return;
+    GlExt<D> num[AUX_TERM_ROWS], den[AUX_TERM_ROWS], pre[AUX_TERM_ROWS];
+    bool zero[AUX_TERM_ROWS];
+    GlExt<D> run = ext_from_base<D>(1);
+    GlExt<D> ra[AUX_MAX_REGS];
+    const u32 ab = 2 * p.w, pb = 2 * p.w + 2 * p.aw;
+#pragma unroll
+    for (int r = 0; r < AUX_TERM_ROWS; r++) {
+        const size_t i = row0 + r, nx = (i + 1) & (n - 1);
+        // the registers a program may read (wf_aux_build_check): main rows, aux columns < col, periodic values, random elements
+        for (u32 c = 0; c < p.w; c++) { ra[c] = ext_from_base<D>(seg_at(p.main, i, c)); ra[p.w + c] = ext_from_base<D>(seg_at(p.main, nx, c)); }
+        for (u32 j = 0; j < p.col; j++) {
+#pragma unroll
+            for (int q = 0; q < D; q++) {
+                ra[ab + j].v[q] = seg_at(p.aux, i, j * D + q);
+                ra[ab + p.aw + j].v[q] = seg_at(p.aux, nx, j * D + q);
+            }
+        }
+        for (u32 j = 0; j < p.np; j++) ra[pb + j] = ext_from_base<D>(p.ptab[p.ptab_off[j] + (u32)(i & (p.ptab_len[j] - 1))]);
+        for (u32 j = 0; j < p.nr; j++) ra[pb + p.np + j] = ld_ext<D>(p.rnd + (size_t)j * D);
+        num[r] = ext_zero<D>();
+        den[r] = ext_from_base<D>(1);
+        for (u32 k = 0; k < p.prog_len; k++) {
+            const u32 op = p.prog[4 * k], dst = p.prog[4 * k + 1], a = p.prog[4 * k + 2], b = p.prog[4 * k + 3];
+            switch (op) {
+                case 0: ra[dst] = ext_add(ra[a], ra[b]); break;
+                case 1: ra[dst] = ext_sub(ra[a], ra[b]); break;
+                case 2: ra[dst] = ext_mul(ra[a], ra[b]); break;
+                case 3: ra[dst] = ext_from_base<D>(p.consts[a]); break;
+                default: if (dst == 0) num[r] = ra[a]; else den[r] = ra[a]; break;  // OUT 0 numerator, OUT 1 denominator
+            }
+        }
+        // Montgomery's trick; a zero denominator becomes 1 inside the batch and its term 0 (inv(0) = 0)
+        zero[r] = true;
+#pragma unroll
+        for (int q = 0; q < D; q++) zero[r] = zero[r] && den[r].v[q] == 0;
+        if (zero[r]) den[r] = ext_from_base<D>(1);
+        pre[r] = run;
+        run = ext_mul(run, den[r]);
+    }
+    run = ext_inv(run);
+#pragma unroll
+    for (int r = AUX_TERM_ROWS - 1; r >= 0; r--) {
+        const GlExt<D> inv = ext_mul(run, pre[r]);
+        run = ext_mul(run, den[r]);
+        const GlExt<D> t = zero[r] ? ext_zero<D>() : ext_mul(num[r], inv);
+        const size_t i = row0 + r;
+        if (p.terms) {
+#pragma unroll
+            for (int q = 0; q < D; q++) p.terms[i * D + q] = t.v[q];
+        } else {
+            st_aux<D>(p.aux, i, p.col, t);
+        }
+    }
+}
+
+template <int D, bool MUL>
+__device__ __forceinline__ GlExt<D> scan_op(const GlExt<D>& a, const GlExt<D>& b) { return MUL ? ext_mul(a, b) : ext_add(a, b); }
+template <int D, bool MUL>
+__device__ __forceinline__ GlExt<D> scan_id() { return MUL ? ext_from_base<D>(1) : ext_zero<D>(); }
+template <int D>
+__device__ __forceinline__ GlExt<D> shfl_up_ext(const GlExt<D>& v, u32 off) {
+    GlExt<D> r;
+#pragma unroll
+    for (int q = 0; q < D; q++) r.v[q] = __shfl_up_sync(0xffffffffu, v.v[q], off);
+    return r;
+}
+// exclusive scan of one value per thread over the block (AUX_SCAN_THREADS threads); `total` = the whole block's result
+template <int D, bool MUL>
+__device__ __forceinline__ GlExt<D> block_exclusive_scan(const GlExt<D>& v, GlExt<D>& total) {
+    __shared__ u64 wsum[AUX_SCAN_THREADS / 32][D];
+    const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    constexpr u32 NW = AUX_SCAN_THREADS / 32;
+    GlExt<D> x = v;
+#pragma unroll
+    for (u32 off = 1; off < 32; off <<= 1) {
+        const GlExt<D> y = shfl_up_ext(x, off);
+        if (lane >= off) x = scan_op<D, MUL>(y, x);
+    }
+    if (lane == 31) {
+#pragma unroll
+        for (int q = 0; q < D; q++) wsum[wid][q] = x.v[q];
+    }
+    __syncthreads();
+    if (wid == 0) {
+        GlExt<D> s = lane < NW ? ld_ext<D>(&wsum[lane][0]) : scan_id<D, MUL>();
+#pragma unroll
+        for (u32 off = 1; off < NW; off <<= 1) {
+            const GlExt<D> y = shfl_up_ext(s, off);
+            if (lane >= off) s = scan_op<D, MUL>(y, s);
+        }
+        if (lane < NW) {
+#pragma unroll
+            for (int q = 0; q < D; q++) wsum[lane][q] = s.v[q];
+        }
+    }
+    __syncthreads();
+    total = ld_ext<D>(&wsum[NW - 1][0]);
+    const GlExt<D> wpre = wid ? ld_ext<D>(&wsum[wid - 1][0]) : scan_id<D, MUL>();
+    GlExt<D> ex = shfl_up_ext(x, 1);
+    if (lane == 0) ex = scan_id<D, MUL>();
+    __syncthreads();  // wsum is free for the next call
+    return scan_op<D, MUL>(wpre, ex);
+}
+
+template <int D, bool MUL>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_scan_reduce(const u64* terms, size_t n, u64* agg) {
+    const size_t t0 = (size_t)blockIdx.x * AUX_SCAN_TILE;
+    GlExt<D> v = scan_id<D, MUL>();
+#pragma unroll
+    for (int k = 0; k < AUX_SCAN_ITEMS; k++) {   // coalesced: the order inside a tile does not matter for its aggregate
+        const size_t i = t0 + (size_t)k * AUX_SCAN_THREADS + threadIdx.x;
+        if (i < n) v = scan_op<D, MUL>(v, ld_ext<D>(terms + i * D));
+    }
+    GlExt<D> total;
+    block_exclusive_scan<D, MUL>(v, total);
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int q = 0; q < D; q++) agg[(size_t)blockIdx.x * D + q] = total.v[q];
+    }
+}
+
+// one block; tile aggregates -> exclusive prefixes seeded with init, in place. Thread t owns a run of consecutive tiles.
+template <int D, bool MUL>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_scan_carry(u64* agg, size_t ntiles, GlExt<D> init) {
+    const size_t per = (ntiles + AUX_SCAN_THREADS - 1) / AUX_SCAN_THREADS;
+    const size_t b = threadIdx.x * per, e = b + per < ntiles ? b + per : ntiles;
+    GlExt<D> v = scan_id<D, MUL>();
+    for (size_t i = b; i < e; i++) v = scan_op<D, MUL>(v, ld_ext<D>(agg + i * D));
+    GlExt<D> total;
+    GlExt<D> run = scan_op<D, MUL>(init, block_exclusive_scan<D, MUL>(v, total));
+    for (size_t i = b; i < e; i++) {
+        const GlExt<D> a = ld_ext<D>(agg + i * D);
+#pragma unroll
+        for (int q = 0; q < D; q++) agg[i * D + q] = run.v[q];
+        run = scan_op<D, MUL>(run, a);
+    }
+}
+
+// a[i] = carry(tile) * (terms of the tile's rows before i), written as aux column `col`; thread t owns AUX_SCAN_ITEMS
+// consecutive rows (the second pass re-reads them from L1)
+template <int D, bool MUL>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_scan_apply(const u64* terms, size_t n, const u64* carry, SegMatrix out, u32 col) {
+    const size_t r0 = (size_t)blockIdx.x * AUX_SCAN_TILE + (size_t)threadIdx.x * AUX_SCAN_ITEMS;
+    GlExt<D> v = scan_id<D, MUL>();
+#pragma unroll
+    for (int k = 0; k < AUX_SCAN_ITEMS; k++)
+        if (r0 + k < n) v = scan_op<D, MUL>(v, ld_ext<D>(terms + (r0 + k) * D));
+    GlExt<D> total;
+    GlExt<D> run = scan_op<D, MUL>(ld_ext<D>(carry + (size_t)blockIdx.x * D), block_exclusive_scan<D, MUL>(v, total));
+#pragma unroll
+    for (int k = 0; k < AUX_SCAN_ITEMS; k++) {
+        const size_t i = r0 + k;
+        if (i < n) {
+            st_aux<D>(out, i, col, run);
+            run = scan_op<D, MUL>(run, ld_ext<D>(terms + i * D));
+        }
+    }
+}
+
+// ---- host ---------------------------------------------------------------------------------------------------------------
+// Parses and checks an aux build description against the AIR's shape (w main columns, aw aux columns, np periodic columns,
+// nr random elements). Returns nullptr, or the reason it is rejected.
+const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, u32 nr, AuxBuildHost& b) {
+    size_t p = 0;
+    auto rd = [&](u64& v) { if (p >= len) return false; v = d[p++]; return true; };
+    u64 v, cnt;
+    if (!d || !rd(v)) return "malformed aux build description";
+    if (v != aw) return "aux build width does not match the AIR's aux width";
+    b.aw = aw;
+    if (!rd(cnt) || cnt > len) return "malformed aux build description";
+    for (u64 i = 0; i < cnt; i++) {
+        if (!rd(v)) return "malformed aux build description";
+        if (v >= GL_P) return "aux build constant is not a canonical field element";
+        b.consts.push_back(v);
+    }
+    const u32 ab = 2 * w, pb = 2 * w + 2 * aw, first_tmp = pb + np + nr;
+    for (u32 j = 0; j < aw; j++) {
+        AuxBuildCol c;
+        if (!rd(v)) return "malformed aux build description";
+        if (v > 2) return "unknown aux column kind";
+        c.kind = (u32)v;
+        for (int q = 0; q < 3; q++) {
+            if (!rd(c.init[q])) return "malformed aux build description";
+            if (c.init[q] >= GL_P) return "aux column init is not a canonical field element";
+        }
+        if (!rd(v)) return "malformed aux build description";
+        if (v > AUX_MAX_REGS || v < first_tmp) return "aux build register count out of range";
+        c.num_regs = (u32)v;
+        if (!rd(cnt) || cnt > (1u << 20)) return "malformed aux build description";
+        std::vector<bool> written(c.num_regs, false);
+        for (u32 r = 0; r < first_tmp; r++) written[r] = !(r >= ab && r < pb) || ((r - ab) % aw) < j;
+        u32 outs[2] = {0, 0};
+        for (u64 k = 0; k < cnt; k++) {
+            u64 op, ds, x, y;
+            if (!rd(op) || !rd(ds) || !rd(x) || !rd(y)) return "malformed aux build description";
+            if (op > 4) return "unknown aux build opcode";
+            auto readable = [&](u64 r) { return r < c.num_regs && written[r]; };
+            if (op == 4) {
+                if (ds > 1) return "aux build OUT selects neither numerator (0) nor denominator (1)";
+                if (!readable(x)) return "aux build program reads a register out of range, an aux column >= its own, or an unwritten temporary";
+                outs[ds]++;
+            } else {
+                if (ds >= c.num_regs || ds < first_tmp) return "aux build program writes a register outside its temporaries";
+                if (op == 3) { if (x >= b.consts.size()) return "aux build constant index out of range"; }
+                else if (!readable(x) || !readable(y))
+                    return "aux build program reads a register out of range, an aux column >= its own, or an unwritten temporary";
+                written[ds] = true;
+            }
+            c.prog.insert(c.prog.end(), {(u32)op, (u32)ds, (u32)x, (u32)y});
+        }
+        if (outs[0] != 1) return "aux build column needs exactly one numerator (OUT 0)";
+        if (outs[1] > 1) return "aux build column has more than one denominator (OUT 1)";
+        b.cols.push_back(c);
+    }
+    if (p != len) return "malformed aux build description";
+    return nullptr;
+}
+
+template <int D, bool MUL>
+static int aux_scan(wf_ctx* ctx, const u64* terms, size_t n, u64* agg, const u64* init, SegMatrix out, u32 col) {
+    const size_t ntiles = (n + AUX_SCAN_TILE - 1) / AUX_SCAN_TILE;
+    GlExt<D> in;
+    for (int q = 0; q < D; q++) in.v[q] = init[q];
+    aux_scan_reduce<D, MUL><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(terms, n, agg);
+    aux_scan_carry<D, MUL><<<1, AUX_SCAN_THREADS, 0, ctx->st>>>(agg, ntiles, in);
+    aux_scan_apply<D, MUL><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(terms, n, agg, out, col);
+    ctx->launches += 3;
+    CK(cudaGetLastError());
+    return WF_OK;
+}
+
+template <int D>
+static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u32 w, const std::vector<std::vector<u64>>& periodic,
+                       const u64* rnd, u32 nr, wf_mat** out) {
+    const size_t n = main->m.rows;
+    u32 log_n = 0;
+    while (((size_t)1 << log_n) < n) log_n++;
+    const u32 np = (u32)periodic.size();
+    // one upload: constants | random elements | periodic tables | programs (u32 pairs) -- pageable, staged before return
+    std::vector<u64> up(b.consts);
+    const size_t o_rnd = up.size();
+    up.insert(up.end(), rnd, rnd + (size_t)nr * D);
+    const size_t o_per = up.size();
+    std::vector<u32> poff, plen;
+    for (auto& c : periodic) { poff.push_back((u32)(up.size() - o_per)); plen.push_back((u32)c.size()); up.insert(up.end(), c.begin(), c.end()); }
+    std::vector<u32> u32s(poff);
+    u32s.insert(u32s.end(), plen.begin(), plen.end());
+    std::vector<size_t> prog_off;
+    for (auto& c : b.cols) { prog_off.push_back(u32s.size()); u32s.insert(u32s.end(), c.prog.begin(), c.prog.end()); }
+    if (u32s.size() & 1) u32s.push_back(0);
+    const size_t o_u32 = up.size();
+    for (size_t i = 0; i < u32s.size(); i += 2) up.push_back((u64)u32s[i] | ((u64)u32s[i + 1] << 32));
+    bool running = false;
+    for (auto& c : b.cols) running = running || c.kind != 0;
+    DevScratch tmp(ctx);
+    void *d_up, *d_terms = nullptr, *d_agg = nullptr;
+    CKI(tmp.alloc(std::max(up.size(), (size_t)1) * 8, &d_up));
+    if (running) {
+        CKI(tmp.alloc(n * D * 8, &d_terms));
+        CKI(tmp.alloc((n + AUX_SCAN_TILE - 1) / AUX_SCAN_TILE * D * 8, &d_agg));
+    }
+    CK(cudaMemcpyAsync(d_up, up.data(), up.size() * 8, cudaMemcpyHostToDevice, ctx->st));
+    wf_mat* a;
+    CKI(wf_mat_alloc(ctx, n, b.aw * D, &a));
+    const u64* dev = (const u64*)d_up;
+    const u32* dev32 = (const u32*)(dev + o_u32);
+    AuxTermParams p{};
+    p.main = main->m; p.aux = a->m;
+    p.w = w; p.aw = b.aw; p.np = np; p.nr = nr; p.log_n = log_n;
+    p.consts = dev; p.rnd = dev + o_rnd; p.ptab = dev + o_per; p.ptab_off = dev32; p.ptab_len = dev32 + np;
+    const unsigned grid = (unsigned)((n / AUX_TERM_ROWS + AUX_TERM_THREADS - 1) / AUX_TERM_THREADS);
+    int r = WF_OK;
+    for (u32 j = 0; j < b.aw && r == WF_OK; j++) {
+        const AuxBuildCol& c = b.cols[j];
+        p.col = j;
+        p.prog = dev32 + prog_off[j];
+        p.prog_len = (u32)(c.prog.size() / 4);
+        p.terms = c.kind ? (u64*)d_terms : nullptr;
+        aux_term_kernel<D><<<grid, AUX_TERM_THREADS, 0, ctx->st>>>(p);
+        ctx->launches++;
+        if (cudaGetLastError() != cudaSuccess) { r = wf_fail(ctx, WF_ERR_CUDA, "aux_term_kernel launch failed"); break; }
+        if (c.kind == 1) r = aux_scan<D, true>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
+        else if (c.kind == 2) r = aux_scan<D, false>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
+    }
+    if (r != WF_OK) { wf_mat_free(ctx, a); return r; }
+    *out = a;
+    return WF_OK;
+}
+
+int wf_aux_build_run(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u32 w, const std::vector<std::vector<u64>>& periodic,
+                     const u64* rnd, u32 nr, int D, wf_mat** out) {
+    const size_t n = main->m.rows;
+    if (n < 8 || (n & (n - 1)) || main->m.cols != w) return wf_fail(ctx, WF_ERR_INVALID, "main trace shape does not match the AIR (n x width, n a power of two >= 8)");
+    for (auto& c : periodic) if (c.size() > n) return wf_fail(ctx, WF_ERR_INVALID, "periodic column longer than the trace");
+    for (auto& c : b.cols)
+        for (int q = D; q < 3; q++) if (c.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
+    for (size_t i = 0; i < (size_t)nr * D; i++) if (rnd[i] >= GL_P) return wf_fail(ctx, WF_ERR_INVALID, "random element is not a canonical field element");
+    switch (D) {
+        case 1: return aux_build_d<1>(ctx, b, main, w, periodic, rnd, nr, out);
+        case 2: return aux_build_d<2>(ctx, b, main, w, periodic, rnd, nr, out);
+        case 3: return aux_build_d<3>(ctx, b, main, w, periodic, rnd, nr, out);
+    }
+    return wf_fail(ctx, WF_ERR_INVALID, "field extension %d", D);
+}

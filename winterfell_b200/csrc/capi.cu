@@ -624,7 +624,9 @@ static int mat_transform(wf_ctx* ctx, const wf_mat* in, int inverse, wf_mat** ou
     u32 log_n;
     if (log2_exact(in->m.rows, &log_n) || log_n < 1) return wf_fail(ctx, WF_ERR_INVALID, "rows must be a power of two >= 2");
     wf_mat* o;
-    CKI(wf_mat_alloc(ctx, in->m.rows, in->m.cols, &o));
+    // the passes write the input's segment geometry: the output keeps its segment width (the coefficient matrix of
+    // wf_trace_lde_from_host has the pipeline's chunk width, narrower than wf_mat_alloc's for the same column count)
+    CKI(wf_mat_alloc_w(ctx, in->m.rows, in->m.cols, in->m.W, &o));
     SegMatrix tmp = in->m;
     void* tp = nullptr;
     if (log_n > NTT_MAX_LOGS) {

@@ -113,6 +113,22 @@ int wf_jit_compile(const std::string& src, std::vector<char>& cubin, std::string
 int wf_jit_get_kernel(wf_ctx* ctx, const std::string& src, cudaKernel_t* kernel);
 int wf_dev_alloc(wf_ctx* ctx, size_t bytes, void** out);
 void wf_dev_free(wf_ctx* ctx, void* p);
+// auxbuild.cu: the aux segment built on the device from a column-program description (format at wf_aux_build in the header)
+struct AuxBuildCol {
+    u32 kind = 0;          // 0 POINTWISE, 1 RUNNING_PRODUCT, 2 RUNNING_SUM
+    u64 init[3] = {0, 0, 0};
+    u32 num_regs = 0;
+    std::vector<u32> prog; // 4 words per instruction
+};
+struct AuxBuildHost {
+    u32 aw = 0;
+    std::vector<u64> consts;
+    std::vector<AuxBuildCol> cols;
+};
+const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, u32 nr, AuxBuildHost& out);
+// main: n x w evaluations; rnd: host [nr][D] canonical; *out: n x aw*D in the layout of wf_mat_from_host_columns(..., D)
+int wf_aux_build_run(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u32 w, const std::vector<std::vector<u64>>& periodic,
+                     const u64* rnd, u32 nr, int D, wf_mat** out);
 // Scratch buffers of one call: whatever is still registered when the scope ends (every early error return included) goes back
 // to the context's pool. free() hands one back early, keep() passes ownership on (the buffer outlives the call).
 struct DevScratch {

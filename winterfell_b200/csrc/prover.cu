@@ -1185,7 +1185,7 @@ struct ProofScope {
 template <int D>
 int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont, u32 log_n,
               const Options& o, wf_aux_builder_fn aux_builder, void* aux_user, std::vector<u8>& proof_out,
-              wf_aux_assertions_fn aux_assertions = nullptr) {
+              wf_aux_assertions_fn aux_assertions = nullptr, const AuxBuildHost* aux_build = nullptr) {
     AirHost air_dyn;                       // copy whose aux assertion values are rewritten from the random elements
     if (aux_assertions) air_dyn = air_in;  // (Air::get_aux_assertions(aux_rand_elements), air/src/air/mod.rs:279)
     const AirHost& air = aux_assertions ? air_dyn : air_in;
@@ -1198,7 +1198,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     const u32 aw = air.aw, n_atr = (u32)air.aux_degrees.size(), n_aas = (u32)air.aux_asserts.size();
     const u32 n_mtr = (u32)air.degrees.size(), n_mas = (u32)air.asserts.size();
     const u32 n_tr = n_mtr + n_atr, n_as = n_mas + n_aas;  // context.rs:205-207, :223-225
-    if (aw && !aux_builder) return wf_fail(ctx, WF_ERR_INVALID, "multi-segment AIR needs an aux trace builder");
+    if (aw && !aux_builder && !aux_build) return wf_fail(ctx, WF_ERR_INVALID, "multi-segment AIR needs an aux trace builder");
     if (log_ceb > log_b) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
     for (auto& col : air.periodic) if (col.size() > n) return wf_fail(ctx, WF_ERR_INVALID, "periodic column longer than the trace");
     CKI(validate_degrees(ctx, air.all_degrees(), n));
@@ -1214,12 +1214,12 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     Channel<D> ch(h, seed);
 
     // ---- 1. trace commitment (lib.rs:497-522) ----
-    wf_mat *trace = nullptr, *polys = nullptr, *lde = nullptr, *apolys = nullptr, *alde = nullptr, *comp = nullptr, *cpolys = nullptr,
-           *clde = nullptr, *deep = nullptr;
+    wf_mat *trace = nullptr, *polys = nullptr, *lde = nullptr, *atrace = nullptr, *apolys = nullptr, *alde = nullptr, *comp = nullptr,
+           *cpolys = nullptr, *clde = nullptr, *deep = nullptr;
     wf_tree *ttree = nullptr, *atree = nullptr, *ctree = nullptr;
     wf_fri* fri = nullptr;
     ProofScope scope(ctx);
-    scope.own({&trace, &polys, &lde, &apolys, &alde, &comp, &cpolys, &clde, &deep});
+    scope.own({&trace, &polys, &lde, &atrace, &apolys, &alde, &comp, &cpolys, &clde, &deep});
     scope.own({&ttree, &atree, &ctree});
     scope.fri = &fri;
     wf_mark(ctx, "start");
@@ -1227,7 +1227,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
         CKI(wf_mat_from_device_columns(ctx, d_trace, c, n, &trace));
         wf_mark(ctx, "trace_upload_layout");
         CKI(wf_mat_interpolate(ctx, trace, &polys));
-        scope.drop(trace);
+        if (!aux_build) scope.drop(trace);   // else: the evaluations the aux build reads
         wf_mark(ctx, "trace_interpolate");
         CKI(wf_mat_lde(ctx, polys, log_b, &lde));
     } else {
@@ -1248,8 +1248,18 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
         for (u32 i = 0; i < air.nr; i++) { GlExt<D> e = ch.draw(); for (int q = 0; q < D; q++) rnd_flat.push_back(e.v[q]); }
         std::vector<u64> rnd_user = rnd_flat;
         if (mont) for (u64& v : rnd_user) v = gl_mul(v, 0xFFFFFFFFULL);  // x * R, R = 2^64 mod p
-        std::vector<u64> aux_host((size_t)aw * n * D);  // [aw][n][D]: ColMatrix<E>, one Vec<E> per column
-        if (aux_builder(aux_user, rnd_user.data(), aux_host.data()) != 0) return wf_fail(ctx, WF_ERR_INVALID, "aux trace builder failed");
+        std::vector<u64> aux_host;  // [aw][n][D]: ColMatrix<E>, one Vec<E> per column
+        if (aux_build) {
+            // the described build reads the main trace's evaluations: kept from the device trace, or one forward NTT of the
+            // polynomials for a host trace (its pipelined upload + LDE never materialises the layouted trace)
+            if (!trace) CKI(wf_mat_evaluate(ctx, polys, &trace));
+            CKI(wf_aux_build_run(ctx, *aux_build, trace, c, air.periodic, rnd_flat.data(), air.nr, D, &atrace));
+            scope.drop(trace);
+            wf_mark(ctx, "aux_build");
+        } else {
+            aux_host.resize((size_t)aw * n * D);
+            if (aux_builder(aux_user, rnd_user.data(), aux_host.data()) != 0) return wf_fail(ctx, WF_ERR_INVALID, "aux trace builder failed");
+        }
         if (aux_assertions) {
             size_t total = 0;
             for (auto& a : air_dyn.aux_asserts) total += a.values.size() / 3;
@@ -1269,14 +1279,14 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
                         a.values[i * 3 + k] = v;
                     }
         }
-        // E column j -> D base columns j*D + q (rows of the LDE then serialise exactly like [E] rows)
-        std::vector<const u64*> cols(aw);
-        for (u32 j = 0; j < aw; j++) cols[j] = &aux_host[(size_t)j * n * D];
-        wf_mat* atrace = nullptr;
-        CKI(wf_mat_from_host_columns(ctx, cols.data(), aw, n, D, mont, &atrace));
-        int ir = wf_mat_interpolate(ctx, atrace, &apolys);
-        wf_mat_free(ctx, atrace);
-        if (ir != WF_OK) return ir;
+        if (!aux_build) {
+            // E column j -> D base columns j*D + q (rows of the LDE then serialise exactly like [E] rows)
+            std::vector<const u64*> cols(aw);
+            for (u32 j = 0; j < aw; j++) cols[j] = &aux_host[(size_t)j * n * D];
+            CKI(wf_mat_from_host_columns(ctx, cols.data(), aw, n, D, mont, &atrace));
+        }
+        CKI(wf_mat_interpolate(ctx, atrace, &apolys));
+        scope.drop(atrace);
         CKI(wf_mat_lde(ctx, apolys, log_b, &alde));
         CKI(wf_commit_rows_partitioned(ctx, h, alde, o.part_words(aw, D), &atree));
         CKI(wf_tree_root(ctx, atree, root));
@@ -2023,13 +2033,13 @@ static int parse_options(wf_ctx* ctx, const uint32_t* opts, Options& o) {
 }
 static int prove_dispatch(wf_ctx* ctx, const AirHost& air, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont,
                           uint32_t log_n, const Options& o, uint8_t* proof, size_t* proof_len, wf_aux_builder_fn aux_builder = nullptr,
-                          void* aux_user = nullptr, wf_aux_assertions_fn aux_assertions = nullptr) {
+                          void* aux_user = nullptr, wf_aux_assertions_fn aux_assertions = nullptr, const AuxBuildHost* aux_build = nullptr) {
     std::vector<u8> out;
     int r;
     switch (o.ext) {
-        case 1: r = prove_air<1>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions); break;
-        case 2: r = prove_air<2>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions); break;
-        case 3: r = prove_air<3>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions); break;
+        case 1: r = prove_air<1>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions, aux_build); break;
+        case 2: r = prove_air<2>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions, aux_build); break;
+        case 3: r = prove_air<3>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions, aux_build); break;
         default: return wf_fail(ctx, WF_ERR_UNSUPPORTED, "field extension %u", o.ext);
     }
     if (r != WF_OK) return r;
@@ -2079,6 +2089,55 @@ extern "C" int wf_prove_air_aux_dyn(wf_ctx* ctx, const uint64_t* air_desc, size_
     AirHost air;
     if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
     return prove_dispatch(ctx, air, trace_cols, nullptr, mont, log_n, o, proof, proof_len, aux_builder, aux_user, aux_assertions);
+}
+
+// ---- aux segment from a described build (auxbuild.cu): the device analogue of Prover::build_aux_trace ----
+static int parse_aux_build(wf_ctx* ctx, const AirHost& air, const uint64_t* aux_build, size_t aux_build_len, AuxBuildHost& b) {
+    if (!air.aw) return wf_fail(ctx, WF_ERR_INVALID, "single-segment AIR: it has no aux segment to build");
+    if (const char* why = wf_aux_build_parse(aux_build, aux_build_len, air.w, air.aw, (u32)air.periodic.size(), air.nr, b))
+        return wf_fail(ctx, WF_ERR_INVALID, "%s", why);
+    return WF_OK;
+}
+extern "C" int wf_aux_build_check(const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len,
+                                  uint32_t log_n, char* msg, size_t msg_cap) {
+    auto say = [&](const char* t) { if (msg && msg_cap) { strncpy(msg, t, msg_cap - 1); msg[msg_cap - 1] = 0; } };
+    say("");
+    if (!air_desc || !aux_build || log_n < 3 || log_n > 32) { say("bad arguments"); return WF_ERR_INVALID; }
+    AirHost air;
+    if (!parse_air_host(air_desc, air_desc_len, air)) { say("malformed AIR description"); return WF_ERR_INVALID; }
+    wf_ctx note{};   // carries the message, nothing else
+    AuxBuildHost b;
+    int r = parse_aux_build(&note, air, aux_build, aux_build_len, b);
+    for (auto& col : air.periodic)
+        if (r == WF_OK && col.size() > ((size_t)1 << log_n)) r = wf_fail(&note, WF_ERR_INVALID, "periodic column longer than the trace");
+    say(note.err.c_str());
+    return r;
+}
+extern "C" int wf_aux_build(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len,
+                            const wf_mat* main_evals, const uint64_t* rand, uint32_t ext, wf_mat** aux) {
+    if (!ctx || !air_desc || !aux_build || !main_evals || !aux || ext < 1 || ext > 3) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    AirHost air;
+    if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
+    AuxBuildHost b;
+    CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
+    if (air.nr && !rand) return wf_fail(ctx, WF_ERR_INVALID, "random elements missing");
+    return wf_aux_build_run(ctx, b, main_evals, air.w, air.periodic, rand, air.nr, (int)ext, aux);
+}
+extern "C" int wf_prove_air_aux_built(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build,
+                                      size_t aux_build_len, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont,
+                                      uint32_t log_n, const uint32_t* opts, wf_aux_assertions_fn aux_assertions, void* aux_user,
+                                      uint8_t* proof, size_t* proof_len) {
+    if (!ctx || !air_desc || !aux_build || !opts || !proof || !proof_len || log_n < 3) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    if (!trace_cols == !d_trace) return wf_fail(ctx, WF_ERR_INVALID, "pass exactly one of trace_cols (host) and d_trace (device)");
+    Options o;
+    CKI(parse_options(ctx, opts, o));
+    AirHost air;
+    if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
+    AuxBuildHost b;
+    CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
+    for (auto& col : b.cols)
+        for (u32 q = o.ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
+    return prove_dispatch(ctx, air, trace_cols, d_trace, mont, log_n, o, proof, proof_len, nullptr, aux_user, aux_assertions, &b);
 }
 
 // Compiles the constraint kernel of an AIR description; needs no device (a build-time / CI check of the JIT path and of the
