@@ -336,9 +336,9 @@ typedef struct wf_comm {
  * `results` and `opts` are the full proof's; every rank returns the same proof bytes.
  * stats (optional, 8 doubles): [0] bytes this rank sent through exchanges ordered on the ctx stream, [1] ms inside those,
  * [2] number of collectives, [3] ms inside all_gather_host + all_reduce_sum, [4] FRI layers folded on shards, [5] bytes sent
- * overlapped with compute (the trace LDE's cosets), [6] how those travelled: 2 = written by the last LDE pass itself into the
- * owners' row shards mapped through CUDA IPC (stores over NVLink; the default when the driver allows it and world <= 8),
- * 1 = peer copies (copy engines) into mapped staging buffers, 0 = comm->exchange between fork and join (WF_PEER_PUSH=0). */
+ * overlapped with compute (the trace LDE's cosets), [6] how those travelled: 1 = peer copies (copy engines) into the owners'
+ * staging buffers mapped through CUDA IPC (the default when the driver allows it), 0 = comm->exchange between fork and join
+ * (the driver refused the mapping, or WF_PEER_PUSH=0). */
 int wf_prove_fib_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* const* local_cols, const uint64_t* d_local, int mont,
                          uint32_t k, uint32_t log_n, const uint64_t* results, const uint32_t* opts, uint8_t* proof,
                          size_t* proof_len, double* stats);

@@ -49,10 +49,9 @@ def test_sharded_proof_with_partitions():
     _run(2, 8, 12, 3, hash_id=0 | (2 << 8) | (8 << 16), fri_min_log=6)
 
 
-@pytest.mark.parametrize("env", [{"WF_FUSED_SCATTER": "1"}, {"WF_PEER_PUSH": "0"}])
-def test_sharded_proof_other_transports(env):
-    # the trace exchange has three transports: copy-engine pushes into mapped staging buffers (default, the tests above), the
-    # LDE's last pass storing rows straight into the owners' shards (WF_FUSED_SCATTER=1), and the communicator's exchange
-    # (WF_PEER_PUSH=0: what a multi-node run would use) — same proof bytes
+def test_sharded_proof_communicator_exchange():
+    # the trace exchange has two transports: copy-engine pushes into mapped staging buffers (default, the tests above) and the
+    # communicator's exchange (WF_PEER_PUSH=0: what a multi-node run would use) — same proof bytes
+    env = {"WF_PEER_PUSH": "0"}
     _run(2, 8, 12, 3, fri_min_log=6, extra_env=env)
     _run(4, 16, 13, 1, resident=1, extra_env=env)

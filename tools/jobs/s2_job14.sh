@@ -12,6 +12,5 @@ for l in open('gpurun_out/s2_bench_$name.json'):
 PY
 }
 run g8_push 8 29571 WF_X=0
-run g8_scatter 8 29572 WF_FUSED_SCATTER=1
 run g4_push 4 29573 WF_X=0
 run g8_nccl 8 29574 WF_PEER_PUSH=0

@@ -12,4 +12,3 @@ for l in open('gpurun_out/s2_bench_$name.json'):
 PY
 }
 run g8_push 8 29571 WF_X=0
-run g8_nccl_blocking 8 29574 WF_PEER_PUSH=0 WF_COMM_NO_FORK=1

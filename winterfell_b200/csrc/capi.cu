@@ -288,17 +288,11 @@ static int run_ntt(wf_ctx* ctx, const SegMatrix& in, SegMatrix& out, const SegMa
 // LDE of coefficient columns over 7 * <w_N>: out has n << log_b rows, row b*j + k = P(7 w_N^k w_n^j).
 // `out` may be a view of a wider matrix: segment width out.W >= polys.W, the polys' columns landing at
 // column offset out_col0 of each out row (column-chunked trace pipeline, wf_trace_lde_from_host).
-static int set_scatter(wf_ctx* ctx, NttPassParams& p, const LdeScatter& sc, u32 log_b, u32 coset) {
-    if (p.logS < NTT2_MIN_LOGS || p.W < 2) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "scattered LDE output needs sub-transforms of >= 64 points and W >= 2");
-    p.sc_on = 1; p.sc_log_nj = sc.log_nj; p.sc_log_b = log_b; p.sc_coset = coset; p.sc_seg0 = sc.seg0; p.sc_seg_stride = sc.seg_stride; p.sc_world = sc.world;
-    for (int q = 0; q < 8; q++) p.sc_peer[q] = sc.peer[q];
-    return WF_OK;
-}
 // k0 <= k < k1 (k1 = 0: all cosets) selects the cosets computed; coset k, point j lands in out row j * row_mul + (k - k0) * row_add
 // (row_mul = 0: the natural order b*j + k). Coset-major output (row_mul = 1, row_add = n) is what a rank of a sharded proof
 // produces for the cosets it owns (prover.cu, composition polynomial).
 static int run_lde(wf_ctx* ctx, const SegMatrix& polys, SegMatrix& out, u32 log_n, u32 log_b, u32 out_col0 = 0, u32 k0 = 0, u32 k1 = 0,
-                   u32 row_mul = 0, u32 row_add = 1, const LdeScatter* sc = nullptr) {
+                   u32 row_mul = 0, u32 row_add = 1) {
     u32 logR, logC;
     split_log(log_n, &logR, &logC);
     u32 b = 1u << log_b;
@@ -306,7 +300,6 @@ static int run_lde(wf_ctx* ctx, const SegMatrix& polys, SegMatrix& out, u32 log_
     if (row_mul == 0) { row_mul = b; row_add = 1; }
     LdeTables tabs;
     NttPassParams p;
-    if (sc && logC > NTT_MAX_LOGS) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "scattered LDE output is limited to two-pass sizes");
     if (logC > NTT_MAX_LOGS) {
         // THREE passes per coset (n > 2^22), same structure as run_ntt: pass A carries the coset scaling
         // and the four-step twiddle, the contiguous size-C step is a batch of R two-pass transforms whose
@@ -349,43 +342,26 @@ static int run_lde(wf_ctx* ctx, const SegMatrix& polys, SegMatrix& out, u32 log_
         p.logS = (int)logC; p.logR = 0; p.logC = logC;
         p.pre_tab = tabs.pre + ((size_t)k0 << log_n); p.pre_batch_stride = (size_t)1 << log_n;
         p.out_row_mul = row_mul; p.out_row_add = row_add; p.out_col0 = out_col0;
-        if (sc) CKI(set_scatter(ctx, p, *sc, log_b, k0));
         return launch_pass(ctx, NTT_CONTIG, p, polys.nseg(), k1 - k0);
     }
     // Two passes, one launch each for all cosets [k0, k1) (batch z = coset k0 + z): Y_k is written into the rows of `out` that
-    // X_k will occupy and pass 2 transforms it in place, so the polynomials are read once and no scratch is needed. A
-    // scattered output is not written locally: there Y goes to a scratch as large as the polynomials, one coset at a time.
-    SegMatrix y = polys;
-    void* yp = nullptr;
-    if (sc) {
-        CKI(wf_dev_alloc(ctx, polys.words() * 8, &yp));
-        y.base = (u64*)yp;
-    }
-    const u32 kb = sc ? 1 : k1 - k0;
-    int rc = WF_OK;
-    for (u32 k = k0; k < k1 && rc == WF_OK; k += kb) {
-        // pass 1: Y_k[j1][m2] = 7^m2 w_N^((b j1 + k) m2) sum_m1 a[C m1 + m2] (s_k^C)^m1 w_R^(j1 m1)
-        pass_defaults(p, polys, sc ? y : out);
-        p.logS = (int)logR; p.logR = logR; p.logC = logC;
-        p.pre_tab = tabs.pre + ((size_t)k << logR); p.pre_batch_stride = (size_t)1 << logR;
-        // exponent (b*j1 + k)*m2 = (j1*a_mul + (batch0 + z)*b_mul)*m2
-        p.has_post = 1; p.logM = log_n + log_b; p.a_mul = b; p.b_mul = 1; p.batch0 = k;
-        p.ctab = tabs.pow7;
-        if (!sc) { p.y_in_out = 1; p.out_row_mul = row_mul; p.out_row_add = row_add; p.out_col0 = out_col0; }
-        rc = launch_pass(ctx, NTT_STRIDED, p, polys.nseg(), kb);
-        if (rc != WF_OK) break;
-        // pass 2: X_k[j1 + R j2] = sum_m2 Y_k[j1][m2] w_C^(j2 m2)  -> row b*(j1 + R j2) + k
-        pass_defaults(p, polys, out);
-        p.in = sc ? y.base : out.base;
-        p.in_seg_stride = sc ? y.seg_stride : out.seg_stride;
-        p.logS = (int)logC; p.logR = logR; p.logC = logC;
-        p.out_row_mul = row_mul; p.out_row_add = row_add; p.out_col0 = out_col0;
-        if (sc) { rc = set_scatter(ctx, p, *sc, log_b, k); if (rc != WF_OK) break; }
-        else p.y_in_out = 1;
-        rc = launch_pass(ctx, NTT_CONTIG, p, polys.nseg(), kb);
-    }
-    wf_dev_free(ctx, yp);
-    return rc;
+    // X_k will occupy and pass 2 transforms it in place, so the polynomials are read once and no scratch is needed.
+    // pass 1: Y_k[j1][m2] = 7^m2 w_N^((b j1 + k) m2) sum_m1 a[C m1 + m2] (s_k^C)^m1 w_R^(j1 m1)
+    pass_defaults(p, polys, out);
+    p.logS = (int)logR; p.logR = logR; p.logC = logC;
+    p.pre_tab = tabs.pre + ((size_t)k0 << logR); p.pre_batch_stride = (size_t)1 << logR;
+    // exponent (b*j1 + k)*m2 = (j1*a_mul + (batch0 + z)*b_mul)*m2
+    p.has_post = 1; p.logM = log_n + log_b; p.a_mul = b; p.b_mul = 1; p.batch0 = k0;
+    p.ctab = tabs.pow7;
+    p.y_in_out = 1; p.out_row_mul = row_mul; p.out_row_add = row_add; p.out_col0 = out_col0;
+    CKI(launch_pass(ctx, NTT_STRIDED, p, polys.nseg(), k1 - k0));
+    // pass 2: X_k[j1 + R j2] = sum_m2 Y_k[j1][m2] w_C^(j2 m2)  -> row b*(j1 + R j2) + k
+    pass_defaults(p, polys, out);
+    p.in = out.base;
+    p.in_seg_stride = out.seg_stride;
+    p.logS = (int)logC; p.logR = logR; p.logC = logC;
+    p.y_in_out = 1; p.out_row_mul = row_mul; p.out_row_add = row_add; p.out_col0 = out_col0;
+    return launch_pass(ctx, NTT_CONTIG, p, polys.nseg(), k1 - k0);
 }
 
 // =================================================================================================
@@ -684,7 +660,7 @@ int wf_mat_lde_cosets(wf_ctx* ctx, const wf_mat* polys, uint32_t log_blowup, uin
 // compute stream. Columns are independent, so the result equals from_host_columns -> interpolate -> lde.
 int wf_trace_lde_from_host(wf_ctx* ctx, const uint64_t* const* cols, uint32_t ncols, size_t nrows, int mont, uint32_t log_blowup,
                            wf_mat** polys_out, wf_mat** lde_out) {
-    return wf_trace_lde_cosetwise(ctx, cols, nullptr, ncols, nrows, mont, log_blowup, polys_out, lde_out, false, nullptr, nullptr);
+    return wf_trace_lde_cosetwise(ctx, cols, nullptr, ncols, nrows, mont, log_blowup, polys_out, lde_out, false, nullptr);
 }
 // The same pipeline with two knobs for the sharded prover (prover.cu): coset_major = the LDE is written coset-major
 // (row k * n + j = P(7 w_N^k w_n^j); *lde_out must then be preallocated with the natural segment width) and after_coset(k)
@@ -692,23 +668,18 @@ int wf_trace_lde_from_host(wf_ctx* ctx, const uint64_t* const* cols, uint32_t nc
 // d_cols != NULL: the columns are already on the device (column-major), no upload stage.
 int wf_trace_lde_cosetwise(wf_ctx* ctx, const uint64_t* const* cols, const uint64_t* d_cols, uint32_t ncols, size_t nrows, int mont,
                            uint32_t log_blowup, wf_mat** polys_out, wf_mat** lde_out, bool coset_major,
-                           const std::function<int(u32)>* after_coset, const LdeScatter* scatter) {
-    if (!ctx || (!cols && !d_cols) || !polys_out || (!lde_out && !scatter) || ncols == 0) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+                           const std::function<int(u32)>* after_coset) {
+    if (!ctx || (!cols && !d_cols) || !polys_out || !lde_out || ncols == 0) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     u32 log_n;
     if (log2_exact(nrows, &log_n) || log_n < 1) return wf_fail(ctx, WF_ERR_INVALID, "rows must be a power of two >= 2");
     if (log_blowup > 7 || log_n + log_blowup > 32) return wf_fail(ctx, WF_ERR_INVALID, "bad blowup");
     const int Wout = seg_width_for(ncols);
     const u32 nseg_out = (ncols + Wout - 1) / Wout;
     const u32 nb = 1u << log_blowup;
-    if (coset_major && !scatter && (!*lde_out || (*lde_out)->m.rows != (nrows << log_blowup) || (*lde_out)->m.W != Wout || (*lde_out)->m.cols != ncols))
+    if (coset_major && (!*lde_out || (*lde_out)->m.rows != (nrows << log_blowup) || (*lde_out)->m.W != Wout || (*lde_out)->m.cols != ncols))
         return wf_fail(ctx, WF_ERR_INVALID, "coset-major output must be preallocated");
     // cosets of one column chunk: all at once, or one by one with the callback when this is the last chunk
-    auto extend = [&](const SegMatrix& pv, SegMatrix& ov, u32 out_col0, bool last, u32 out_seg) -> int {
-        if (scatter) {  // every coset straight into the owners' row shards (natural order there); `ov` is not written
-            LdeScatter s2 = *scatter;
-            s2.seg0 += out_seg;
-            return run_lde(ctx, pv, ov, log_n, log_blowup, out_col0, 0, nb, 0, 1, &s2);
-        }
+    auto extend = [&](const SegMatrix& pv, SegMatrix& ov, u32 out_col0, bool last) -> int {
         if (!after_coset || !last) {
             if (!coset_major) return run_lde(ctx, pv, ov, log_n, log_blowup, out_col0);
             return run_lde(ctx, pv, ov, log_n, log_blowup, out_col0, 0, nb, 1, (u32)nrows);
@@ -732,10 +703,9 @@ int wf_trace_lde_cosetwise(wf_ctx* ctx, const uint64_t* const* cols, const uint6
         int r = wf_mat_interpolate(ctx, tr, polys_out);
         wf_mat_free(ctx, tr);
         if (r != WF_OK) return r;
-        if (scatter) { SegMatrix none = (*polys_out)->m; none.W = Wout; return extend((*polys_out)->m, none, 0, true, 0); }
         if (!coset_major && !after_coset) return wf_mat_lde(ctx, *polys_out, log_blowup, lde_out);
         if (!coset_major) CKI(wf_mat_alloc(ctx, nrows << log_blowup, ncols, lde_out));
-        return extend((*polys_out)->m, (*lde_out)->m, 0, true, 0);
+        return extend((*polys_out)->m, (*lde_out)->m, 0, true);
     }
     if (!ctx->copy_st) {
         CK(cudaStreamCreateWithFlags(&ctx->copy_st, cudaStreamNonBlocking));
@@ -753,16 +723,16 @@ int wf_trace_lde_cosetwise(wf_ctx* ctx, const uint64_t* const* cols, const uint6
         wf_mat_free(ctx, tr);
         for (int i = 0; i < 2; i++) wf_dev_free(ctx, stage[i]);
         wf_dev_free(ctx, tmp);
-        if (results_too) { wf_mat_free(ctx, polys); if (!coset_major && !scatter) wf_mat_free(ctx, lde); }
+        if (results_too) { wf_mat_free(ctx, polys); if (!coset_major) wf_mat_free(ctx, lde); }
     };
     auto body = [&]() -> int {
         CKI(wf_mat_alloc_w(ctx, nrows, ncols, Wc, &polys));
-        if (coset_major || scatter) lde = lde_out ? *lde_out : nullptr;
+        if (coset_major) lde = *lde_out;
         else CKI(wf_mat_alloc(ctx, nrows << log_blowup, ncols, &lde));
         CKI(wf_mat_alloc_w(ctx, nrows, Wc, Wc, &tr));                       // one chunk of trace values (reused)
         for (int i = 0; i < 2; i++) CKI(wf_dev_alloc(ctx, (size_t)Wc * nrows * 8, &stage[i]));
         CKI(wf_dev_alloc(ctx, (size_t)Wc * nrows * 8, &tmp));               // two-pass scratch
-        if (lde && lde->m.W > (int)ncols) CK(cudaMemsetAsync(lde->m.base, 0, lde->m.words() * 8, ctx->st));  // padding columns
+        if (lde->m.W > (int)ncols) CK(cudaMemsetAsync(lde->m.base, 0, lde->m.words() * 8, ctx->st));  // padding columns
         // the copy stream must not write pool buffers before their previous users on the compute stream are done
         CK(cudaEventRecord(ctx->ev_start, ctx->st));
         CK(cudaStreamWaitEvent(ctx->copy_st, ctx->ev_start, 0));
@@ -785,11 +755,10 @@ int wf_trace_lde_cosetwise(wf_ctx* ctx, const uint64_t* const* cols, const uint6
             SegMatrix tv = trv;
             tv.base = (u64*)tmp;
             CKI(run_ntt(ctx, trv, pv, &tv, log_n, 1));
-            SegMatrix ov = pv;                                                // out segment holding columns c0..
-            ov.W = Wout;
-            if (lde) { ov = lde->m; ov.base = lde->m.base + (size_t)(c0 / Wout) * lde->m.seg_stride; }
+            SegMatrix ov = lde->m;                                            // out segment holding columns c0..
+            ov.base = lde->m.base + (size_t)(c0 / Wout) * lde->m.seg_stride;
             ov.cols = cw;
-            CKI(extend(pv, ov, c0 % Wout, k + 1 == nchunks, c0 / Wout));
+            CKI(extend(pv, ov, c0 % Wout, k + 1 == nchunks));
         }
         return WF_OK;
     };
@@ -801,7 +770,7 @@ int wf_trace_lde_cosetwise(wf_ctx* ctx, const uint64_t* const* cols, const uint6
     }
     release(false);
     *polys_out = polys;
-    if (lde_out) *lde_out = lde;
+    *lde_out = lde;
     return WF_OK;
 }
 

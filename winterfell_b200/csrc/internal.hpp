@@ -149,17 +149,9 @@ struct DevScratch {
 };
 int wf_mat_alloc(wf_ctx* ctx, size_t rows, u32 cols, wf_mat** out);
 int wf_mat_alloc_w(wf_ctx* ctx, size_t rows, u32 cols, int W, wf_mat** out);
-// LDE output scattered into the row shards of the ranks of a sharded proof (NttPassParams::sc_*, ntt.cuh)
-struct LdeScatter {
-    u64* peer[8];        // shard base per rank (peer memory mapped through CUDA IPC; own rank: the local shard)
-    size_t seg_stride;   // words between segments of a shard
-    u32 seg0;            // global segment the first local segment maps to
-    u32 log_nj;          // log2(points of one coset per rank)
-    u32 world;           // > 0: also write the halo rows of the previous rank (NttPassParams::sc_world)
-};
 extern "C" int wf_trace_lde_cosetwise(wf_ctx* ctx, const uint64_t* const* cols, const uint64_t* d_cols, uint32_t ncols, size_t nrows, int mont,
                            uint32_t log_blowup, wf_mat** polys_out, wf_mat** lde_out, bool coset_major,
-                           const std::function<int(u32)>* after_coset, const LdeScatter* scatter);
+                           const std::function<int(u32)>* after_coset);
 extern "C" int wf_mat_lde_cosets(wf_ctx* ctx, const wf_mat* polys, uint32_t log_blowup, uint32_t k0, uint32_t k1, wf_mat* lde);  // internal (not in the public header)
 struct PublicCoin;
 struct Digest;

@@ -77,16 +77,6 @@ struct NttPassParams {
     const u64 *tw_hi, *tw_lo;
     u32 tw_split;
     int vec_in, vec_out;                       // lane pairs are contiguous (16-byte aligned) in the input / output
-    // CONTIG output scattered over the ranks of a sharded proof (peer memory mapped through CUDA IPC, prover.cu): point
-    // jj = col + R * j of coset (sc_coset + batch) goes to rank jj >> sc_log_nj, row ((jj mod 2^sc_log_nj) << sc_log_b) + coset
-    // of that rank's row shard — natural order there, written straight from the tile by stores over NVLink: the exchange IS
-    // the write-back of the last LDE pass (no staging buffer, no copy, no interleaving pass). ntt2 kernels, lane pairs only.
-    int sc_on;
-    u32 sc_log_nj, sc_log_b, sc_coset, sc_seg0;
-    u32 sc_world;                              // > 0: the first point of every rank's range is also stored into the halo rows
-                                               // (rows 2^(sc_log_nj + sc_log_b) ..) of the PREVIOUS rank: its next-state frame wraps there
-    size_t sc_seg_stride;                      // words between segments of a shard
-    u64* sc_peer[8];                           // shard base per rank (own rank: the local shard)
     const u64* ctab;                           // optional per-column constant table
     u64 cconst;                                // constant factor (e.g. 1/n) folded into the post twiddle, or applied
                                                // alone at write-back when has_post == 0; 1 if unused

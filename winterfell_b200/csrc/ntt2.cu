@@ -325,24 +325,11 @@ __global__ void __launch_bounds__(NTT2_THREADS, NTT2_MINB) ntt2_pass_kernel(cons
         const bool post = p.has_post, scale = !p.has_post && p.cconst != 1, vec = p.vec_out;
         const u32 inv_mask = p.inverse ? (S - 1) : 0;  // jf = inverse ? (S - j) mod S : j
         constexpr u32 ROWS_PER_IT = NTT2_THREADS / LP;
-        const bool scatter = MODE == NTT_CONTIG && p.sc_on;
-        const u32 sc_k = p.sc_coset + b, sc_mask = (1u << p.sc_log_nj) - 1;
-        const size_t sc_off = (size_t)(p.sc_seg0 + g) * p.sc_seg_stride + p.out_col0 + w0;
 #pragma unroll 4
         for (u32 j = tid / LP; j < S; j += ROWS_PER_IT) {
             const u32 jf = inv_mask ? ((S - j) & inv_mask) : j;
             const u32 r = __brev(jf) >> (32 - LOGS);
             ulonglong2 v = *reinterpret_cast<const ulonglong2*>(s + prow<LK>(r) * LANES + l0);
-            if (scatter) {  // no post factor on this path (CONTIG passes of the LDE carry none)
-                const u32 jj = c0 + (j << p.logR);
-                u64* dst = p.sc_peer[jj >> p.sc_log_nj] + sc_off + (((size_t)(jj & sc_mask) << p.sc_log_b) + sc_k) * p.out_W;
-                if (ok0) *reinterpret_cast<ulonglong2*>(dst) = v;
-                if (p.sc_world && (jj & sc_mask) == 0 && ok0) {   // halo copy for the rank before the owner
-                    const u32 q = jj >> p.sc_log_nj, qp = q ? q - 1 : p.sc_world - 1;
-                    *reinterpret_cast<ulonglong2*>(p.sc_peer[qp] + sc_off + ((((size_t)sc_mask + 1) << p.sc_log_b) + sc_k) * p.out_W) = v;
-                }
-                continue;
-            }
             if (post) {
                 const u64 f0 = ctw[j * T + t0];
                 v.x = gl_mul(v.x, f0);

@@ -1597,31 +1597,6 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     CKI(wf_mat_alloc(ctx, rows_per + b, c, &shard));
     shard->m.rows = rows_per;  // seg_stride stays (rows_per + b) * 8: rows [rows_per, rows_per + b) are the halo
     const size_t sstride = shard->m.seg_stride;
-    // Transport 1 — the exchange fused into the LDE: every rank maps the others' row shards (CUDA IPC) and the last
-    // pass of every coset's transform writes each row straight to its owner (and the first rows of a range also into the halo
-    // of the rank before it) with stores over NVLink: natural order at the destination, no staging buffer, no copy kernel,
-    // no interleaving pass, nothing left to overlap. Closed by one stream synchronisation + host barrier.
-    std::vector<void*> peer_shard;
-    u32 log_nj = 0;
-    while (((size_t)1 << log_nj) < nj) log_nj++;
-    // (measured at 2 GPUs, cfg3: the remote 64-byte stores stall the pass by about what the transfer costs — 37.4 ms LDE + 0.6 ms
-    // exposed against 30.3 + 5.6 with copy-engine pushes and 28.1 + 8.1 with a blocking NCCL all-to-all — so the fused form is
-    // opt-in, WF_FUSED_SCATTER=1, and the copy-engine push below is the default)
-    const char* fused_env = getenv("WF_FUSED_SCATTER");
-    const bool scat = fused_env && atoi(fused_env) != 0 && G <= 8 && log_n <= 22 && sc.map_peers(shard->m.base, peer_shard) == WF_OK;
-    bool push = false;
-    if (scat) {
-        LdeScatter sct;
-        for (int q = 0; q < 8; q++) sct.peer[q] = q < G ? (u64*)peer_shard[q] : nullptr;
-        sct.seg_stride = sstride; sct.seg0 = (u32)r * nsl; sct.log_nj = log_nj; sct.world = (u32)G;
-        CKI(wf_trace_lde_cosetwise(ctx, local_cols, d_local, cl, n, mont, log_b, &polys, nullptr, false, nullptr, &sct));
-        wf_mark(ctx, "trace_lde");
-        CK(cudaStreamSynchronize(ctx->st));   // my stores have landed; everybody's have when every rank says so
-        CKI(sc.host_barrier());
-        sc.ncoll += 1;
-        sc.bytes_overlapped += (double)(G - 1) * nsl * (double)rows_per * 64;
-        push = true;
-    } else {
     wf_mat*& stage = tstage;           // what arrives: [global segment][coset][nj][8]
     CKI(wf_mat_alloc_w(ctx, N, cl, 8, &lde));          // mine, coset-major: [local segment][coset][n][8]
     CKI(wf_mat_alloc_w(ctx, rows_per, c, 8, &stage));
@@ -1629,7 +1604,7 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     // on side streams — copy engines over NVLink, no SM taken from the NTT kernels they overlap (NCCL send/recv kernels on a
     // side stream were measured: they slow the LDE down by as much as they hide). Fallback: the communicator's exchange.
     std::vector<void*> peer_stage;
-    push = sc.map_peers(stage->m.base, peer_stage) == WF_OK;
+    const bool push = sc.map_peers(stage->m.base, peer_stage) == WF_OK;
     if (push) {
         for (int i = 0; i < 4; i++) if (!ctx->push_st[i]) CK(cudaStreamCreateWithFlags(&ctx->push_st[i], cudaStreamNonBlocking));
         for (int i = 0; i < 16; i++) if (!ctx->push_ev[i]) CK(cudaEventCreateWithFlags(&ctx->push_ev[i], cudaEventDisableTiming));
@@ -1671,7 +1646,7 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     };
     // (upload ->) layout -> interpolate -> extend, pipelined per column chunk for host columns; the cosets of the last chunk
     // are extended one by one and after_coset(k) ships coset k while coset k + 1 is computed
-    CKI(wf_trace_lde_cosetwise(ctx, local_cols, d_local, cl, n, mont, log_b, &polys, &lde, true, &after_coset, nullptr));
+    CKI(wf_trace_lde_cosetwise(ctx, local_cols, d_local, cl, n, mont, log_b, &polys, &lde, true, &after_coset));
     wf_mark(ctx, "trace_lde");
     if (push) {
         // my pushes have landed when my side streams drain; everybody's have when every rank says so
@@ -1700,7 +1675,6 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
         CK(cudaMemcpy2DAsync(shard->m.base + rows_per * 8, sstride * 8, pk2, hb, hb, nsg, cudaMemcpyDeviceToDevice, ctx->st));
         wf_dev_free(ctx, pk);
         wf_dev_free(ctx, pk2);
-    }
     }
     wf_mark(ctx, "trace_exchange");
     // ---- 3. leaves + subtree over my rows, all-gather of the subtree roots ----
@@ -2001,7 +1975,7 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
         for (int i = 4; i < 8; i++) stats[i] = 0;
         stats[4] = (double)slayers.size();
         stats[5] = sc.bytes_overlapped;
-        stats[6] = scat ? 2.0 : (push ? 1.0 : 0.0);
+        stats[6] = push ? 1.0 : 0.0;
     }
     return WF_OK;
 }

@@ -18,8 +18,6 @@ prover/src/trace/trace_lde/default/mod.rs:63, :245-282):
 This module contains no arithmetic: local compute goes through a backend (the CUDA context in the
 product; the tests substitute a CPU backend), collectives through torch.distributed.
 """
-import os
-
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -173,10 +171,8 @@ class TorchComm:
         self.side = torch.cuda.Stream(device=self.device) if self.nccl else None   # exchanges overlapped with compute (fork / join)
         self._forked = False
         # gloo (host-staged test double): no overlap, the callbacks stay NULL and every exchange is ordered on the ctx stream
-        # WF_COMM_NO_FORK=1: NCCL exchanges stay on the context stream (blocking in stream order; the measured alternative)
-        overlap = self.nccl and os.environ.get("WF_COMM_NO_FORK", "0") in ("", "0")
-        fork = _FORK_FN(self._fork) if overlap else _FORK_FN()
-        join = _FORK_FN(self._join) if overlap else _FORK_FN()
+        fork = _FORK_FN(self._fork) if self.nccl else _FORK_FN()
+        join = _FORK_FN(self._join) if self.nccl else _FORK_FN()
         self._keep = (_EXCHANGE_FN(self._exchange), _GATHER_FN(self._gather), _REDUCE_FN(self._reduce), fork, join)
         self.struct = WfComm(None, self.rank, self.world, *self._keep)
 
@@ -386,11 +382,7 @@ def bench_sharded(ctx, stream, cfg, steps, warmup, configs, proof_opts, flush, c
             "wall_ms": wall, "clocks": sampler.summary(),
             "parallelism": f"one proof sharded over {world} GPUs: column-sharded interpolate + LDE, exchange into row shards, row-sharded "
                            "commitments / constraints / DEEP / first FRI layers, subtree-root all-gathers (winterfell_b200/dist.py)",
-            "comm": {"limiting_collective": ("column shards -> row shards of the trace LDE fused into the LDE: the last pass of every coset's transform stores each "
-                                             "row (and the halo rows) straight into its owner's shard, peer memory mapped through CUDA IPC, over NVLink; closed "
-                                             "by one host barrier; no NCCL call on the data path"
-                                             if res_stats.get("peer_push") == 2 else
-                                             "column shards -> row shards of the trace LDE, per coset, as peer copies (copy engines over NVLink) into the other "
+            "comm": {"limiting_collective": ("column shards -> row shards of the trace LDE, per coset, as peer copies (copy engines over NVLink) into the other "
                                              "ranks' buffers mapped through CUDA IPC, overlapped with the extension of the next coset; closed by one host barrier"
                                              if res_stats.get("peer_push") else
                                              "exchange (NCCL send/recv all-to-all: column shards -> row shards of the trace LDE), issued per coset on the "
