@@ -92,11 +92,25 @@ __device__ __forceinline__ void bulk_wait(u64* mbar) {
         asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(mb) : "memory");
 }
 
+// ---- cp.async tile loads (global -> shared, no register staging) ---------------------------------------
+// src_size 0 fills the destination with zeros without reading `gsrc`, which must still be a valid address
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc, bool ok) {
+    const u32 dst = (u32)__cvta_generic_to_shared(smem_dst);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(gsrc), "r"(ok ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc, bool ok) {
+    const u32 dst = (u32)__cvta_generic_to_shared(smem_dst);
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(dst), "l"(gsrc), "r"(ok ? 8 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+
 // ---- one round ----------------------------------------------------------------------------------------
 // Round K of the plan on the tile `s` (S rows x LANES words, swizzled rows). tw: this round's table
-// [span][2^R] (null for the last round). Each task = 16 values.
+// [span][2^R] (null for the last round). pre: null, or the input scale pre[row] applied as the round reads the tile
+// (round 0 only). Each task = 16 values.
 template <int LOGS, int K>
-__device__ __forceinline__ void tile_round(u64* __restrict__ s, const u64* __restrict__ tw, int tid) {
+__device__ __forceinline__ void tile_round(u64* __restrict__ s, const u64* __restrict__ tw, const u64* __restrict__ pre, int tid) {
     constexpr int LANES = Plan<LOGS>::lanes, LK = LANES == 8 ? 1 : 2;
     constexpr int R = plan_radix<LOGS>(K), ST = plan_stage<LOGS>(K);
     constexpr int LOGSPAN = LOGS - ST - R;
@@ -114,6 +128,10 @@ __device__ __forceinline__ void tile_round(u64* __restrict__ s, const u64* __res
             for (int q = 0; q < 16; q++) {
                 const u32 row = (base + ((u32)q << LOGSPAN)) ^ (hb ^ swz_const<LK>((u32)q << LOGSPAN));
                 x[q] = s[row * LANES + lane];
+            }
+            if (K == 0 && pre) {
+#pragma unroll
+                for (int q = 0; q < 16; q++) x[q] = gl_mul(x[q], __ldg(pre + base + ((u32)q << LOGSPAN)));
             }
             mini_dft<4>(x);
             if (!LAST) {
@@ -145,6 +163,14 @@ __device__ __forceinline__ void tile_round(u64* __restrict__ s, const u64* __res
                 const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(s + row * LANES + 2 * lp);
                 xa[q] = v.x;
                 xb[q] = v.y;
+            }
+            if (K == 0 && pre) {
+#pragma unroll
+                for (int q = 0; q < 8; q++) {
+                    const u64 f = __ldg(pre + base + ((u32)q << LOGSPAN));
+                    xa[q] = gl_mul(xa[q], f);
+                    xb[q] = gl_mul(xb[q], f);
+                }
             }
             mini_dft<3>(xa);
             mini_dft<3>(xb);
@@ -192,6 +218,45 @@ __global__ void __launch_bounds__(NTT2_THREADS, NTT2_MINB) ntt2_pass_kernel(cons
     const u32 R = 1u << p.logR, C = 1u << p.logC;
     const u32 ncols = MODE == NTT_STRIDED ? C : R;
 
+    // ---- load, issued first: thread -> (row i, lane pair), every 16-byte (W = 1: 8-byte) piece of the tile in flight at once
+    // as a cp.async copy, so that the post twiddles below are computed while the tile arrives. The coset pre-scale is applied
+    // by round 0 as it first reads each element.
+    {
+        const u64* in = p.in + (size_t)g * p.in_seg_stride + (size_t)b * p.in_batch_stride;
+        const u32 lp = tid % LP;
+        const u32 l0 = 2 * lp;                                     // first lane of the pair
+        const u32 t0 = W >= LANES ? 0 : (l0 >> logW), t1 = W >= LANES ? 0 : ((l0 + 1) >> logW);
+        const u32 w0 = W >= LANES ? q0 + l0 : (l0 & (W - 1)), w1 = W >= LANES ? q0 + l0 + 1 : ((l0 + 1) & (W - 1));
+        const u32 c0 = tile * T + t0, c1 = tile * T + t1;
+        const bool ok0 = c0 < ncols, ok1 = c1 < ncols;
+        // element (i, col c, word w): STRIDED row C*i + c; CONTIG row c*C + i, or with y_in_out the row it is written back
+        // to, (c + R*i)*mul + b*add of the output geometry. A lane past the last column is zero-filled from a valid address.
+        const bool yin = MODE == NTT_CONTIG && ymap;
+        const u64 istride = MODE == NTT_STRIDED ? ((u64)W << p.logC) : (yin ? ((u64)p.out_row_mul << p.logR) * p.out_W : (u64)W);
+        const u64* a0 = MODE == NTT_STRIDED ? in + (size_t)c0 * W + w0
+                        : yin ? in + ((size_t)c0 * p.out_row_mul + (size_t)b * p.out_row_add) * p.out_W + p.out_col0 + w0
+                              : in + (((size_t)c0 << p.logC) * W + w0);
+        const u64* a1 = MODE == NTT_STRIDED ? in + (size_t)c1 * W + w1
+                        : yin ? in + ((size_t)c1 * p.out_row_mul + (size_t)b * p.out_row_add) * p.out_W + p.out_col0 + w1
+                              : in + (((size_t)c1 << p.logC) * W + w1);
+        if (!ok0) a0 = p.in;
+        if (!ok1) a1 = p.in;
+        const u64 s0 = ok0 ? istride : 0, s1 = ok1 ? istride : 0;
+        const bool vec = p.vec_in;
+        constexpr u32 ROWS_PER_IT = NTT2_THREADS / LP;
+#pragma unroll 4
+        for (u32 i = tid / LP; i < S; i += ROWS_PER_IT) {
+            u64* dst = s + prow<LK>(i) * LANES + l0;
+            if (vec) {
+                cp_async16(dst, a0 + i * s0, ok0);
+            } else {
+                cp_async8(dst, a0 + i * s0, ok0);
+                cp_async8(dst + 1, a1 + i * s1, ok1);
+            }
+        }
+        cp_async_commit();
+    }
+
     // round twiddles: one TMA bulk copy
     bulk_init(mbar, tid);
     __syncthreads();
@@ -235,68 +300,19 @@ __global__ void __launch_bounds__(NTT2_THREADS, NTT2_MINB) ntt2_pass_kernel(cons
         }
     }
 
-    // ---- load: thread -> (row i, lane pair); NTT_LD_BATCH independent 128-bit loads in flight ----
-    const u64* in = p.in + (size_t)g * p.in_seg_stride + (size_t)b * p.in_batch_stride;
-    const u64* pre = p.pre_tab ? p.pre_tab + (size_t)b * p.pre_batch_stride : nullptr;
-    {
-        const u32 lp = tid % LP;
-        const u32 l0 = 2 * lp;                                     // first lane of the pair
-        const u32 t0 = W >= LANES ? 0 : (l0 >> logW), t1 = W >= LANES ? 0 : ((l0 + 1) >> logW);
-        const u32 w0 = W >= LANES ? q0 + l0 : (l0 & (W - 1)), w1 = W >= LANES ? q0 + l0 + 1 : ((l0 + 1) & (W - 1));
-        const u32 c0 = tile * T + t0, c1 = tile * T + t1;
-        const bool ok0 = c0 < ncols, ok1 = c1 < ncols;
-        // element (i, col c, word w): STRIDED row C*i + c; CONTIG row c*C + i, or with y_in_out the row it is written back
-        // to, (c + R*i)*mul + b*add of the output geometry
-        const bool yin = MODE == NTT_CONTIG && ymap;
-        const u64 istride = MODE == NTT_STRIDED ? ((u64)W << p.logC) : (yin ? ((u64)p.out_row_mul << p.logR) * p.out_W : (u64)W);
-        const u64* a0 = MODE == NTT_STRIDED ? in + (size_t)c0 * W + w0
-                        : yin ? in + ((size_t)c0 * p.out_row_mul + (size_t)b * p.out_row_add) * p.out_W + p.out_col0 + w0
-                              : in + (((size_t)c0 << p.logC) * W + w0);
-        const u64* a1 = MODE == NTT_STRIDED ? in + (size_t)c1 * W + w1
-                        : yin ? in + ((size_t)c1 * p.out_row_mul + (size_t)b * p.out_row_add) * p.out_W + p.out_col0 + w1
-                              : in + (((size_t)c1 << p.logC) * W + w1);
-        const bool vec = p.vec_in;
-        constexpr u32 ROWS_PER_IT = NTT2_THREADS / LP;
-        constexpr int LDB = 8;
-#pragma unroll 1
-        for (u32 i0 = tid / LP; i0 < S; i0 += ROWS_PER_IT * LDB) {
-            u64 va[LDB], vb[LDB], f[LDB];
-#pragma unroll
-            for (int k = 0; k < LDB; k++) {
-                const u32 i = i0 + k * ROWS_PER_IT;
-                va[k] = 0; vb[k] = 0; f[k] = 1;
-                if (i < S) {
-                    if (vec) {
-                        if (ok0) { const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(a0 + (u64)i * istride); va[k] = v.x; vb[k] = v.y; }
-                    } else {
-                        if (ok0) va[k] = a0[(u64)i * istride];
-                        if (ok1) vb[k] = a1[(u64)i * istride];
-                    }
-                    if (pre) f[k] = pre[i];
-                }
-            }
-#pragma unroll
-            for (int k = 0; k < LDB; k++) {
-                const u32 i = i0 + k * ROWS_PER_IT;
-                if (i < S) {
-                    if (pre) { va[k] = gl_mul(va[k], f[k]); vb[k] = gl_mul(vb[k], f[k]); }
-                    *reinterpret_cast<ulonglong2*>(s + prow<LK>(i) * LANES + l0) = make_ulonglong2(va[k], vb[k]);
-                }
-            }
-        }
-    }
+    cp_async_wait_all();
     bulk_wait(mbar);
     __syncthreads();
 
     // ---- the sub-transform: forward DIF network, output position pos holds X[bitrev(pos)] ----
-    tile_round<LOGS, 0>(s, rtw, tid);
+    tile_round<LOGS, 0>(s, rtw, p.pre_tab ? p.pre_tab + (size_t)b * p.pre_batch_stride : nullptr, tid);
     __syncthreads();
     if (Plan<LOGS>::rounds == 3) {
-        tile_round<LOGS, 1>(s, rtw + Plan<LOGS>::tw0_entries, tid);
+        tile_round<LOGS, 1>(s, rtw + Plan<LOGS>::tw0_entries, nullptr, tid);
         __syncthreads();
-        tile_round<LOGS, 2>(s, nullptr, tid);
+        tile_round<LOGS, 2>(s, nullptr, nullptr, tid);
     } else {
-        tile_round<LOGS, 1>(s, nullptr, tid);
+        tile_round<LOGS, 1>(s, nullptr, nullptr, tid);
     }
     __syncthreads();
 
