@@ -295,6 +295,14 @@ int wf_mat_evaluate_at(wf_ctx* ctx, const wf_mat* polys, uint32_t ext, uint32_t 
  * composition columns][ext] in that order (DeepCompositionCoefficients, TraceOodFrame + QuotientOodFrame rows). */
 int wf_deep_compose(wf_ctx* ctx, uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const wf_mat* cons_lde, uint32_t log_n,
                     const uint64_t* z, const uint64_t* coeffs, const uint64_t* ood_cur, const uint64_t* ood_next, wf_mat** out);
+/* The same DEEP composition from the COEFFICIENT matrices, as the reference builds it: S = sum_j coeffs_j p_j over the n
+ * coefficients, the synthetic divisions by (X - z) and (X - z*g), and one LDE of the quotient (blowup 2^log_blowup) — the
+ * N x ext matrix wf_deep_compose returns for the LDEs of the same polynomials, bit for bit. main_polys n x width,
+ * aux_polys n x aux_width*ext (NULL for single-segment AIRs), cons_polys n x composition columns*ext (wf_composition_commit's
+ * polys); n a power of two >= 8. No OOD values are taken: the quotient of a synthetic division does not depend on the constant
+ * term, which is all that subtracting S(z) and S(z*g) changes. Reads the n coefficient rows instead of the N LDE rows. */
+int wf_deep_compose_polys(wf_ctx* ctx, uint32_t ext, const wf_mat* main_polys, const wf_mat* aux_polys, const wf_mat* cons_polys,
+                          uint32_t log_blowup, const uint64_t* z, const uint64_t* coeffs, wf_mat** out);
 
 /* ProverChannel::grind_query_seed (prover/src/channel.rs:169-184), serial semantics: the SMALLEST
  * nonce >= 1 with trailing_zeros(first 8 LE bytes of H::merge_with_int(seed, nonce)) >= grinding. */

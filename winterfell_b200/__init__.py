@@ -89,6 +89,7 @@ _SIGS = [
                                                     C.POINTER(vp), C.POINTER(vp)]),
     ("wf_mat_evaluate_at", C.c_int, [vp, vp, C.c_uint32, C.c_uint32, u64p, u64p, u64p, u64p]),
     ("wf_deep_compose", C.c_int, [vp, C.c_uint32, vp, vp, vp, C.c_uint32, u64p, u64p, u64p, u64p, C.POINTER(vp)]),
+    ("wf_deep_compose_polys", C.c_int, [vp, C.c_uint32, vp, vp, vp, C.c_uint32, u64p, u64p, C.POINTER(vp)]),
     ("wf_prove_fib_dev", C.c_int, [vp, vp, C.c_uint32, C.c_uint32, u64p, C.POINTER(C.c_uint32), u8p, C.POINTER(C.c_size_t)]),
     ("wf_grind", C.c_int, [vp, C.c_int, u8p, C.c_uint32, C.POINTER(C.c_uint64)]),
     ("wf_ntt_dev", C.c_int, [vp, vp, C.c_uint32, C.c_uint32, C.c_int]),
@@ -280,6 +281,16 @@ class Context:
         h = vp()
         self.check(self.L.wf_deep_compose(self.h, ext, main_lde.h, aux_lde.h if aux_lde else None, cons_lde.h, log_n, zp, cp, ap, bp,
                                           C.byref(h)))
+        return Mat(self, h)
+
+    def deep_compose_polys(self, ext, main_polys, aux_polys, cons_polys, log_blowup, z, coeffs):
+        """DeepCompositionPoly in coefficient form (composer/mod.rs:67-210): combination of the coefficient matrices, synthetic
+        division by (X - z) and (X - z*g), LDE. Returns the same N x ext Mat as deep_compose on the LDEs of these polynomials."""
+        z_, zp = _u64(z)
+        c_, cp = _u64(coeffs)
+        h = vp()
+        self.check(self.L.wf_deep_compose_polys(self.h, ext, main_polys.h, aux_polys.h if aux_polys else None, cons_polys.h,
+                                                log_blowup, zp, cp, C.byref(h)))
         return Mat(self, h)
 
     def prove_fib(self, trace, results, opts, mont=False, out_buf=None):

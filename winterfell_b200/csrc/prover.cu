@@ -5,18 +5,18 @@
 //   K5     constraint evaluation     (fib_ / generic_constraints) DefaultConstraintEvaluator::evaluate
 //   K6/K7  composition poly + commit (ntt.cu, commit.cu)          DefaultConstraintCommitment::new
 //   K8     out-of-domain frames      (ood_partial_kernel)         TracePolyTable/CompositionPoly::get_ood_frame
-//   K9/K10 DEEP composition          (deep_sum/div_kernel)        DeepCompositionPoly::{add_trace_polys, evaluate}
+//   K9/K10 DEEP composition          (deep_sum_kernel, syn_div_*) DeepCompositionPoly::{add_trace_polys, evaluate}
 //   K11    FRI commit phase          (fri.cu, device coin)        FriProver::build_layers
 //   K13    proof-of-work grinding    (grind_kernel)               ProverChannel::grind_query_seed, smallest nonce
 // The Fiat-Shamir transcript (ProverChannel, prover/src/channel.rs) and the proof wire format
 // (air/src/proof/*.rs) are host code here, bit-exact with the reference; during the FRI commit phase the
 // coin is mirrored on the device and the host replays it afterwards.
 //
-// The DEEP composition is computed in EVALUATION form over the LDE domain,
-//   D(x) = (S(x) - S(z)) / (x - z) + (S(x) - S(zg)) / (x - zg),  S = sum_j cc_j T_j + sum_j cc'_j H_j,
-// which is the same polynomial the reference builds in coefficient form by synthetic division
-// (composer/mod.rs:67-210) and evaluates by LDE (:171): exact field arithmetic, identical values
-// (SURVEY.md A.4), but row-parallel and without the extra LDE.
+// The DEEP composition D = (S - S(z)) / (X - z) + (S - S(zg)) / (X - zg),  S = sum_j cc_j T_j + sum_j cc'_j H_j, is built as the
+// reference builds it (composer/mod.rs:67-210): S over the coefficients, two synthetic divisions (a parallel suffix scan
+// here), one LDE (:171). The stepwise wf_deep_compose and the row-sharded prover, which hold LDE rows and not coefficients,
+// compute the same values in EVALUATION form row by row over the LDE domain: exact field arithmetic, identical values
+// (SURVEY.md A.4).
 //
 // Constraint evaluation needs the AIR on the device (Air::evaluate_transition is user Rust code,
 // air/src/air/mod.rs:210): generic AIRs arrive as a flat description (transition programs for both
@@ -272,7 +272,8 @@ struct DeepParams {
 };
 // DeepCompositionPoly in evaluation form, two kernels:
 //   deep_sum_kernel: S(x) = sum_j cc_j T_j(x) + sum_j cc'_j A_j(x) + sum_j cc''_j H_j(x) for every LDE row — the
-//     pass that reads the whole LDE; one row per thread, coefficients in shared memory, ~40 registers, so
+//     pass that reads the whole LDE (the coefficient form runs it over the coefficient rows, see syn_div_* below);
+//     one row per thread, coefficients in shared memory, ~40 registers, so
 //     the SMs stay full (the earlier single kernel needed 242 registers per thread with cubic elements:
 //     12 % occupancy, 28 % issue utilisation, 2.0 ms for 2^21 rows x 64 columns);
 //   deep_div_kernel: D(x) = (S(x) - S(z)) / (x - z) + (S(x) - S(zg)) / (x - zg) in place, DEEP_ROWS rows per
@@ -353,6 +354,7 @@ __global__ void __launch_bounds__(DEEP_SUM_THREADS) deep_sum_kernel(DeepParams p
     u64* o = p.out.base + row * p.out.W;
 #pragma unroll
     for (int q = 0; q < D; q++) o[q] = S.v[q];
+    for (int q = D; q < p.out.W; q++) o[q] = 0;  // pad lane (W = 4 for D = 3): the LDE of the coefficient form transforms it too
 }
 
 // rows per thread sharing one batch inversion
@@ -462,6 +464,191 @@ static bool deep_point(const GlExt<D>& z, DeepPoint<D>& pt) {
     bool ok = true;
     for (int k = 1; k < D; k++) ok = ok && tr.v[k] == 0 && sm.v[k] == 0 && nm.v[k] == 0;
     return ok;
+}
+
+// DeepCompositionPoly in coefficient form (prove_air, wf_deep_compose_polys), as the reference builds it: S = sum_j dc_j p_j over
+// the n coefficients (deep_sum_kernel run on the coefficient matrices), the synthetic divisions by X - z and X - zg
+// (polynom/mod.rs:498-505), q_i = sum_{k > i} s_k b^(k-i-1), q_(n-1) = 0, i.e. the recurrence q_(i-1) = s_i + b q_i run downwards,
+// then one LDE of q_z + q_zg. The constant term s_0 only reaches the remainder, so S(z) and S(zg) need not be subtracted first (the
+// reference subtracts them, composer/mod.rs:202-210, and the remainder it then drops is zero).
+// The rows [u, v) map q_(v-1) to q_(u-1) = a + p q_(v-1), a = sum_{k in [u, v)} s_k b^(k-u), p = b^(v-u); adjacent runs L = [u, v)
+// and R = [v, w) compose to (a_L + p_L a_R, p_L p_R). The recurrence is a suffix scan of these runs, in the three-launch shape of
+// auxbuild.cu's prefix scans, both points in the same launches:
+//   syn_div_reduce  per tile of SYN_TILE rows: the a of the tile's run (its p is b^SYN_TILE);
+//   syn_div_carry   one block: exclusive suffix scan of the tile runs = q at the top row of every tile;
+//   syn_div_apply   per tile: block-wide exclusive suffix scan with the tile's carry-in, then the recurrence down each thread's
+//                   SYN_ITEMS rows, q_z + q_zg written in place.
+// Rows >= n read as zero, which changes no q (q_(n-1) = 0 either way). Field arithmetic is exact, so the association order of the
+// scan changes no bit, and the LDE of the quotient equals deep_div_kernel's rows.
+#define SYN_THREADS 256
+#define SYN_ITEMS 8
+#define SYN_TILE (SYN_THREADS * SYN_ITEMS)
+template <int D>
+struct SynDivParams {
+    GlExt<D> b[2];        // z, zg
+    GlExt<D> b_items[2];  // b^SYN_ITEMS
+    GlExt<D> b_tile[2];   // b^SYN_TILE
+};
+template <int D>
+struct SynRun {  // x -> a + p x for each point
+    GlExt<D> a[2], p[2];
+};
+template <int D>
+__device__ __forceinline__ SynRun<D> syn_ident() {
+    SynRun<D> r;
+#pragma unroll
+    for (int pt = 0; pt < 2; pt++) { r.a[pt] = ext_zero<D>(); r.p[pt] = ext_from_base<D>(1); }
+    return r;
+}
+// lo: the lower rows, hi: the rows right above them
+template <int D>
+__device__ __forceinline__ SynRun<D> syn_cat(const SynRun<D>& lo, const SynRun<D>& hi) {
+    SynRun<D> r;
+#pragma unroll
+    for (int pt = 0; pt < 2; pt++) { r.a[pt] = ext_add(lo.a[pt], ext_mul(lo.p[pt], hi.a[pt])); r.p[pt] = ext_mul(lo.p[pt], hi.p[pt]); }
+    return r;
+}
+template <int D>
+__device__ __forceinline__ SynRun<D> syn_shfl_down(const SynRun<D>& v, u32 off) {
+    SynRun<D> r;
+#pragma unroll
+    for (int pt = 0; pt < 2; pt++)
+#pragma unroll
+        for (int q = 0; q < D; q++) {
+            r.a[pt].v[q] = __shfl_down_sync(0xffffffffu, v.a[pt].v[q], off);
+            r.p[pt].v[q] = __shfl_down_sync(0xffffffffu, v.p[pt].v[q], off);
+        }
+    return r;
+}
+// exclusive suffix scan over the block (SYN_THREADS threads, thread order = row order): the run of the threads above this one;
+// `total` = the whole block's run
+template <int D>
+__device__ __forceinline__ SynRun<D> syn_block_suffix(const SynRun<D>& v, SynRun<D>& total) {
+    constexpr u32 NW = SYN_THREADS / 32;
+    __shared__ SynRun<D> wrun[NW];
+    const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    SynRun<D> x = v;
+#pragma unroll
+    for (u32 off = 1; off < 32; off <<= 1) {
+        const SynRun<D> y = syn_shfl_down(x, off);
+        if (lane + off < 32) x = syn_cat(x, y);
+    }
+    if (lane == 0) wrun[wid] = x;
+    __syncthreads();
+    if (wid == 0) {
+        SynRun<D> s = lane < NW ? wrun[lane] : syn_ident<D>();
+#pragma unroll
+        for (u32 off = 1; off < NW; off <<= 1) {
+            const SynRun<D> y = syn_shfl_down(s, off);
+            if (lane + off < NW) s = syn_cat(s, y);
+        }
+        if (lane < NW) wrun[lane] = s;
+    }
+    __syncthreads();
+    total = wrun[0];
+    SynRun<D> ex = syn_shfl_down(x, 1);
+    if (lane == 31) ex = syn_ident<D>();
+    if (wid + 1 < NW) ex = syn_cat(ex, wrun[wid + 1]);
+    __syncthreads();  // wrun is free for the next call
+    return ex;
+}
+// rows of the n x D quotient matrix (one segment of width 1, 2 or 4; the pad lane stays zero)
+template <int D>
+__device__ __forceinline__ GlExt<D> syn_ld(const u64* m, size_t i) {
+    GlExt<D> r;
+    if constexpr (D == 1) {
+        r.v[0] = m[i];
+    } else {
+        const ulonglong2 lo = *reinterpret_cast<const ulonglong2*>(m + i * (D == 3 ? 4 : 2));
+        r.v[0] = lo.x; r.v[1] = lo.y;
+        if constexpr (D == 3) r.v[2] = m[i * 4 + 2];
+    }
+    return r;
+}
+template <int D>
+__device__ __forceinline__ void syn_st(u64* m, size_t i, const GlExt<D>& v) {
+    if constexpr (D == 1) {
+        m[i] = v.v[0];
+    } else if constexpr (D == 2) {
+        *reinterpret_cast<ulonglong2*>(m + i * 2) = make_ulonglong2(v.v[0], v.v[1]);
+    } else {
+        ulonglong2* o = reinterpret_cast<ulonglong2*>(m + i * 4);
+        o[0] = make_ulonglong2(v.v[0], v.v[1]);
+        o[1] = make_ulonglong2(v.v[2], 0);
+    }
+}
+// the run of this thread's rows [r0, r0 + SYN_ITEMS): a by Horner from the top row down
+template <int D>
+__device__ __forceinline__ SynRun<D> syn_thread_run(const u64* m, size_t n, size_t r0, const SynDivParams<D>& sp) {
+    SynRun<D> r;
+#pragma unroll
+    for (int pt = 0; pt < 2; pt++) { r.a[pt] = ext_zero<D>(); r.p[pt] = sp.b_items[pt]; }
+#pragma unroll
+    for (int k = SYN_ITEMS - 1; k >= 0; k--) {
+        const GlExt<D> s = r0 + k < n ? syn_ld<D>(m, r0 + k) : ext_zero<D>();
+#pragma unroll
+        for (int pt = 0; pt < 2; pt++) r.a[pt] = ext_add(s, ext_mul(sp.b[pt], r.a[pt]));
+    }
+    return r;
+}
+template <int D>
+__global__ void __launch_bounds__(SYN_THREADS) syn_div_reduce(const u64* s, size_t n, SynDivParams<D> sp, u64* agg /*[tiles][2][D]*/) {
+    const size_t r0 = (size_t)blockIdx.x * SYN_TILE + (size_t)threadIdx.x * SYN_ITEMS;
+    SynRun<D> total;
+    syn_block_suffix<D>(syn_thread_run<D>(s, n, r0, sp), total);
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int pt = 0; pt < 2; pt++)
+#pragma unroll
+            for (int q = 0; q < D; q++) agg[((size_t)blockIdx.x * 2 + pt) * D + q] = total.a[pt].v[q];
+    }
+}
+// one block; tile runs -> carry-in of every tile (q at its top row), in place. Thread t owns a run of consecutive tiles.
+template <int D>
+__global__ void __launch_bounds__(SYN_THREADS) syn_div_carry(u64* agg, size_t ntiles, SynDivParams<D> sp) {
+    const size_t per = (ntiles + SYN_THREADS - 1) / SYN_THREADS;
+    const size_t b = threadIdx.x * per < ntiles ? threadIdx.x * per : ntiles, e = b + per < ntiles ? b + per : ntiles;
+    SynRun<D> mine;
+#pragma unroll
+    for (int pt = 0; pt < 2; pt++) { mine.a[pt] = ext_zero<D>(); mine.p[pt] = ext_from_base<D>(1); }
+    for (size_t i = e; i-- > b;) {
+#pragma unroll
+        for (int pt = 0; pt < 2; pt++) {
+            mine.a[pt] = ext_add(ld_ext<D>(agg + (i * 2 + pt) * D), ext_mul(sp.b_tile[pt], mine.a[pt]));
+            mine.p[pt] = ext_mul(sp.b_tile[pt], mine.p[pt]);
+        }
+    }
+    SynRun<D> total;
+    const SynRun<D> above = syn_block_suffix<D>(mine, total);
+    GlExt<D> run[2] = {above.a[0], above.a[1]};  // nothing lies above the last tile: q there is the run's a
+    for (size_t i = e; i-- > b;) {
+#pragma unroll
+        for (int pt = 0; pt < 2; pt++) {
+            u64* g = agg + (i * 2 + pt) * D;
+            const GlExt<D> a = ld_ext<D>(g);
+#pragma unroll
+            for (int q = 0; q < D; q++) g[q] = run[pt].v[q];
+            run[pt] = ext_add(a, ext_mul(sp.b_tile[pt], run[pt]));
+        }
+    }
+}
+template <int D>
+__global__ void __launch_bounds__(SYN_THREADS) syn_div_apply(u64* s, size_t n, SynDivParams<D> sp, const u64* carry) {
+    const size_t r0 = (size_t)blockIdx.x * SYN_TILE + (size_t)threadIdx.x * SYN_ITEMS;
+    SynRun<D> total;
+    const SynRun<D> above = syn_block_suffix<D>(syn_thread_run<D>(s, n, r0, sp), total);
+    GlExt<D> q[2];  // q at row r0 + SYN_ITEMS - 1
+#pragma unroll
+    for (int pt = 0; pt < 2; pt++) q[pt] = ext_add(above.a[pt], ext_mul(above.p[pt], ld_ext<D>(carry + ((size_t)blockIdx.x * 2 + pt) * D)));
+#pragma unroll
+    for (int k = SYN_ITEMS - 1; k >= 0; k--) {
+        const size_t i = r0 + k;
+        if (i >= n) continue;
+        const GlExt<D> si = syn_ld<D>(s, i);  // read before the row is overwritten
+        syn_st<D>(s, i, ext_add(q[0], q[1]));
+#pragma unroll
+        for (int pt = 0; pt < 2; pt++) q[pt] = ext_add(si, ext_mul(sp.b[pt], q[pt]));
+    }
 }
 
 // Proof-of-work grinding (K13; prover/src/channel.rs:169-184, crypto/src/random/default.rs:141-146):
@@ -1142,7 +1329,6 @@ int deep_compose(wf_ctx* ctx, const wf_mat* lde, const wf_mat* alde, const wf_ma
     d_dq = d_dt + (size_t)ct * D;
     wf_mat* deep;
     CKI(wf_mat_alloc(ctx, N, D, &deep));
-    if (deep->m.W > D) CK(cudaMemsetAsync(deep->m.base, 0, deep->m.words() * 8, ctx->st));
     DeepParams p;
     p.trace = lde->m; p.cons = clde->m; p.out = deep->m; p.c = c; p.kc = kc; p.log_N = log_N;
     p.row0 = row0; p.nrows = nrows;
@@ -1162,6 +1348,43 @@ int deep_compose(wf_ctx* ctx, const wf_mat* lde, const wf_mat* alde, const wf_ma
     wf_dev_free(ctx, d_dt);
     *out = deep;
     return WF_OK;
+}
+
+// The same DEEP composition in coefficient form (see syn_div_*): polys n x c, apolys n x aw*D (nullptr: single segment), cpolys
+// n x kc*D coefficient matrices -> the N x D LDE of the quotient, N = n << log_b, the matrix deep_compose returns. It reads the
+// coefficients (8(c + a·d + k·d) B per coefficient row) instead of the LDE rows.
+template <int D>
+int deep_compose_polys(wf_ctx* ctx, const wf_mat* polys, const wf_mat* apolys, const wf_mat* cpolys, u32 kc, u32 log_b,
+                       const std::vector<GlExt<D>>& dc, const GlExt<D>& z, const GlExt<D>& zg, wf_mat** out) {
+    const u32 c = polys->m.cols, aw = apolys ? apolys->m.cols / D : 0, ct = c + aw;
+    const size_t n = polys->m.rows, ntiles = (n + SYN_TILE - 1) / SYN_TILE;
+    u32 log_n = 0;
+    while (((size_t)1 << log_n) < n) log_n++;
+    DevScratch tmp(ctx);
+    u64* d_dt;
+    CKI(upload_ext<D>(ctx, dc, 0, ct + kc, &d_dt));
+    tmp.bufs.push_back(d_dt);
+    void* d_agg;
+    CKI(tmp.alloc(ntiles * 2 * D * 8, &d_agg));
+    wf_mat* quot;
+    CKI(wf_mat_alloc(ctx, n, D, &quot));
+    DeepParams p{};
+    p.trace = polys->m; p.cons = cpolys->m; p.out = quot->m; p.c = c; p.kc = kc; p.log_N = log_n;
+    p.tcc = d_dt; p.acc = d_dt + (size_t)c * D; p.ccc = d_dt + (size_t)ct * D; p.aw = aw;
+    p.aux = aw ? apolys->m : polys->m;
+    deep_sum_kernel<D><<<(unsigned)((n + DEEP_SUM_THREADS - 1) / DEEP_SUM_THREADS), DEEP_SUM_THREADS, (size_t)(ct + kc) * D * 8, ctx->st>>>(p);
+    SynDivParams<D> sp;
+    sp.b[0] = z; sp.b[1] = zg;
+    for (int pt = 0; pt < 2; pt++) { sp.b_items[pt] = ext_pow(sp.b[pt], SYN_ITEMS); sp.b_tile[pt] = ext_pow(sp.b[pt], SYN_TILE); }
+    syn_div_reduce<D><<<(unsigned)ntiles, SYN_THREADS, 0, ctx->st>>>(quot->m.base, n, sp, (u64*)d_agg);
+    syn_div_carry<D><<<1, SYN_THREADS, 0, ctx->st>>>((u64*)d_agg, ntiles, sp);
+    syn_div_apply<D><<<(unsigned)ntiles, SYN_THREADS, 0, ctx->st>>>(quot->m.base, n, sp, (const u64*)d_agg);
+    ctx->launches += 4;
+    const cudaError_t e = cudaGetLastError();
+    // the quotient and the scratch go back to the pool in stream order, behind the LDE that reads them
+    const int r = e == cudaSuccess ? wf_mat_lde(ctx, quot, log_b, out) : wf_fail(ctx, WF_ERR_CUDA, "DEEP quotient launch: %s", cudaGetErrorString(e));
+    wf_mat_free(ctx, quot);
+    return r;
 }
 
 // Device objects of one proof: whatever is still registered when prove_air leaves (normally or through
@@ -1348,12 +1571,9 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
         ch.coin.reseed(dg);  // channel.rs:109-112 (not added to the commitments)
     }
     wf_mark(ctx, "ood_frames");
-    // ---- 5. DEEP composition (lib.rs:403-440), evaluation form ----
+    // ---- 5. DEEP composition (lib.rs:403-440), coefficient form ----
     std::vector<GlExt<D>> dc = ch.draw_coeffs(o.batch_d, ct + kc);
-    GlExt<D> Sz = ext_zero<D>(), Szg = ext_zero<D>();  // S(z), S(zg): the constant terms composer/mod.rs:202-210 subtracts
-    for (u32 j = 0; j < ct; j++) { Sz = ext_add(Sz, ext_mul(dc[j], t_cur[j])); Szg = ext_add(Szg, ext_mul(dc[j], t_nxt[j])); }
-    for (u32 j = 0; j < kc; j++) { Sz = ext_add(Sz, ext_mul(dc[ct + j], q_cur[j])); Szg = ext_add(Szg, ext_mul(dc[ct + j], q_nxt[j])); }
-    CKI(deep_compose<D>(ctx, lde, alde, clde, kc, log_n + log_b, dc, z, zg, Sz, Szg, &deep));
+    CKI(deep_compose_polys<D>(ctx, polys, apolys, cpolys, kc, log_b, dc, z, zg, &deep));
     wf_mark(ctx, "deep_composition");
     // ---- 6. FRI (lib.rs:442-448) ----
     {   // transcript replicated on the device: one synchronisation for the whole commit phase (capi.cu)
@@ -2273,6 +2493,33 @@ extern "C" int wf_deep_compose(wf_ctx* ctx, uint32_t ext, const wf_mat* main_lde
         case 1: return deep_entry<1>(ctx, main_lde, aux_lde, cons_lde, log_n, z, coeffs, ood_cur, ood_next, out);
         case 2: return deep_entry<2>(ctx, main_lde, aux_lde, cons_lde, log_n, z, coeffs, ood_cur, ood_next, out);
         default: return deep_entry<3>(ctx, main_lde, aux_lde, cons_lde, log_n, z, coeffs, ood_cur, ood_next, out);
+    }
+}
+
+template <int D>
+static int deep_polys_entry(wf_ctx* ctx, const wf_mat* polys, const wf_mat* apolys, const wf_mat* cpolys, u32 log_n, u32 log_b,
+                            const uint64_t* zw, const uint64_t* coeffs, wf_mat** out) {
+    const u32 kc = cpolys->m.cols / D, tot = polys->m.cols + (apolys ? apolys->m.cols / D : 0) + kc;
+    std::vector<GlExt<D>> dc(tot);
+    GlExt<D> z = ext_zero<D>();
+    for (int q = 0; q < D; q++) z.v[q] = zw[q];
+    for (u32 i = 0; i < tot; i++) for (int q = 0; q < D; q++) dc[i].v[q] = coeffs[i * D + q];
+    return deep_compose_polys<D>(ctx, polys, apolys, cpolys, kc, log_b, dc, z, ext_mul_base(z, gl_root_of_unity(log_n)), out);
+}
+extern "C" int wf_deep_compose_polys(wf_ctx* ctx, uint32_t ext, const wf_mat* main_polys, const wf_mat* aux_polys, const wf_mat* cons_polys,
+                                     uint32_t log_blowup, const uint64_t* z, const uint64_t* coeffs, wf_mat** out) {
+    if (!ctx || !main_polys || !cons_polys || !z || !coeffs || !out || ext < 1 || ext > 3 || cons_polys->m.cols % ext ||
+        cons_polys->m.rows != main_polys->m.rows || (aux_polys && (aux_polys->m.cols % ext || aux_polys->m.rows != main_polys->m.rows)))
+        return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    const size_t n = main_polys->m.rows;
+    u32 log_n = 0;
+    while (((size_t)1 << log_n) < n) log_n++;
+    if (n < 8 || (n & (n - 1))) return wf_fail(ctx, WF_ERR_INVALID, "rows must be a power of two >= 8");
+    if (log_blowup < 1 || log_blowup > 7 || log_n + log_blowup > 32) return wf_fail(ctx, WF_ERR_INVALID, "bad blowup");
+    switch (ext) {
+        case 1: return deep_polys_entry<1>(ctx, main_polys, aux_polys, cons_polys, log_n, log_blowup, z, coeffs, out);
+        case 2: return deep_polys_entry<2>(ctx, main_polys, aux_polys, cons_polys, log_n, log_blowup, z, coeffs, out);
+        default: return deep_polys_entry<3>(ctx, main_polys, aux_polys, cons_polys, log_n, log_blowup, z, coeffs, out);
     }
 }
 
