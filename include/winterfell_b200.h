@@ -263,6 +263,23 @@ int wf_prove_air_aux_built(wf_ctx* ctx, const uint64_t* air_desc, size_t air_des
                            const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont, uint32_t log_n, const uint32_t* opts,
                            wf_aux_assertions_fn aux_assertions, void* aux_user, uint8_t* proof, size_t* proof_len);
 
+/* ---- batches: `batch` proofs of ONE AIR structure in one call ----------------------------------------------------------
+ * Proof j is byte-identical to wf_prove_air (aux_build == NULL) or to wf_prove_air_aux_built (aux_build given, no aux
+ * assertion callback) on air_descs[j] and trace j, with the same opts and log_n. air_descs[j] may differ from air_descs[0]
+ * only in the public inputs and in the VALUES of the assertions (sequence assertions included); everything else the prover
+ * reads from a description must be identical (wf_air_batch_check). Exactly one of trace_cols ([batch * width] host column pointers,
+ * proof-major, representation by `mont`) and d_traces (device, [batch][width][2^log_n], canonical). proofs[j] /
+ * proof_lens[j]: in = capacity, out = bytes. All or nothing: on any error no proof is written, the error names the proof
+ * it concerns, and no device buffer stays live. The proofs are currently computed one after the other inside the call: a
+ * batch issues as many kernel launches as a loop over wf_prove_air. */
+int wf_prove_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
+                       const uint64_t* aux_build, size_t aux_build_len, const uint64_t* const* trace_cols, const uint64_t* d_traces,
+                       int mont, uint32_t log_n, const uint32_t* opts, uint8_t* const* proofs, size_t* proof_lens);
+/* The checks wf_prove_air_batch runs on its descriptions, without a device: every description passes wf_air_check, and all
+ * share the structure of air_descs[0]. WF_OK, or WF_ERR_INVALID with the reason (and the proof it concerns) in msg. */
+int wf_air_batch_check(uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens, uint32_t log_n, uint32_t blowup,
+                       char* msg, size_t msg_cap);
+
 /* ---- the same pipeline as separate steps, for a host that owns the transcript (the Rust shim of
  *      INTEGRATION.md: impl ConstraintEvaluator / ConstraintCommitment, prover/src/lib.rs:195-223) ---- */
 /* ConstraintEvaluator::evaluate (prover/src/constraints/evaluator/mod.rs:28-42, default.rs:60-118) +

@@ -102,6 +102,9 @@ _SIGS = [
     ("wf_ctx_jit_stats", C.c_int, [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     ("wf_jit_compile_air", C.c_int, [u64p, C.c_size_t, C.c_uint32, C.POINTER(C.c_size_t), C.c_char_p, C.c_size_t]),
     ("wf_air_check", C.c_int, [u64p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]),
+    ("wf_prove_air_batch", C.c_int, [vp, C.c_uint32, C.POINTER(u64p), C.POINTER(C.c_size_t), u64p, C.c_size_t, C.POINTER(u64p), vp, C.c_int,
+                                     C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(u8p), C.POINTER(C.c_size_t)]),
+    ("wf_air_batch_check", C.c_int, [C.c_uint32, C.POINTER(u64p), C.POINTER(C.c_size_t), C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]),
     ("wf_host_hash_elements", C.c_int, [C.c_int, u64p, C.c_size_t, u8p]),
     ("wf_host_merge", C.c_int, [C.c_int, u8p, u8p]),
     ("wf_host_merge_with_int", C.c_int, [C.c_int, u8p, C.c_uint64, u8p]),
@@ -441,6 +444,39 @@ class Context:
                                                  C.byref(ln)))
         return buf[: ln.value].tobytes()
 
+    def prove_air_batch(self, descs, traces, opts, mont=False, aux_build=None, device=False, proof_cap=1 << 21):
+        """wf_prove_air_batch: one proof per description of the list `descs` (one AIR structure; public inputs and assertion
+        values may differ). traces: host [batch, width, n] uint64 (an array or a list of [width, n] arrays), or with
+        device=True a CUDA tensor of shape [batch, width, n] holding canonical 64-bit words. aux_build: build description of
+        the aux segments (wf_prove_air_aux_built). proof_cap: bytes reserved per proof. Returns the list of proof bytes."""
+        ds = [np.ascontiguousarray(d, dtype=np.uint64) for d in descs]
+        batch = len(ds)
+        dps = (u64p * batch)(*[d.ctypes.data_as(u64p) for d in ds])
+        dls = (C.c_size_t * batch)(*[d.size for d in ds])
+        ptrs, dev = None, None
+        if device:
+            if tuple(traces.shape[:1]) != (batch,) or not traces.is_contiguous():
+                raise ValueError("device traces: a contiguous [batch, width, n] tensor")
+            n = int(traces.shape[2])
+            dev = vp(traces.data_ptr())
+        else:
+            arrs = [np.ascontiguousarray(t, dtype=np.uint64) for t in traces]   # no copy of contiguous uint64 traces
+            if len(arrs) != batch or len({a.shape for a in arrs}) != 1:
+                raise ValueError("one trace of one shape per description")
+            n = arrs[0].shape[1]
+            ptrs = (u64p * (batch * arrs[0].shape[0]))(*[row.ctypes.data_as(u64p) for a in arrs for row in a])
+        bp, bl = None, 0
+        if aux_build is not None:
+            b_, bp = _u64(aux_build)
+            bl = b_.size
+        o_ = np.ascontiguousarray(opts, dtype=np.uint32)
+        buf = np.zeros((batch, proof_cap), dtype=np.uint8)
+        outs = (u8p * batch)(*[buf[j].ctypes.data_as(u8p) for j in range(batch)])
+        lens = (C.c_size_t * batch)(*([proof_cap] * batch))
+        self.check(self.L.wf_prove_air_batch(self.h, batch, dps, dls, bp, bl, ptrs, dev, int(mont), int(n).bit_length() - 1,
+                                             o_.ctypes.data_as(C.POINTER(C.c_uint32)), outs, lens))
+        return [buf[j, : lens[j]].tobytes() for j in range(batch)]
+
     def prove_fib_dev(self, d_trace, k, log_n, results, opts, out_buf=None):
         """trace resident on the device: column-major [2k][n] at raw pointer d_trace."""
         r_, rp = _u64(results)
@@ -671,6 +707,17 @@ def air_check(desc, log_n, blowup):
     d_, dp = _u64(desc)
     msg = C.create_string_buffer(512)
     rc = lib().wf_air_check(dp, d_.size, log_n, blowup, msg, 512)
+    return rc, msg.value.decode(errors="replace")
+
+
+def air_batch_check(descs, log_n, blowup):
+    """The checks wf_prove_air_batch runs on its descriptions (each passes air_check, all share one structure), without a
+    device. Returns (status, reason)."""
+    ds = [np.ascontiguousarray(d, dtype=np.uint64) for d in descs]
+    dps = (u64p * len(ds))(*[d.ctypes.data_as(u64p) for d in ds])
+    dls = (C.c_size_t * len(ds))(*[d.size for d in ds])
+    msg = C.create_string_buffer(512)
+    rc = lib().wf_air_batch_check(len(ds), dps, dls, log_n, blowup, msg, 512)
     return rc, msg.value.decode(errors="replace")
 
 

@@ -2225,18 +2225,22 @@ static int parse_options(wf_ctx* ctx, const uint32_t* opts, Options& o) {
     if (!WF_HASH_IS_KNOWN(o.hash_id)) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "unknown hash %d", o.hash_id);
     return WF_OK;
 }
+// the proof bytes of one proof, prove_air<D> for the extension degree of the options
+static int prove_bytes(wf_ctx* ctx, const AirHost& air, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont,
+                       uint32_t log_n, const Options& o, std::vector<u8>& out, wf_aux_builder_fn aux_builder, void* aux_user,
+                       wf_aux_assertions_fn aux_assertions, const AuxBuildHost* aux_build) {
+    switch (o.ext) {
+        case 1: return prove_air<1>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions, aux_build);
+        case 2: return prove_air<2>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions, aux_build);
+        case 3: return prove_air<3>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions, aux_build);
+    }
+    return wf_fail(ctx, WF_ERR_UNSUPPORTED, "field extension %u", o.ext);
+}
 static int prove_dispatch(wf_ctx* ctx, const AirHost& air, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont,
                           uint32_t log_n, const Options& o, uint8_t* proof, size_t* proof_len, wf_aux_builder_fn aux_builder = nullptr,
                           void* aux_user = nullptr, wf_aux_assertions_fn aux_assertions = nullptr, const AuxBuildHost* aux_build = nullptr) {
     std::vector<u8> out;
-    int r;
-    switch (o.ext) {
-        case 1: r = prove_air<1>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions, aux_build); break;
-        case 2: r = prove_air<2>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions, aux_build); break;
-        case 3: r = prove_air<3>(ctx, air, trace_cols, d_trace, mont, log_n, o, aux_builder, aux_user, out, aux_assertions, aux_build); break;
-        default: return wf_fail(ctx, WF_ERR_UNSUPPORTED, "field extension %u", o.ext);
-    }
-    if (r != WF_OK) return r;
+    CKI(prove_bytes(ctx, air, trace_cols, d_trace, mont, log_n, o, out, aux_builder, aux_user, aux_assertions, aux_build));
     if (out.size() > *proof_len) return wf_fail(ctx, WF_ERR_INVALID, "proof buffer too small (%zu needed)", out.size());
     memcpy(proof, out.data(), out.size());
     *proof_len = out.size();
@@ -2353,6 +2357,16 @@ extern "C" int wf_jit_compile_air(const uint64_t* air_desc, size_t air_desc_len,
 // The checks wf_prove_air / wf_eval_constraints run on an AIR description before touching the device, without a device:
 // structure of the description, degrees against the blowup factor, periodic columns, assertion validity and overlaps
 // (the panics of Air::new / BoundaryConstraints::new / prepare_assertions in the reference, returned as a status).
+static int air_check_host(wf_ctx* ctx, const AirHost& air, uint32_t log_n, uint32_t blowup) {
+    u32 log_b = 0;
+    while ((1u << log_b) < blowup) log_b++;
+    const size_t n = (size_t)1 << log_n;
+    if (air.log_ce_blowup() > log_b) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
+    for (auto& col : air.periodic) if (col.size() > n) return wf_fail(ctx, WF_ERR_INVALID, "periodic column longer than the trace");
+    CKI(validate_degrees(ctx, air.all_degrees(), n));
+    CKI(validate_assertions(ctx, air.aux_asserts, n, 3, "aux assertion"));
+    return validate_assertions(ctx, air.asserts, n, 1, "assertion");
+}
 extern "C" int wf_air_check(const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup, char* msg, size_t msg_cap) {
     auto say = [&](const char* t) { if (msg && msg_cap) { strncpy(msg, t, msg_cap - 1); msg[msg_cap - 1] = 0; } };
     say("");
@@ -2360,17 +2374,102 @@ extern "C" int wf_air_check(const uint64_t* air_desc, size_t air_desc_len, uint3
     AirHost air;
     if (!parse_air_host(air_desc, air_desc_len, air)) { say("malformed AIR description"); return WF_ERR_INVALID; }
     wf_ctx note{};   // carries the message of the shared validators, nothing else
-    u32 log_b = 0;
-    while ((1u << log_b) < blowup) log_b++;
-    const size_t n = (size_t)1 << log_n;
-    int r = WF_OK;
-    if (air.log_ce_blowup() > log_b) r = wf_fail(&note, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
-    for (auto& col : air.periodic) if (r == WF_OK && col.size() > n) r = wf_fail(&note, WF_ERR_INVALID, "periodic column longer than the trace");
-    if (r == WF_OK) r = validate_degrees(&note, air.all_degrees(), n);
-    if (r == WF_OK) r = validate_assertions(&note, air.aux_asserts, n, 3, "aux assertion");
-    if (r == WF_OK) r = validate_assertions(&note, air.asserts, n, 1, "assertion");
+    const int r = air_check_host(&note, air, log_n, blowup);
     say(note.err.c_str());
     return r;
+}
+
+// ---- batches of proofs of one AIR (wf_prove_air_batch) ----
+// What the descriptions of one batch must share: everything but the public inputs and the assertion values. Returns the first
+// part that differs, nullptr when the two have the same structure.
+static const char* air_structure_mismatch(const AirHost& a, const AirHost& b) {
+    // reasons[0..4]: count, columns, steps, strides, value counts
+    auto layout = [](const std::vector<AirAssertion>& x, const std::vector<AirAssertion>& y, const char* const* reasons) -> const char* {
+        if (x.size() != y.size()) return reasons[0];
+        for (size_t i = 0; i < x.size(); i++) {
+            if (x[i].column != y[i].column) return reasons[1];
+            if (x[i].first_step != y[i].first_step) return reasons[2];
+            if (x[i].stride != y[i].stride) return reasons[3];
+            if (x[i].values.size() != y[i].values.size()) return reasons[4];
+        }
+        return nullptr;
+    };
+    static const char* const main_r[] = {"number of assertions", "assertion columns", "assertion steps", "assertion strides",
+                                         "assertion value counts"};
+    static const char* const aux_r[] = {"number of aux assertions", "aux assertion columns", "aux assertion steps",
+                                        "aux assertion strides", "aux assertion value counts"};
+    if (a.w != b.w) return "trace width";
+    if (a.degrees != b.degrees) return "transition constraint degrees";
+    if (a.periodic != b.periodic) return "periodic columns";
+    if (a.consts != b.consts) return "constants";
+    if (a.num_regs != b.num_regs || a.prog != b.prog) return "transition program";
+    if (const char* why = layout(a.asserts, b.asserts, main_r)) return why;
+    if (a.exemptions != b.exemptions) return "transition exemptions";
+    if ((a.aw == 0) != (b.aw == 0)) return "aux segment";
+    if (a.aw != b.aw || a.nr != b.nr) return "aux width or random elements";
+    if (a.aux_degrees != b.aux_degrees) return "aux transition constraint degrees";
+    if (a.aux_num_regs != b.aux_num_regs || a.aux_prog != b.aux_prog) return "aux transition program";
+    return layout(a.aux_asserts, b.aux_asserts, aux_r);
+}
+// Parses the descriptions of a batch and runs every check of wf_air_check on each, and the structure check against proof 0
+static int air_batch_parse(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens, uint32_t log_n,
+                           uint32_t blowup, std::vector<AirHost>& airs) {
+    if (batch == 0 || !air_descs || !air_desc_lens || log_n < 3 || log_n > 32 || blowup < 2 || blowup > 128 || (blowup & (blowup - 1)))
+        return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    airs.assign(batch, AirHost());
+    for (u32 j = 0; j < batch; j++) {
+        if (!air_descs[j] || !parse_air_host(air_descs[j], air_desc_lens[j], airs[j]))
+            return wf_fail(ctx, WF_ERR_INVALID, "proof %u: malformed AIR description", j);
+        if (air_check_host(ctx, airs[j], log_n, blowup) != WF_OK) return wf_fail(ctx, WF_ERR_INVALID, "proof %u: %s", j, std::string(ctx->err).c_str());
+        if (const char* why = j ? air_structure_mismatch(airs[0], airs[j]) : nullptr)
+            return wf_fail(ctx, WF_ERR_INVALID, "proof %u differs from proof 0 in its %s", j, why);
+    }
+    return WF_OK;
+}
+extern "C" int wf_air_batch_check(uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens, uint32_t log_n,
+                                  uint32_t blowup, char* msg, size_t msg_cap) {
+    wf_ctx note{};
+    std::vector<AirHost> airs;
+    const int r = air_batch_parse(&note, batch, air_descs, air_desc_lens, log_n, blowup, airs);
+    if (msg && msg_cap) { strncpy(msg, note.err.c_str(), msg_cap - 1); msg[msg_cap - 1] = 0; }
+    return r;
+}
+extern "C" int wf_prove_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
+                                  const uint64_t* aux_build, size_t aux_build_len, const uint64_t* const* trace_cols, const uint64_t* d_traces,
+                                  int mont, uint32_t log_n, const uint32_t* opts, uint8_t* const* proofs, size_t* proof_lens) {
+    if (!ctx || !opts || !proofs || !proof_lens) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    if (!trace_cols == !d_traces) return wf_fail(ctx, WF_ERR_INVALID, "pass exactly one of trace_cols (host) and d_traces (device)");
+    Options o;
+    CKI(parse_options(ctx, opts, o));
+    std::vector<AirHost> airs;
+    CKI(air_batch_parse(ctx, batch, air_descs, air_desc_lens, log_n, o.blowup, airs));
+    for (u32 j = 0; j < batch; j++) if (!proofs[j]) return wf_fail(ctx, WF_ERR_INVALID, "proof %u: no output buffer", j);
+    AuxBuildHost b;
+    if (aux_build) {
+        CKI(parse_aux_build(ctx, airs[0], aux_build, aux_build_len, b));
+        for (auto& col : b.cols)
+            for (u32 q = o.ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
+    } else if (airs[0].aw) {
+        return wf_fail(ctx, WF_ERR_INVALID, "multi-segment AIR: a batch builds its aux segments from aux_build");
+    }
+    const u32 w = airs[0].w;
+    const size_t n = (size_t)1 << log_n;
+    // The proofs run one after another through the single-proof sequence: launches and synchronisations grow with the batch.
+    // They are kept on the host until all of them exist: nothing is written when one fails.
+    std::vector<std::vector<u8>> out(batch);
+    for (u32 j = 0; j < batch; j++) {
+        const uint64_t* const* cols = trace_cols ? trace_cols + (size_t)j * w : nullptr;
+        const uint64_t* dev = d_traces ? d_traces + (size_t)j * w * n : nullptr;
+        const int r = prove_bytes(ctx, airs[j], cols, dev, mont, log_n, o, out[j], nullptr, nullptr, nullptr, aux_build ? &b : nullptr);
+        if (r != WF_OK) return wf_fail(ctx, r, "proof %u: %s", j, std::string(ctx->err).c_str());
+    }
+    for (u32 j = 0; j < batch; j++)
+        if (out[j].size() > proof_lens[j]) return wf_fail(ctx, WF_ERR_INVALID, "proof %u: proof buffer too small (%zu needed)", j, out[j].size());
+    for (u32 j = 0; j < batch; j++) {
+        memcpy(proofs[j], out[j].data(), out[j].size());
+        proof_lens[j] = out[j].size();
+    }
+    return WF_OK;
 }
 
 // ---- stepwise exports: the seams of prover/src/lib.rs:125-223 (ConstraintEvaluator, ConstraintCommitment)
