@@ -280,6 +280,49 @@ int wf_prove_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_d
 int wf_air_batch_check(uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens, uint32_t log_n, uint32_t blowup,
                        char* msg, size_t msg_cap);
 
+/* ---- checking a trace against its AIR: the reference's debug builds (Trace::validate, prover/src/trace/mod.rs:86-201;
+ *      ConstraintEvaluationTable::validate_transition_degrees, prover/src/constraints/evaluation_table.rs:181-230) ----------
+ * Trace check: every main assertion (description order, each one's steps increasing), then every aux assertion (values in E:
+ * the first `ext` words of each value), then every transition constraint on steps 0 .. n - exemptions over the trace rows
+ * (step, step + 1); periodic value j at step i is column j's value i mod its length. A constraint's value is the sum of all
+ * its OUT instructions. Degree check (check_degrees != 0): each transition constraint's evaluations over the constraint
+ * evaluation domain 7 <w_ce>, divided by the transition divisor, interpolated; the index of the highest non-zero coefficient
+ * must equal the declared degree base (n-1) + sum (n/c)(c-1) - (n - exemptions), and max(max actual, n + 1) rounded up to a
+ * power of two must equal ce. */
+#define WF_VALID 0
+#define WF_VIOLATION_MAIN_ASSERTION 1
+#define WF_VIOLATION_AUX_ASSERTION 2
+#define WF_VIOLATION_MAIN_TRANSITION 3
+#define WF_VIOLATION_AUX_TRANSITION 4
+#define WF_VIOLATION_DEGREES 5
+#define WF_VIOLATION_CE_DOMAIN 6
+typedef struct wf_validation {
+    uint32_t kind;    /* the FIRST violation in the reference's order (assertions, transitions by step with main before aux,
+                         degrees, domain size), or WF_VALID */
+    uint32_t index;   /* assertion index in description order, or constraint index within its segment */
+    uint64_t step;    /* failing step (assertions, transitions) */
+    uint32_t column;  /* assertion column */
+    uint32_t num_transition_constraints;  /* main + aux: length of the arrays below */
+} wf_validation;
+/* Exactly one of trace_cols (host columns, representation by `mont`) and d_trace (device, column-major [width][2^log_n],
+ * canonical). A two-segment AIR takes exactly one of aux_build (the aux segment built on the device from rand, as
+ * wf_aux_build) and aux_cols ([aw] host columns of [2^log_n][ext] words, representation by `mont`). rand: [nr][ext] canonical.
+ * WF_OK when the check ran (report->kind says whether the trace is valid; msg gets the reference's panic message);
+ * WF_ERR_INVALID for a bad description or arguments, with the reason of wf_air_check / wf_aux_build_check.
+ * first_failing_step (or NULL): per transition constraint, main then aux, the smallest failing step, ~0 when it never fails.
+ * expected_degrees / actual_degrees (or NULL): filled when check_degrees is set, even when the trace check failed. No device
+ * buffer stays live after any return. Device scratch of the degree check: ce * (n_main + n_aux * ext) * 8 bytes, twice. */
+int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len,
+                      const uint64_t* const* aux_cols, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont,
+                      const uint64_t* rand, uint32_t log_n, uint32_t ext, int check_degrees, wf_validation* report,
+                      uint64_t* first_failing_step, uint64_t* expected_degrees, uint64_t* actual_degrees, char* msg, size_t msg_cap);
+/* The analogue of a debug build (default off). On: wf_prove_air, wf_prove_air_aux, wf_prove_air_aux_dyn, wf_prove_air_aux_built
+ * and wf_prove_air_batch run the trace check after the aux segment is built and its assertion values are final (with the
+ * transcript's random elements), and the degree check on their own LDEs right after constraint evaluation;
+ * wf_eval_constraints runs the degree check. A violation returns WF_ERR_INVALID with the reference's message, writes no proof
+ * and leaves no buffer live. Off: these paths are unchanged. wf_prove_fib* and the sharded prover are not checked. */
+int wf_ctx_set_validation(wf_ctx* ctx, int on);
+
 /* ---- the same pipeline as separate steps, for a host that owns the transcript (the Rust shim of
  *      INTEGRATION.md: impl ConstraintEvaluator / ConstraintCommitment, prover/src/lib.rs:195-223) ---- */
 /* ConstraintEvaluator::evaluate (prover/src/constraints/evaluator/mod.rs:28-42, default.rs:60-118) +

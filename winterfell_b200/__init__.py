@@ -30,6 +30,16 @@ FRI_COMMIT_FN = C.CFUNCTYPE(None, C.c_void_p, u8p)
 FRI_DRAW_FN = C.CFUNCTYPE(None, C.c_void_p, u64p)
 AUX_BUILDER = C.CFUNCTYPE(C.c_int, C.c_void_p, u64p, u64p)
 
+# wf_validation (include/winterfell_b200.h): the first violation wf_trace_validate found, in the reference's order
+VALID, VIOLATION_MAIN_ASSERTION, VIOLATION_AUX_ASSERTION, VIOLATION_MAIN_TRANSITION, VIOLATION_AUX_TRANSITION, VIOLATION_DEGREES, \
+    VIOLATION_CE_DOMAIN = range(7)
+
+
+class Validation(C.Structure):
+    _fields_ = [("kind", C.c_uint32), ("index", C.c_uint32), ("step", C.c_uint64), ("column", C.c_uint32),
+                ("num_transition_constraints", C.c_uint32)]
+
+
 _lib = None
 
 # every symbol include/winterfell_b200.h declares: (name, restype, argtypes)
@@ -104,6 +114,9 @@ _SIGS = [
     ("wf_air_check", C.c_int, [u64p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]),
     ("wf_prove_air_batch", C.c_int, [vp, C.c_uint32, C.POINTER(u64p), C.POINTER(C.c_size_t), u64p, C.c_size_t, C.POINTER(u64p), vp, C.c_int,
                                      C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(u8p), C.POINTER(C.c_size_t)]),
+    ("wf_trace_validate", C.c_int, [vp, u64p, C.c_size_t, u64p, C.c_size_t, C.POINTER(u64p), C.POINTER(u64p), vp, C.c_int, u64p, C.c_uint32,
+                                    C.c_uint32, C.c_int, C.POINTER(Validation), u64p, u64p, u64p, C.c_char_p, C.c_size_t]),
+    ("wf_ctx_set_validation", C.c_int, [vp, C.c_int]),
     ("wf_air_batch_check", C.c_int, [C.c_uint32, C.POINTER(u64p), C.POINTER(C.c_size_t), C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]),
     ("wf_host_hash_elements", C.c_int, [C.c_int, u64p, C.c_size_t, u8p]),
     ("wf_host_merge", C.c_int, [C.c_int, u8p, u8p]),
@@ -476,6 +489,52 @@ class Context:
         self.check(self.L.wf_prove_air_batch(self.h, batch, dps, dls, bp, bl, ptrs, dev, int(mont), int(n).bit_length() - 1,
                                              o_.ctypes.data_as(C.POINTER(C.c_uint32)), outs, lens))
         return [buf[j, : lens[j]].tobytes() for j in range(batch)]
+
+    def trace_validate(self, desc, trace, ext=1, rand=None, aux=None, aux_build=None, n=None, mont=False, check_degrees=True):
+        """wf_trace_validate: checks a trace against its AIR as the reference's debug builds do (Trace::validate, then
+        validate_transition_degrees when check_degrees). trace: [width, n] uint64 host array, or an integer device pointer to
+        column-major [width][n] canonical words (then `n` is required). Two-segment AIRs take rand [num_rands, ext] (canonical)
+        and either aux, host columns [aux_width, n, ext], or aux_build, a build description the device runs. Returns a dict:
+        kind, index, step, column (the first violation, VALID when none), first_failing_step (per transition constraint, main
+        then aux; None where it never fails), expected_degrees / actual_degrees (lists, or None without check_degrees), msg."""
+        d_, dp = _u64(desc)
+        ptrs, dev = None, None
+        if isinstance(trace, int):
+            if n is None:
+                raise ValueError("n is required with a device trace pointer")
+            dev = vp(trace)
+        else:
+            a = np.ascontiguousarray(trace, dtype=np.uint64)
+            c, n = a.shape
+            ptrs = (u64p * c)(*[a[j].ctypes.data_as(u64p) for j in range(c)])
+        rp = aps = bp = None
+        bl = 0
+        if rand is not None:
+            r_, rp = _u64(np.asarray(rand, dtype=np.uint64).reshape(-1))
+        if aux is not None:
+            x_ = np.ascontiguousarray(aux, dtype=np.uint64)
+            aps = (u64p * x_.shape[0])(*[x_[j].ctypes.data_as(u64p) for j in range(x_.shape[0])])
+        if aux_build is not None:
+            b_, bp = _u64(aux_build)
+            bl = b_.size
+        cap = 1 + len(desc)   # constraint counts are bounded by the description's length
+        first, exp, act = (np.zeros(cap, dtype=np.uint64) for _ in range(3))
+        rep = Validation()
+        msg = C.create_string_buffer(1 << 16)
+        self.check(self.L.wf_trace_validate(self.h, dp, d_.size, bp, bl, aps, ptrs, dev, int(mont), rp, int(n).bit_length() - 1, ext,
+                                            int(check_degrees), C.byref(rep), first.ctypes.data_as(u64p), exp.ctypes.data_as(u64p),
+                                            act.ctypes.data_as(u64p), msg, 1 << 16))
+        k = rep.num_transition_constraints
+        return {"kind": rep.kind, "index": rep.index, "step": rep.step, "column": rep.column,
+                "first_failing_step": [None if int(v) == 2**64 - 1 else int(v) for v in first[:k]],
+                "expected_degrees": [int(v) for v in exp[:k]] if check_degrees else None,
+                "actual_degrees": [int(v) for v in act[:k]] if check_degrees else None,
+                "msg": msg.value.decode(errors="replace")}
+
+    def set_validation(self, on):
+        """The analogue of a debug build (default off): the proving entry points and eval_constraints check the trace against
+        its AIR and refuse a violation with the reference's panic message."""
+        self.check(self.L.wf_ctx_set_validation(self.h, int(on)))
 
     def prove_fib_dev(self, d_trace, k, log_n, results, opts, out_buf=None):
         """trace resident on the device: column-major [2k][n] at raw pointer d_trace."""

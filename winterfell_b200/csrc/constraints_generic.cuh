@@ -78,6 +78,39 @@ template <int D> __device__ __forceinline__ void wf_jit_main(u64* r, const GenEv
 template <int D> __device__ __forceinline__ void wf_jit_aux(GlExt<D>* ra, const GenEvalParams& p, GlExt<D>& T);
 #endif
 
+#ifndef WF_JIT
+// The two transition programs, interpreted over the register files r (base field) and ra (E) laid out as above. Every
+// OUT j, v hands register v to out(j, value): the combining kernel weighs it with constraint j's coefficient, the checks of
+// validate.cu sum and test it or write it to constraint j's column. A constraint may have several OUT instructions; its value
+// is the sum of all of them.
+template <class Out>
+__device__ __forceinline__ void run_main_program(const GenEvalParams& p, u64* r, Out out) {
+    for (u32 k = 0; k < p.prog_len; k++) {
+        const u32 op = p.prog[4 * k], dst = p.prog[4 * k + 1], a = p.prog[4 * k + 2], b = p.prog[4 * k + 3];
+        switch (op) {
+            case 0: r[dst] = gl_add(r[a], r[b]); break;
+            case 1: r[dst] = gl_sub(r[a], r[b]); break;
+            case 2: r[dst] = gl_mul(r[a], r[b]); break;
+            case 3: r[dst] = p.consts[a]; break;
+            default: out(dst, r[a]); break;  // OUT
+        }
+    }
+}
+template <int D, class Out>
+__device__ __forceinline__ void run_aux_program(const GenEvalParams& p, GlExt<D>* ra, Out out) {
+    for (u32 k = 0; k < p.aprog_len; k++) {
+        const u32 op = p.aprog[4 * k], dst = p.aprog[4 * k + 1], a = p.aprog[4 * k + 2], b = p.aprog[4 * k + 3];
+        switch (op) {
+            case 0: ra[dst] = ext_add(ra[a], ra[b]); break;
+            case 1: ra[dst] = ext_sub(ra[a], ra[b]); break;
+            case 2: ra[dst] = ext_mul(ra[a], ra[b]); break;
+            case 3: ra[dst] = ext_from_base<D>(p.consts[a]); break;
+            default: out(dst, ra[a]); break;  // OUT
+        }
+    }
+}
+#endif
+
 template <int D, bool AUX>
 __device__ __forceinline__ void generic_constraints_row(const GenEvalParams& p) {
     const size_t ce = (size_t)1 << (p.log_n + p.log_ce_blowup);
@@ -123,16 +156,7 @@ __device__ __forceinline__ void generic_constraints_row(const GenEvalParams& p) 
     u64 r[GEN_MAX_REGS];
     for (u32 c = 0; c < p.w; c++) { r[c] = seg_at(p.lde, ls, c); r[p.w + c] = seg_at(p.lde, nx, c); }
     for (u32 j = 0; j < p.num_periodic; j++) r[2 * p.w + j] = p.ptab[p.ptab_off[j] + (u32)(i & (p.ptab_len[j] - 1))];
-    for (u32 k = 0; k < p.prog_len; k++) {
-        const u32 op = p.prog[4 * k], dst = p.prog[4 * k + 1], a = p.prog[4 * k + 2], b = p.prog[4 * k + 3];
-        switch (op) {
-            case 0: r[dst] = gl_add(r[a], r[b]); break;
-            case 1: r[dst] = gl_sub(r[a], r[b]); break;
-            case 2: r[dst] = gl_mul(r[a], r[b]); break;
-            case 3: r[dst] = p.consts[a]; break;
-            default: T = ext_add(T, ext_mul_base(ld_ext<D>(p.tcoef + (size_t)dst * D), r[a])); break;  // OUT
-        }
-    }
+    run_main_program(p, r, [&](u32 j, u64 v) { T = ext_add(T, ext_mul_base(ld_ext<D>(p.tcoef + (size_t)j * D), v)); });
     GlExt<D> ra[AUX ? AUX_MAX_REGS : 1];
     if constexpr (AUX) {  // evaluator/default.rs:306-341 evaluate_aux_transition
         for (u32 c = 0; c < 2 * p.w; c++) ra[c] = ext_from_base<D>(r[c]);
@@ -146,16 +170,7 @@ __device__ __forceinline__ void generic_constraints_row(const GenEvalParams& p) 
         const u32 pb = 2 * p.w + 2 * p.aw;
         for (u32 j = 0; j < p.num_periodic; j++) ra[pb + j] = ext_from_base<D>(r[2 * p.w + j]);
         for (u32 j = 0; j < p.nr; j++) ra[pb + p.num_periodic + j] = ld_ext<D>(p.rnd + (size_t)j * D);
-        for (u32 k = 0; k < p.aprog_len; k++) {
-            const u32 op = p.aprog[4 * k], dst = p.aprog[4 * k + 1], a = p.aprog[4 * k + 2], b = p.aprog[4 * k + 3];
-            switch (op) {
-                case 0: ra[dst] = ext_add(ra[a], ra[b]); break;
-                case 1: ra[dst] = ext_sub(ra[a], ra[b]); break;
-                case 2: ra[dst] = ext_mul(ra[a], ra[b]); break;
-                case 3: ra[dst] = ext_from_base<D>(p.consts[a]); break;
-                default: T = ext_add(T, ext_mul(ra[a], ld_ext<D>(p.atcoef + (size_t)dst * D))); break;  // OUT
-            }
-        }
+        run_aux_program<D>(p, ra, [&](u32 j, const GlExt<D>& v) { T = ext_add(T, ext_mul(v, ld_ext<D>(p.atcoef + (size_t)j * D))); });
     }
 #define WF_MAIN_CUR(col) r[col]
 #define WF_AUX_CUR(col) ra[2 * p.w + (col)]

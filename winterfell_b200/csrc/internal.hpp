@@ -47,6 +47,7 @@ struct wf_ctx {
     // constraint kernels compiled per AIR (jit.cu): generated source -> (cudaLibrary_t, cudaKernel_t); (null, null) = failed
     std::map<std::string, std::pair<void*, void*>> jit_cache;
     bool jit_enabled = true;
+    bool validate = false;                   // wf_ctx_set_validation: the reference's debug-build trace checks in the provers
     uint64_t jit_compiled = 0, jit_hits = 0, jit_fallbacks = 0;
     bool profiling;                          // record a CUDA event at every pipeline stage boundary
     std::vector<std::pair<std::string, cudaEvent_t>> marks;

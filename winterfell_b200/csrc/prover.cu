@@ -28,6 +28,7 @@
 #include <chrono>
 
 #include "internal.hpp"
+#include "air_host.hpp"
 #include "blake3.cuh"
 #include "alg_hash.cuh"
 
@@ -723,71 +724,6 @@ struct Options {
     }
 };
 
-// Host-side AIR description (mirrors oracle/wf_prover.cpp `Air`; flat format documented at
-// wf_prove_air in include/winterfell_b200.h)
-// stride 0: Assertion::single; one value + stride: ::periodic; n / stride values: ::sequence
-// (air/src/air/assertions/mod.rs:62-120). Main values: one word each; aux values: three words each.
-struct AirAssertion { u64 column, first_step, stride; std::vector<u64> values; };
-typedef AirAssertion AuxAssertion;
-struct AirHost {
-    u32 w = 0;
-    // auxiliary segment (air/src/air/trace_info.rs:24-40): aw columns over E, nr random elements
-    u32 aw = 0, nr = 0, aux_num_regs = 0;
-    std::vector<std::pair<u32, std::vector<u32>>> aux_degrees;
-    std::vector<u32> aux_prog;
-    std::vector<AuxAssertion> aux_asserts;
-    std::vector<std::pair<u32, std::vector<u32>>> all_degrees() const {  // context.rs:268-271
-        auto r = degrees; r.insert(r.end(), aux_degrees.begin(), aux_degrees.end()); return r;
-    }
-    std::vector<u64> pub_inputs;
-    std::vector<std::pair<u32, std::vector<u32>>> degrees;
-    std::vector<std::vector<u64>> periodic;
-    std::vector<u64> consts;
-    std::vector<u32> prog;  // 4 words per instruction
-    u32 num_regs = 0;
-    std::vector<AirAssertion> asserts;
-    u32 exemptions = 1;
-    bool is_fib = false;  // FibSmall x k: use the specialised kernel
-    u32 fib_k = 0;
-    std::vector<u64> fib_results;
-    u32 log_ce_blowup() const {  // air/src/air/context.rs:87-100, transition/degree.rs min_blowup_factor
-        u32 r = 1;
-        for (auto& dg : all_degrees()) {
-            u32 bound = dg.first + (u32)dg.second.size() - 1, l = 0;
-            while ((1u << l) < bound) l++;
-            r = std::max(r, std::max(l, 1u));
-        }
-        return r;
-    }
-    u32 num_comp_cols(size_t n) const {  // context.rs:265-285
-        size_t hi = 0;
-        for (auto& dg : all_degrees()) {
-            size_t e = (size_t)dg.first * (n - 1);
-            for (u32 cyc : dg.second) e += (n / cyc) * (cyc - 1);
-            hi = std::max(hi, e);
-        }
-        size_t div = n - exemptions;
-        return (u32)std::max((hi - div + n - 1) / n, (size_t)1);
-    }
-    std::vector<AuxAssertion> sorted_aux_assertions() const {
-        std::vector<AuxAssertion> a = aux_asserts;
-        std::stable_sort(a.begin(), a.end(), [](const AuxAssertion& x, const AuxAssertion& y) {
-            if (x.stride != y.stride) return x.stride < y.stride;
-            if (x.first_step != y.first_step) return x.first_step < y.first_step;
-            return x.column < y.column;
-        });
-        return a;
-    }
-    std::vector<AirAssertion> sorted_assertions() const {  // assertions/mod.rs:301-315
-        std::vector<AirAssertion> a = asserts;
-        std::stable_sort(a.begin(), a.end(), [](const AirAssertion& x, const AirAssertion& y) {
-            if (x.stride != y.stride) return x.stride < y.stride;
-            if (x.first_step != y.first_step) return x.first_step < y.first_step;
-            return x.column < y.column;
-        });
-        return a;
-    }
-};
 static AirHost fib_air_host(u32 k, size_t n, const u64* results) {
     AirHost a;
     a.w = 2 * k;
@@ -1143,15 +1079,7 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
         // periodic value tables (evaluator/periodic_table.rs:24-76): poly_j over offset^(n/L) <w_(L*ceb)>
         std::vector<u64> ptab;
         std::vector<u32> poff, plen;
-        for (auto& col : air.periodic) {
-            const size_t L = col.size(), M = L << log_ceb;
-            std::vector<u64> v = col;
-            wf_host_dft(v, L, 1, true, 1);              // get_periodic_column_polys (air/mod.rs:325-360)
-            v.resize(M, 0);
-            wf_host_dft(v, M, 1, false, gl_pow(GL_GENERATOR, n / L));
-            poff.push_back((u32)ptab.size()); plen.push_back((u32)M);
-            ptab.insert(ptab.end(), v.begin(), v.end());
-        }
+        air.periodic_ce_tables(n, log_ceb, ptab, poff, plen);
         CKI(upload(ptab.data(), ptab.size() * 8, &dp)); p.ptab = (u64*)dp;
         CKI(upload(poff.data(), poff.size() * 4, &dp)); p.ptab_off = (u32*)dp;
         CKI(upload(plen.data(), plen.size() * 4, &dp)); p.ptab_len = (u32*)dp;
@@ -1387,6 +1315,12 @@ int deep_compose_polys(wf_ctx* ctx, const wf_mat* polys, const wf_mat* apolys, c
     return r;
 }
 
+// wf_ctx_set_validation: a violation found by a check stops the call with the reference's panic message
+static int validation_result(wf_ctx* ctx, int r, const TraceReport& rep) {
+    if (r != WF_OK) return r;
+    return rep.kind == WF_VALID ? WF_OK : wf_fail(ctx, WF_ERR_INVALID, "%s", rep.msg.c_str());
+}
+
 // Device objects of one proof: whatever is still registered when prove_air leaves (normally or through
 // an error return) goes back to the context's pool.
 struct ProofScope {
@@ -1422,6 +1356,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     const u32 n_mtr = (u32)air.degrees.size(), n_mas = (u32)air.asserts.size();
     const u32 n_tr = n_mtr + n_atr, n_as = n_mas + n_aas;  // context.rs:205-207, :223-225
     if (aw && !aux_builder && !aux_build) return wf_fail(ctx, WF_ERR_INVALID, "multi-segment AIR needs an aux trace builder");
+    const bool validate = ctx->validate && !air.is_fib;   // wf_ctx_set_validation; the FibSmall path is not checked
     if (log_ceb > log_b) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
     for (auto& col : air.periodic) if (col.size() > n) return wf_fail(ctx, WF_ERR_INVALID, "periodic column longer than the trace");
     CKI(validate_degrees(ctx, air.all_degrees(), n));
@@ -1450,7 +1385,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
         CKI(wf_mat_from_device_columns(ctx, d_trace, c, n, &trace));
         wf_mark(ctx, "trace_upload_layout");
         CKI(wf_mat_interpolate(ctx, trace, &polys));
-        if (!aux_build) scope.drop(trace);   // else: the evaluations the aux build reads
+        if (!aux_build && !validate) scope.drop(trace);   // else: the evaluations the aux build or the trace check reads
         wf_mark(ctx, "trace_interpolate");
         CKI(wf_mat_lde(ctx, polys, log_b, &lde));
     } else {
@@ -1477,7 +1412,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
             // polynomials for a host trace (its pipelined upload + LDE never materialises the layouted trace)
             if (!trace) CKI(wf_mat_evaluate(ctx, polys, &trace));
             CKI(wf_aux_build_run(ctx, *aux_build, trace, c, air.periodic, rnd_flat.data(), air.nr, D, &atrace));
-            scope.drop(trace);
+            if (!validate) scope.drop(trace);
             wf_mark(ctx, "aux_build");
         } else {
             aux_host.resize((size_t)aw * n * D);
@@ -1509,12 +1444,19 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
             CKI(wf_mat_from_host_columns(ctx, cols.data(), aw, n, D, mont, &atrace));
         }
         CKI(wf_mat_interpolate(ctx, atrace, &apolys));
-        scope.drop(atrace);
+        if (!validate) scope.drop(atrace);
         CKI(wf_mat_lde(ctx, apolys, log_b, &alde));
         CKI(wf_commit_rows_partitioned(ctx, h, alde, o.part_words(aw, D), &atree));
         CKI(wf_tree_root(ctx, atree, root));
         wf_mark(ctx, "aux_commit");
         ch.commit(root);
+    }
+    if (validate) {   // Trace::validate (lib.rs:355-356): the aux segment and its assertion values are final
+        if (!trace) CKI(wf_mat_evaluate(ctx, polys, &trace));
+        TraceReport rep;
+        CKI(validation_result(ctx, wf_check_trace(ctx, air, trace, atrace, rnd_flat.data(), log_n, D, rep), rep));
+        scope.drop(trace);
+        scope.drop(atrace);
     }
 
     // ---- 2. constraint evaluation (lib.rs:373-378) ----
@@ -1522,6 +1464,10 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     // aux assertions (boundary/mod.rs:108-110)
     std::vector<GlExt<D>> cc = ch.draw_coeffs(o.batch_c, n_tr + n_as);
     CKI(eval_constraints<D>(ctx, air, lde, alde, cc, rnd_flat, log_n, log_b, &comp));
+    if (validate) {   // validate_transition_degrees (evaluator/default.rs:114) on the prover's own LDEs
+        TraceReport rep;
+        CKI(validation_result(ctx, wf_check_degrees(ctx, air, lde, alde, rnd_flat.data(), log_n, log_b, D, rep), rep));
+    }
     wf_mark(ctx, "constraint_eval");
     // ---- 3. composition polynomial + commitment (lib.rs:527-552) ----
     CKI(composition_commit(ctx, h, comp, log_n, log_b, D, kc, &cpolys, &clde, &ctree, o.part_words(kc, D)));
@@ -2472,6 +2418,67 @@ extern "C" int wf_prove_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* c
     return WF_OK;
 }
 
+// ---- the reference's debug-build checks of a trace (validate.cu), standalone ----
+extern "C" int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len,
+                                 const uint64_t* const* aux_cols, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont,
+                                 const uint64_t* rand, uint32_t log_n, uint32_t ext, int check_degrees, wf_validation* report,
+                                 uint64_t* first_failing_step, uint64_t* expected_degrees, uint64_t* actual_degrees, char* msg, size_t msg_cap) {
+    if (msg && msg_cap) msg[0] = 0;
+    if (!ctx || !air_desc || !report || log_n < 3 || log_n > 30 || ext < 1 || ext > 3) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    if (!trace_cols == !d_trace) return wf_fail(ctx, WF_ERR_INVALID, "pass exactly one of trace_cols (host) and d_trace (device)");
+    AirHost air;
+    if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
+    const u32 log_ceb = air.log_ce_blowup();
+    CKI(air_check_host(ctx, air, log_n, 1u << log_ceb));
+    AuxBuildHost b;
+    if (air.aw) {
+        if (!aux_build == !aux_cols) return wf_fail(ctx, WF_ERR_INVALID, "two-segment AIR: pass exactly one of aux_build and aux_cols");
+        if (air.nr && !rand) return wf_fail(ctx, WF_ERR_INVALID, "random elements missing");
+        if (aux_build) {
+            CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
+            for (auto& col : b.cols)
+                for (u32 q = ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
+        }
+    } else if (aux_build || aux_cols) {
+        return wf_fail(ctx, WF_ERR_INVALID, "single-segment AIR: it has no aux segment");
+    }
+    const size_t n = (size_t)1 << log_n;
+    const u32 c = air.w, n_tr = (u32)(air.degrees.size() + (air.aw ? air.aux_degrees.size() : 0));
+    const std::vector<u64> rnd(rand, rand + (air.aw ? (size_t)air.nr * ext : 0));
+    wf_mat *trace = nullptr, *atrace = nullptr, *polys = nullptr, *apolys = nullptr, *lde = nullptr, *alde = nullptr;
+    ProofScope scope(ctx);
+    scope.own({&trace, &atrace, &polys, &apolys, &lde, &alde});
+    if (d_trace) CKI(wf_mat_from_device_columns(ctx, d_trace, c, n, &trace));
+    else CKI(wf_mat_from_host_columns(ctx, trace_cols, c, n, 1, mont, &trace));
+    if (air.aw) {
+        if (aux_build) CKI(wf_aux_build_run(ctx, b, trace, c, air.periodic, rnd.data(), air.nr, (int)ext, &atrace));
+        else CKI(wf_mat_from_host_columns(ctx, aux_cols, air.aw, n, (int)ext, mont, &atrace));
+    }
+    TraceReport rep;
+    CKI(wf_check_trace(ctx, air, trace, atrace, rnd.data(), log_n, (int)ext, rep));
+    if (check_degrees) {
+        // the CE domain's frames from LDEs at the constraint evaluation blowup: the frame stride is 1 * ce_blowup
+        CKI(wf_mat_interpolate(ctx, trace, &polys));
+        scope.drop(trace);
+        CKI(wf_mat_lde(ctx, polys, log_ceb, &lde));
+        scope.drop(polys);
+        if (atrace) {
+            CKI(wf_mat_interpolate(ctx, atrace, &apolys));
+            scope.drop(atrace);
+            CKI(wf_mat_lde(ctx, apolys, log_ceb, &alde));
+            scope.drop(apolys);
+        }
+        CKI(wf_check_degrees(ctx, air, lde, alde, rnd.data(), log_n, log_ceb, (int)ext, rep));
+    }
+    report->kind = rep.kind; report->index = rep.index; report->step = rep.step; report->column = rep.column;
+    report->num_transition_constraints = n_tr;
+    if (first_failing_step) std::copy(rep.first_fail.begin(), rep.first_fail.end(), first_failing_step);
+    if (check_degrees && expected_degrees) std::copy(rep.expected.begin(), rep.expected.end(), expected_degrees);
+    if (check_degrees && actual_degrees) std::copy(rep.actual.begin(), rep.actual.end(), actual_degrees);
+    if (msg && msg_cap) { strncpy(msg, rep.msg.c_str(), msg_cap - 1); msg[msg_cap - 1] = 0; }
+    return WF_OK;
+}
+
 // ---- stepwise exports: the seams of prover/src/lib.rs:125-223 (ConstraintEvaluator, ConstraintCommitment)
 //      and the concrete steps between them, for a host that keeps the transcript itself ----------------
 template <int D>
@@ -2482,7 +2489,13 @@ static int eval_constraints_entry(wf_ctx* ctx, const AirHost& air, u32 log_n, u3
     for (size_t i = 0; i < ncc; i++) for (int q = 0; q < D; q++) cc[i].v[q] = coeffs[i * D + q];
     std::vector<u64> rnd;
     if (air.aw) rnd.assign(aux_rand, aux_rand + (size_t)air.nr * D);
-    return eval_constraints<D>(ctx, air, lde, alde, cc, rnd, log_n, log_b, out);
+    CKI(eval_constraints<D>(ctx, air, lde, alde, cc, rnd, log_n, log_b, out));
+    if (ctx->validate) {   // validate_transition_degrees, as evaluator/default.rs:114 runs it after the evaluation
+        TraceReport rep;
+        const int r = validation_result(ctx, wf_check_degrees(ctx, air, lde, alde, rnd.data(), log_n, log_b, D, rep), rep);
+        if (r != WF_OK) { wf_mat_free(ctx, *out); *out = nullptr; return r; }
+    }
+    return WF_OK;
 }
 extern "C" int wf_eval_constraints(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup,
                                    uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs,
