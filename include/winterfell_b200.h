@@ -280,6 +280,38 @@ int wf_prove_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_d
 int wf_air_batch_check(uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens, uint32_t log_n, uint32_t blowup,
                        char* msg, size_t msg_cap);
 
+/* ---- verifying a batch of proofs of one AIR (verifier::verify, verifier/src/lib.rs:82-147) ---------------------------------
+ * verdicts[j] is the FIRST check proof j fails, in the reference's order (the code numbers are not that order: CONTEXT comes
+ * first). A refused proof is a result: the call returns WF_OK whenever verdicts were written. */
+#define WF_VERIFY_ACCEPT               0
+#define WF_VERIFY_MALFORMED            1   /* ProofDeserializationError; the ranges ProofOptions::new / TraceInfo::read_from assert */
+#define WF_VERIFY_OOD                  2   /* InconsistentOodConstraintEvaluations */
+#define WF_VERIFY_POW                  3   /* QuerySeedProofOfWorkVerificationFailed */
+#define WF_VERIFY_TRACE_QUERY          4   /* TraceQueryDoesNotMatchCommitment (main or aux) */
+#define WF_VERIFY_CONSTRAINT_QUERY     5   /* ConstraintQueryDoesNotMatchCommitment */
+#define WF_VERIFY_FRI_LAYER            6   /* FriVerificationFailed(LayerCommitmentMismatch) */
+#define WF_VERIFY_FRI_FOLD             7   /* FriVerificationFailed(InvalidLayerFolding) */
+#define WF_VERIFY_FRI_REMAINDER        8   /* FriVerificationFailed(InvalidRemainderFolding / RemainderDegreeMismatch) */
+#define WF_VERIFY_CONTEXT              9   /* the proof's context does not fit the AIR (InconsistentBaseField, widths, constraint count) */
+#define WF_VERIFY_UNACCEPTABLE_OPTIONS 10  /* AcceptableOptions::OptionSet refused the proof's options */
+/* Air::get_aux_assertions(aux_rand_elements) of proof `proof` (its index in the batch): rand_elements [nr][ext], values
+ * [number of aux assertion values][ext], in: the description's values, out: the values to assert. Non-zero = failure. */
+typedef int (*wf_aux_assertions_batch_fn)(void* user, uint32_t proof, const uint64_t* rand_elements, uint64_t* values);
+/* air_descs[j]: the flat description of wf_prove_air / wf_prove_air_aux with proof j's public inputs and assertion values; all
+ * must share the structure of air_descs[0] (the rule of wf_air_batch_check). The trace length is not part of that structure: it
+ * is read from each proof, and a proof whose declared length the AIR does not fit (wf_air_check, the n / stride values of a
+ * sequence assertion) gets WF_VERIFY_CONTEXT. hash_id selects the hasher. acceptable_opts: NULL accepts the options the proof
+ * carries; else num_acceptable opts[9] vectors of the proving entry points (AcceptableOptions::OptionSet, compared on words
+ * 0-7 and the partition bytes of word 8; the hash byte must be hash_id), checked before anything else. aux_assertions
+ * (may be NULL): called on the host once per proof that reaches Air::get_aux_assertions, with its index. WF_ERR_INVALID for
+ * caller errors (NULL pointers, a description that does not parse or breaks the batch rule, a failing callback), naming the
+ * proof; no device buffer stays live after any return. The surviving proofs are checked on the device together: the number
+ * of kernel launches does not depend on `batch` for proofs of one shape. */
+int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
+                        const uint8_t* const* proofs, const size_t* proof_lens, int hash_id,
+                        const uint32_t* acceptable_opts, uint32_t num_acceptable,
+                        wf_aux_assertions_batch_fn aux_assertions, void* aux_user, uint32_t* verdicts);
+
 /* ---- checking a trace against its AIR: the reference's debug builds (Trace::validate, prover/src/trace/mod.rs:86-201;
  *      ConstraintEvaluationTable::validate_transition_degrees, prover/src/constraints/evaluation_table.rs:181-230) ----------
  * Trace check: every main assertion (description order, each one's steps increasing), then every aux assertion (values in E:

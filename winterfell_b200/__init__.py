@@ -29,6 +29,11 @@ vp = C.c_void_p
 FRI_COMMIT_FN = C.CFUNCTYPE(None, C.c_void_p, u8p)
 FRI_DRAW_FN = C.CFUNCTYPE(None, C.c_void_p, u64p)
 AUX_BUILDER = C.CFUNCTYPE(C.c_int, C.c_void_p, u64p, u64p)
+AUX_ASSERTIONS_BATCH = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, u64p, u64p)
+
+# wf_verify_air_batch verdicts (include/winterfell_b200.h WF_VERIFY_*)
+VERIFY_ACCEPT, VERIFY_MALFORMED, VERIFY_OOD, VERIFY_POW, VERIFY_TRACE_QUERY, VERIFY_CONSTRAINT_QUERY, VERIFY_FRI_LAYER, \
+    VERIFY_FRI_FOLD, VERIFY_FRI_REMAINDER, VERIFY_CONTEXT, VERIFY_UNACCEPTABLE_OPTIONS = range(11)
 
 # wf_validation (include/winterfell_b200.h): the first violation wf_trace_validate found, in the reference's order
 VALID, VIOLATION_MAIN_ASSERTION, VIOLATION_AUX_ASSERTION, VIOLATION_MAIN_TRANSITION, VIOLATION_AUX_TRANSITION, VIOLATION_DEGREES, \
@@ -118,6 +123,8 @@ _SIGS = [
                                     C.c_uint32, C.c_int, C.POINTER(Validation), u64p, u64p, u64p, C.c_char_p, C.c_size_t]),
     ("wf_ctx_set_validation", C.c_int, [vp, C.c_int]),
     ("wf_air_batch_check", C.c_int, [C.c_uint32, C.POINTER(u64p), C.POINTER(C.c_size_t), C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]),
+    ("wf_verify_air_batch", C.c_int, [vp, C.c_uint32, C.POINTER(u64p), C.POINTER(C.c_size_t), C.POINTER(u8p), C.POINTER(C.c_size_t), C.c_int,
+                                      C.POINTER(C.c_uint32), C.c_uint32, AUX_ASSERTIONS_BATCH, vp, C.POINTER(C.c_uint32)]),
     ("wf_host_hash_elements", C.c_int, [C.c_int, u64p, C.c_size_t, u8p]),
     ("wf_host_merge", C.c_int, [C.c_int, u8p, u8p]),
     ("wf_host_merge_with_int", C.c_int, [C.c_int, u8p, C.c_uint64, u8p]),
@@ -490,6 +497,45 @@ class Context:
                                              o_.ctypes.data_as(C.POINTER(C.c_uint32)), outs, lens))
         return [buf[j, : lens[j]].tobytes() for j in range(batch)]
 
+    def verify_air_batch(self, descs, proofs, hash_id, acceptable=None, aux_values_fn=None):
+        """wf_verify_air_batch: the verdict (VERIFY_*) of each proof in `proofs` (bytes) against the description of the same
+        index in `descs` (one AIR structure). acceptable: None (accept the options a proof carries) or a list of opts[9] arrays.
+        aux_values_fn(j, rand [nr, d], values [nv, d]) -> values: Air::get_aux_assertions of proof j. Returns a uint32 array."""
+        ds = [np.ascontiguousarray(d, dtype=np.uint64) for d in descs]
+        ps = [np.frombuffer(p, dtype=np.uint8) if len(p) else np.zeros(1, dtype=np.uint8) for p in proofs]
+        batch = len(ds)
+        if len(ps) != batch:
+            raise ValueError("one proof per description")
+        dps = (u64p * batch)(*[d.ctypes.data_as(u64p) for d in ds])
+        dls = (C.c_size_t * batch)(*[d.size for d in ds])
+        pps = (u8p * batch)(*[p.ctypes.data_as(u8p) for p in ps])
+        pls = (C.c_size_t * batch)(*[len(p) for p in proofs])
+        acc, accp, nacc = None, None, 0
+        if acceptable is not None:
+            acc = np.ascontiguousarray(np.stack([np.asarray(a, dtype=np.uint32) for a in acceptable]), dtype=np.uint32)
+            accp, nacc = acc.ctypes.data_as(C.POINTER(C.c_uint32)), acc.shape[0]
+        cb = AUX_ASSERTIONS_BATCH()
+        if aux_values_fn is not None:
+            nv = _aux_value_count(ds[0])
+
+            def cb_values(_user, j, rand_p, val_p):
+                try:
+                    p = bytes(proofs[j])
+                    d = p[6 + (p[4] | p[5] << 8) + 9 + 3]   # ProofOptions::field_extension, after the trace info and modulus
+                    rand = np.ctypeslib.as_array(rand_p, shape=(p[2], d)).copy()
+                    vals = np.ctypeslib.as_array(val_p, shape=(nv, d))
+                    vals[:] = np.ascontiguousarray(aux_values_fn(j, rand, vals.copy()), dtype=np.uint64).reshape(nv, d)
+                    return 0
+                except Exception:  # must not unwind through the C caller
+                    import traceback
+                    traceback.print_exc()
+                    return 1
+            cb = AUX_ASSERTIONS_BATCH(cb_values)
+        out = np.zeros(batch, dtype=np.uint32)
+        self.check(self.L.wf_verify_air_batch(self.h, batch, dps, dls, pps, pls, int(hash_id), accp, nacc, cb, None,
+                                              out.ctypes.data_as(C.POINTER(C.c_uint32))))
+        return out
+
     def trace_validate(self, desc, trace, ext=1, rand=None, aux=None, aux_build=None, n=None, mont=False, check_degrees=True):
         """wf_trace_validate: checks a trace against its AIR as the reference's debug builds do (Trace::validate, then
         validate_transition_degrees when check_degrees). trace: [width, n] uint64 host array, or an integer device pointer to
@@ -767,6 +813,41 @@ def air_check(desc, log_n, blowup):
     msg = C.create_string_buffer(512)
     rc = lib().wf_air_check(dp, d_.size, log_n, blowup, msg, 512)
     return rc, msg.value.decode(errors="replace")
+
+
+def _aux_value_count(desc):
+    """Number of aux assertion values of a flat AIR description (format at wf_prove_air in include/winterfell_b200.h)."""
+    d = [int(x) for x in desc]
+    p = 1
+    def skip_degrees(p):
+        cnt = d[p]; p += 1
+        for _ in range(cnt):
+            p += 2 + d[p + 1]
+        return p
+    p = skip_degrees(p)
+    cnt = d[p]; p += 1
+    for _ in range(cnt):
+        p += 1 + d[p]
+    p += 1 + d[p]                       # constants
+    p += 1                              # num_regs
+    p += 1 + 4 * d[p]                   # program
+    cnt = d[p]; p += 1
+    for _ in range(cnt):
+        p += 4 + d[p + 3]
+    p += 1 + d[p]                       # public inputs
+    p += 1                              # exemptions
+    if p == len(d):
+        return 0
+    p += 2                              # aux width, random elements
+    p = skip_degrees(p)
+    p += 1                              # aux num_regs
+    p += 1 + 4 * d[p]
+    cnt = d[p]; p += 1
+    total = 0
+    for _ in range(cnt):
+        total += d[p + 3]
+        p += 4 + 3 * d[p + 3]
+    return total
 
 
 def air_batch_check(descs, log_n, blowup):

@@ -17,7 +17,7 @@ if out != old:
     open("_build/jit_headers.inc", "w").write(out)
 PY
 pids=()
-for f in ntt ntt2 commit fri layout capi prover jit auxbuild validate ${EXTRA_SRCS}; do
+for f in ntt ntt2 commit fri layout capi prover jit auxbuild validate verify ${EXTRA_SRCS}; do
   if [ ! -f _build/$f.o ] || [ csrc/$f.cu -nt _build/$f.o ] || [ -n "$(find csrc include ../include -newer _build/$f.o \( -name '*.cuh' -o -name '*.hpp' -o -name '*.h' -o -name '*.inc' \) 2>/dev/null | head -1)" ]; then
     $NVCC $FLAGS ${PTXAS_V:+-Xptxas -v} -c csrc/$f.cu -o _build/$f.o &
     pids+=($!)

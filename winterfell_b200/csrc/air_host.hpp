@@ -1,7 +1,8 @@
-// air_host.hpp — the host-side form of an AIR description, shared by the prover (prover.cu) and the trace checks
-// (validate.cu).
+// air_host.hpp — the host-side form of an AIR description, shared by the prover (prover.cu), the trace checks
+// (validate.cu) and the verifier (verify.cu).
 #pragma once
 #include "internal.hpp"
+#include "constraints_generic.cuh"  // GEN_MAX_REGS / AUX_MAX_REGS: the register limits a description is parsed against
 
 // Host-side AIR description (mirrors oracle/wf_prover.cpp `Air`; flat format documented at
 // wf_prove_air in include/winterfell_b200.h)
@@ -81,6 +82,202 @@ struct AirHost {
         return a;
     }
 };
+
+// ---- AIR descriptions and proof options, as the prover (prover.cu) and the verifier (verify.cu) read them ----
+struct Options {
+    u32 num_queries, blowup, grinding, ext, folding, rem_max_deg, batch_c, batch_d, num_partitions, hash_rate;
+    int hash_id;
+    // PartitionOptions::partition_size::<E>(num_columns) (air/src/options.rs:428-438) in BASE columns, for `cols` columns of
+    // extension degree `deg`; cols * deg = the row is hashed whole (RowMatrix::commit_to_rows, row_matrix.rs:191-193)
+    u32 part_words(u32 cols, u32 deg) const {
+        if (num_partitions <= 1) return cols * deg;
+        const u32 min_ps = hash_rate / deg, ps = (cols + num_partitions - 1) / num_partitions;
+        return (ps > min_ps ? ps : min_ps) * deg;
+    }
+};
+
+static inline bool parse_air_host(const u64* d, size_t len, AirHost& a) {
+    size_t p = 0;
+    auto rd = [&](u64& v) { if (p >= len) return false; v = d[p++]; return true; };
+    u64 v, cnt;
+    if (!rd(v) || v == 0 || v > 255) return false;
+    a.w = (u32)v;
+    if (!rd(cnt) || cnt == 0 || cnt > 4096) return false;
+    for (u64 i = 0; i < cnt; i++) {
+        u64 base, nc;
+        if (!rd(base) || !rd(nc) || base == 0 || nc > 16) return false;
+        std::vector<u32> cyc;
+        // TransitionConstraintDegree::with_cycles asserts cycle lengths that are powers of two >= 2 (transition/degree.rs:62-79)
+        for (u64 j = 0; j < nc; j++) { if (!rd(v) || v < 2 || (v & (v - 1)) || v > (1ull << 32)) return false; cyc.push_back((u32)v); }
+        if (base + nc - 1 > 128) return false;  // min_blowup_factor would exceed the largest blowup (options.rs:132-190)
+        a.degrees.push_back({(u32)base, cyc});
+    }
+    if (!rd(cnt) || cnt > 64) return false;
+    for (u64 i = 0; i < cnt; i++) {
+        u64 ln;
+        if (!rd(ln) || ln < 2 || (ln & (ln - 1))) return false;
+        std::vector<u64> col;
+        for (u64 j = 0; j < ln; j++) { if (!rd(v) || v >= GL_P) return false; col.push_back(v); }
+        a.periodic.push_back(col);
+    }
+    if (!rd(cnt)) return false;
+    for (u64 i = 0; i < cnt; i++) { if (!rd(v) || v >= GL_P) return false; a.consts.push_back(v); }
+    if (!rd(v) || v > GEN_MAX_REGS || v < 2 * a.w + a.periodic.size()) return false;
+    a.num_regs = (u32)v;
+    if (!rd(cnt) || cnt > (1u << 20)) return false;
+    for (u64 i = 0; i < cnt; i++) {
+        u64 op, ds, x, y;
+        if (!rd(op) || !rd(ds) || !rd(x) || !rd(y) || op > 4) return false;
+        const u64 first_tmp = 2 * a.w + a.periodic.size();  // inputs are read-only: boundary terms re-read them
+        if (op == 4) { if (ds >= a.degrees.size() || x >= a.num_regs) return false; }
+        else if (op == 3) { if (ds >= a.num_regs || ds < first_tmp || x >= a.consts.size()) return false; }
+        else if (ds >= a.num_regs || ds < first_tmp || x >= a.num_regs || y >= a.num_regs) return false;
+        a.prog.insert(a.prog.end(), {(u32)op, (u32)ds, (u32)x, (u32)y});
+    }
+    if (!rd(cnt) || cnt == 0) return false;
+    for (u64 i = 0; i < cnt; i++) {
+        AirAssertion as;
+        u64 nv;
+        if (!rd(as.column) || !rd(as.first_step) || !rd(as.stride) || !rd(nv) || as.column >= a.w || nv == 0 || nv > len) return false;
+        for (u64 j = 0; j < nv; j++) { if (!rd(v) || v >= GL_P) return false; as.values.push_back(v); }
+        a.asserts.push_back(as);
+    }
+    if (!rd(cnt)) return false;
+    for (u64 i = 0; i < cnt; i++) { if (!rd(v) || v >= GL_P) return false; a.pub_inputs.push_back(v); }
+    if (!rd(v) || v == 0 || v > 8) return false;
+    a.exemptions = (u32)v;
+    if (p == len) return true;
+    // optional aux section: [aw, nr, nTa, {base, ncyc, cyc...}*, aux_num_regs, nIa, {op,dst,a,b}*,
+    //                        nAa, {column, first_step, stride, nvals, {v0, v1, v2} x nvals}*]
+    if (!rd(v) || v == 0 || v > 255) return false;
+    a.aw = (u32)v;
+    if (!rd(v) || v > 255) return false;
+    a.nr = (u32)v;
+    if (!rd(cnt) || cnt == 0 || cnt > 4096) return false;   // context.rs:104-113
+    for (u64 i = 0; i < cnt; i++) {
+        u64 base, nc;
+        if (!rd(base) || !rd(nc) || base == 0 || nc > 16) return false;
+        std::vector<u32> cyc;
+        for (u64 j = 0; j < nc; j++) { if (!rd(v) || v < 2 || (v & (v - 1)) || v > (1ull << 32)) return false; cyc.push_back((u32)v); }
+        if (base + nc - 1 > 128) return false;
+        a.aux_degrees.push_back({(u32)base, cyc});
+    }
+    const u64 first_tmp = 2 * a.w + 2 * a.aw + a.periodic.size() + a.nr;
+    if (!rd(v) || v > AUX_MAX_REGS || v < first_tmp) return false;
+    a.aux_num_regs = (u32)v;
+    if (!rd(cnt) || cnt > (1u << 20)) return false;
+    for (u64 i = 0; i < cnt; i++) {
+        u64 op, ds, x, y;
+        if (!rd(op) || !rd(ds) || !rd(x) || !rd(y) || op > 4) return false;
+        if (op == 4) { if (ds >= a.aux_degrees.size() || x >= a.aux_num_regs) return false; }
+        else if (op == 3) { if (ds >= a.aux_num_regs || ds < first_tmp || x >= a.consts.size()) return false; }
+        else if (ds >= a.aux_num_regs || ds < first_tmp || x >= a.aux_num_regs || y >= a.aux_num_regs) return false;
+        a.aux_prog.insert(a.aux_prog.end(), {(u32)op, (u32)ds, (u32)x, (u32)y});
+    }
+    if (!rd(cnt) || cnt == 0) return false;
+    for (u64 i = 0; i < cnt; i++) {
+        AuxAssertion as;
+        u64 nv;
+        if (!rd(as.column) || !rd(as.first_step) || !rd(as.stride) || !rd(nv) || as.column >= a.aw || nv == 0 || nv > len) return false;
+        for (u64 j = 0; j < 3 * nv; j++) { if (!rd(v) || v >= GL_P) return false; as.values.push_back(v); }
+        a.aux_asserts.push_back(as);
+    }
+    return p == len;
+}
+
+// cycle lengths of a TransitionConstraintDegree must not exceed the trace length (get_evaluation_degree,
+// air/src/air/transition/degree.rs:85-97, divides trace_length by each cycle)
+static inline int validate_degrees(wf_ctx* ctx, const std::vector<std::pair<u32, std::vector<u32>>>& degs, size_t n) {
+    for (auto& dg : degs)
+        for (u32 cyc : dg.second)
+            if (cyc < 2 || (cyc & (cyc - 1)) || cyc > n) return wf_fail(ctx, WF_ERR_INVALID, "constraint degree cycle %u does not fit a trace of %zu rows", cyc, n);
+    return WF_OK;
+}
+
+// Assertion validity (air/src/air/assertions/mod.rs:62-120, :166-230 validate_*)
+static inline int validate_assertions(wf_ctx* ctx, const std::vector<AirAssertion>& as, size_t n, size_t words_per_value, const char* what) {
+    for (auto& a : as) {
+        const size_t nv = a.values.size() / words_per_value;
+        bool ok = a.first_step < n && nv >= 1;
+        if (a.stride != 0) ok = ok && a.stride >= 2 && !(a.stride & (a.stride - 1)) && a.stride <= n && a.first_step < a.stride;
+        if (nv > 1) ok = ok && a.stride != 0 && !(nv & (nv - 1)) && nv * a.stride == n;   // sequence: one value per asserted step
+        if (!ok) return wf_fail(ctx, WF_ERR_INVALID, "invalid %s", what);
+    }
+    // no two assertions may cover the same cell (Assertion::overlaps_with, assertions/mod.rs:175-208;
+    // prepare_assertions panics on it, boundary/mod.rs:205-210)
+    auto overlaps = [](const AirAssertion& s, const AirAssertion& o) {
+        if (s.column != o.column) return false;
+        if (s.first_step == o.first_step) return true;
+        if (s.stride == o.stride) return false;
+        const AirAssertion& lo = s.first_step < o.first_step ? s : o;
+        const AirAssertion& hi = s.first_step < o.first_step ? o : s;
+        if (lo.stride == 0) return false;  // the earlier one is a single assertion
+        if (hi.stride == 0 || lo.stride < hi.stride) return (hi.first_step - lo.first_step) % lo.stride == 0;
+        return false;
+    };
+    for (size_t i = 0; i < as.size(); i++)
+        for (size_t j = i + 1; j < as.size(); j++)
+            if (overlaps(as[i], as[j])) return wf_fail(ctx, WF_ERR_INVALID, "%s %zu overlaps with %zu", what, j, i);
+    return WF_OK;
+}
+
+// The checks wf_prove_air / wf_eval_constraints run on an AIR description before touching the device, without a device:
+// structure of the description, degrees against the blowup factor, periodic columns, assertion validity and overlaps
+// (the panics of Air::new / BoundaryConstraints::new / prepare_assertions in the reference, returned as a status).
+static inline int air_check_host(wf_ctx* ctx, const AirHost& air, uint32_t log_n, uint32_t blowup) {
+    u32 log_b = 0;
+    while ((1u << log_b) < blowup) log_b++;
+    const size_t n = (size_t)1 << log_n;
+    if (air.log_ce_blowup() > log_b) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
+    for (auto& col : air.periodic) if (col.size() > n) return wf_fail(ctx, WF_ERR_INVALID, "periodic column longer than the trace");
+    CKI(validate_degrees(ctx, air.all_degrees(), n));
+    CKI(validate_assertions(ctx, air.aux_asserts, n, 3, "aux assertion"));
+    return validate_assertions(ctx, air.asserts, n, 1, "assertion");
+}
+
+// What the descriptions of one batch must share: everything but the public inputs and the assertion values. Returns the first
+// part that differs, nullptr when the two have the same structure.
+static inline const char* air_structure_mismatch(const AirHost& a, const AirHost& b) {
+    // reasons[0..4]: count, columns, steps, strides, value counts
+    auto layout = [](const std::vector<AirAssertion>& x, const std::vector<AirAssertion>& y, const char* const* reasons) -> const char* {
+        if (x.size() != y.size()) return reasons[0];
+        for (size_t i = 0; i < x.size(); i++) {
+            if (x[i].column != y[i].column) return reasons[1];
+            if (x[i].first_step != y[i].first_step) return reasons[2];
+            if (x[i].stride != y[i].stride) return reasons[3];
+            if (x[i].values.size() != y[i].values.size()) return reasons[4];
+        }
+        return nullptr;
+    };
+    static const char* const main_r[] = {"number of assertions", "assertion columns", "assertion steps", "assertion strides",
+                                         "assertion value counts"};
+    static const char* const aux_r[] = {"number of aux assertions", "aux assertion columns", "aux assertion steps",
+                                        "aux assertion strides", "aux assertion value counts"};
+    if (a.w != b.w) return "trace width";
+    if (a.degrees != b.degrees) return "transition constraint degrees";
+    if (a.periodic != b.periodic) return "periodic columns";
+    if (a.consts != b.consts) return "constants";
+    if (a.num_regs != b.num_regs || a.prog != b.prog) return "transition program";
+    if (const char* why = layout(a.asserts, b.asserts, main_r)) return why;
+    if (a.exemptions != b.exemptions) return "transition exemptions";
+    if ((a.aw == 0) != (b.aw == 0)) return "aux segment";
+    if (a.aw != b.aw || a.nr != b.nr) return "aux width or random elements";
+    if (a.aux_degrees != b.aux_degrees) return "aux transition constraint degrees";
+    if (a.aux_num_regs != b.aux_num_regs || a.aux_prog != b.aux_prog) return "aux transition program";
+    return layout(a.aux_asserts, b.aux_asserts, aux_r);
+}
+
+// air/src/air/coefficients.rs:201-218: Linear / Algebraic / Horner batching of the coefficients drawn from the coin
+template <int D>
+static inline std::vector<GlExt<D>> draw_coeffs(PublicCoin& coin, u32 method, size_t n) {
+    auto draw = [&]() { GlExt<D> r = ext_zero<D>(); coin.draw(D, r.v); return r; };
+    std::vector<GlExt<D>> r;
+    if (method == 0) { for (size_t i = 0; i < n; i++) r.push_back(draw()); return r; }
+    GlExt<D> a = draw(), x = ext_from_base<D>(1);
+    for (size_t i = 0; i < n; i++) { r.push_back(x); x = ext_mul(x, a); }
+    if (method == 2) std::reverse(r.begin(), r.end());
+    return r;
+}
 
 // validate.cu: Trace::validate (prover/src/trace/mod.rs:86-201) and ConstraintEvaluationTable::validate_transition_degrees
 // (prover/src/constraints/evaluation_table.rs:181-230, 421-477) on the device. A violation is a result (kind != WF_VALID and

@@ -932,7 +932,7 @@ void wf_open_finish(const OpenPlan& pl, const uint8_t* got, uint8_t* leaves_out,
     }
 }
 
-static int pinned_reserve(wf_ctx* ctx, size_t bytes) {
+int pinned_reserve(wf_ctx* ctx, size_t bytes) {
     if (ctx->pinned_bytes >= bytes) return WF_OK;
     if (ctx->pinned) cudaFreeHost(ctx->pinned);
     ctx->pinned = nullptr;

@@ -296,6 +296,32 @@ __global__ void __launch_bounds__(256) merkle_subtree_kernel(const u64* __restri
     if (m <= 256 && b == 0 && t < 4) nodes[t] = 0;  // nodes[0] = default digest (merkle/mod.rs:349); set by the last launch
 }
 
+// One level of many batch Merkle openings (BatchMerkleProof::get_root, crypto/src/merkle/proofs.rs:110-205) over one digest
+// arena: op i merges arena[ops[i].x] and arena[ops[i].y] into arena[ops[i].z]
+template <int HASH>
+__global__ void __launch_bounds__(128) merkle_merge_ops_kernel(u64* __restrict__ arena, const uint3* __restrict__ ops, u32 count) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const uint3 op = ops[i];
+    u64 in[8], o[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) { in[k] = arena[(size_t)op.x * 4 + k]; in[4 + k] = arena[(size_t)op.y * 4 + k]; }
+    merge_digests<HASH>(in, o);
+#pragma unroll
+    for (int k = 0; k < 4; k++) arena[(size_t)op.z * 4 + k] = o[k];
+}
+
+cudaError_t commit_merge_ops(int hash_id, u64* arena, const uint3* ops, u32 count, cudaStream_t st) {
+    if (count == 0) return cudaSuccess;
+    const unsigned blocks = (count + 127) / 128;
+    if (hash_id == WF_HASH_BLAKE3_256) merkle_merge_ops_kernel<WF_HASH_BLAKE3_256><<<blocks, 128, 0, st>>>(arena, ops, count);
+    else if (hash_id == WF_HASH_BLAKE3_192) merkle_merge_ops_kernel<WF_HASH_BLAKE3_192><<<blocks, 128, 0, st>>>(arena, ops, count);
+    else if (hash_id == WF_HASH_RP64_256) merkle_merge_ops_kernel<WF_HASH_RP64_256><<<blocks, 128, 0, st>>>(arena, ops, count);
+    else if (hash_id == WF_HASH_SHA3_256) merkle_merge_ops_kernel<WF_HASH_SHA3_256><<<blocks, 128, 0, st>>>(arena, ops, count);
+    else merkle_merge_ops_kernel<WF_HASH_RPJIVE64_256><<<blocks, 128, 0, st>>>(arena, ops, count);
+    return cudaGetLastError();
+}
+
 cudaError_t commit_hash_rows(int hash_id, const SegMatrix& m, u64* digests, cudaStream_t st, u32 partition_size) {
     if (m.rows == 0) return cudaSuccess;
     RowSrc src;

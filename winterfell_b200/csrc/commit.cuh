@@ -38,4 +38,6 @@ static inline int seg_width_for(u32 cols) { return cols >= 8 ? 8 : cols > 2 ? 4 
 cudaError_t commit_hash_rows(int hash_id, const SegMatrix& m, u64* digests, cudaStream_t st, u32 partition_size = 0);
 // nodes: nleaves x 4 words; nodes[0] = 0, nodes[1] = root
 cudaError_t commit_merkle_nodes(int hash_id, const u64* leaves, size_t nleaves, u64* nodes, cudaStream_t st);
+// one level of merges over a digest arena (4 words per slot): arena[z] = merge(arena[x], arena[y]) for each op (x, y, z)
+cudaError_t commit_merge_ops(int hash_id, u64* arena, const uint3* ops, u32 count, cudaStream_t st);
 #endif  // !__CUDACC_RTC__

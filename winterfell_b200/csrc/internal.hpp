@@ -107,6 +107,8 @@ static inline void wf_host_dft(std::vector<u64>& v, size_t n, int d, bool invers
 }
 
 int wf_fail(wf_ctx* ctx, int code, const char* fmt, ...);
+// grows the context's pinned staging buffer (ctx->pinned) to at least `bytes`
+int pinned_reserve(wf_ctx* ctx, size_t bytes);
 // jit.cu
 std::string wf_jit_source(int D, u32 w, u32 nper, u32 nregs, const std::vector<u32>& prog, const std::vector<u64>& consts, u32 aw, u32 nr,
                           u32 naregs, const std::vector<u32>& aprog);
