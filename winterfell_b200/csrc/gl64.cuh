@@ -107,20 +107,24 @@ __device__ __forceinline__ u64 gl_add(u64 a, u64 b) {
         : "l"(a), "l"(b));
     return r;
 }
-// (a, b) -> (a + b, a - b), sharing the operand unpacking: 12 ALU instructions.
+// (a, b) -> (a + b, a - b), sharing the operand unpacking. The sum is folded as in gl_reduce128: U = a + b = carry 2^64 + r
+// (U < 2p), U >= p exactly when carry or r + (2^32 - 1) carries (never both), and then U - p = r + (2^32 - 1) mod 2^64, applied
+// by one IMAD.WIDE. The NTT rounds are bound by the integer ALU pipe, and this form moves the sum's work to the FMA pipe: the
+// sum is 5 ALU + 2 FMA-pipe instructions (the gl_add form, a - (p - b), was 7 + 1), the difference 4 + 1 as in gl_sub.
 __device__ __forceinline__ void gl_butterfly(u64& a, u64& b) {
     u64 s, d;
     asm("{\n\t"
-        ".reg .u32 a0, a1, b0, b1, n0, n1, s0, s1, m;\n\t"
+        ".reg .u32 a0, a1, b0, b1, s0, s1, t0, t1, k, m;\n\t"
         "mov.b64 {a0, a1}, %2;\n\t"
         "mov.b64 {b0, b1}, %3;\n\t"
-        "sub.cc.u32 n0, 1, b0;\n\t"
-        "subc.u32 n1, 0xffffffff, b1;\n\t"
-        "sub.cc.u32 s0, a0, n0;\n\t"
-        "subc.cc.u32 s1, a1, n1;\n\t"
-        "subc.u32 m, 0, 0;\n\t"
-        "sub.cc.u32 s0, s0, m;\n\t"
-        "subc.u32 s1, s1, 0;\n\t"
+        "add.cc.u32 s0, a0, b0;\n\t"
+        "addc.cc.u32 s1, a1, b1;\n\t"
+        "addc.u32 k, 0, 0;\n\t"
+        "add.cc.u32 t0, s0, 0xffffffff;\n\t"
+        "addc.cc.u32 t1, s1, 0;\n\t"
+        "addc.u32 k, k, 0;\n\t"
+        "mad.lo.cc.u32 s0, k, " GL_EPSM(4) ", s0;\n\t"
+        "madc.hi.u32 s1, k, " GL_EPSM(4) ", s1;\n\t"
         "mov.b64 %0, {s0, s1};\n\t"
         "sub.cc.u32 a0, a0, b0;\n\t"
         "subc.cc.u32 a1, a1, b1;\n\t"
@@ -130,7 +134,7 @@ __device__ __forceinline__ void gl_butterfly(u64& a, u64& b) {
         "mov.b64 %1, {a0, a1};\n\t"
         "}"
         : "=l"(s), "=l"(d)
-        : "l"(a), "l"(b));
+        : "l"(a), "l"(b) GL_EPS_OPERAND);
     a = s;
     b = d;
 }
@@ -307,7 +311,8 @@ __device__ __forceinline__ u64 gl_sqr_weak(u64 a) {
 //   K < 32      : (y1:y0) + (2^32 - 1) y2                      -> carry * 2^64 + r < 2p, folded as in gl_reduce128 (11 instr.)
 //   32 <= K < 64: 2^32 y0 + (2^32 - 1) y1 - y2 = ((y0:0) - y2, a borrow repaid with -(2^32 - 1)) + (2^32 - 1) y1 -> fold
 //   64 <= K < 96: (2^32 - 1) y0 - (y2:y1) (2^96 = -1, 2^128 = -2^32): below p already, a borrow repaid with -(2^32 - 1):
-//                 canonical without a fold (11 instr.; the first version went through two 128-bit reductions: 45)
+//                 canonical without a fold (9 instr. with (2^32 - 1) y0 as one IMAD.WIDE; the first version went through two
+//                 128-bit reductions: 45)
 template <int K>
 __device__ __forceinline__ u64 gl_shl_dev(u64 x) {
     constexpr int R = K & 31;
@@ -348,8 +353,9 @@ __device__ __forceinline__ u64 gl_shl_dev(u64 x) {
     } else {
         asm("{\n\t"
             ".reg .u32 m0, m1, b;\n\t"
-            "mul.lo.u32 m0, %1, " GL_EPSM(4) ";\n\t"
-            "mul.hi.u32 m1, %1, " GL_EPSM(4) ";\n\t"
+            ".reg .u64 w;\n\t"
+            "mul.wide.u32 w, %1, " GL_EPSM(4) ";\n\t"    // one IMAD.WIDE (mul.lo / mul.hi: IMAD + IMAD.HI)
+            "mov.b64 {m0, m1}, w;\n\t"
             "sub.cc.u32 m0, m0, %2;\n\t"
             "subc.cc.u32 m1, m1, %3;\n\t"
             "subc.u32 b, 0, 0;\n\t"

@@ -56,6 +56,28 @@ __host__ __device__ constexpr u32 swz_const(u32 r) {
     while (x) { h ^= x & ((1u << LK) - 1); x >>= LK; }
     return h;
 }
+// A round reads rows base + Q (Q = q << LOGSPAN, base zero on Q's bits) at (base + Q) ^ hash(base) ^ swz_const(Q). The XOR
+// only reaches the low LK bits, so that row is ((base ^ hash(base)) ^ swz_lo(Q)) + swz_hi(Q): a task holds 2^LK row pointers
+// and every access is one of them plus a compile-time offset (the per-access form cost four integer instructions).
+template <int LK>
+__host__ __device__ constexpr u32 swz_lo(u32 Q) { return swz_const<LK>(Q) ^ (Q & ((1u << LK) - 1)); }
+template <int LK>
+__host__ __device__ constexpr u32 swz_hi(u32 Q) { return Q & ~((1u << LK) - 1); }
+__host__ __device__ constexpr u32 brev_const(u32 v, int bits) {
+    u32 r = 0;
+    for (int i = 0; i < bits; i++) r |= ((v >> i) & 1u) << (bits - 1 - i);
+    return r;
+}
+// Calls f(it, lo, hi) for it = IT .. N - 1, where tile row brev(it STEP) (LOGS bits) sits at row pointer lo plus hi rows: the
+// offsets are compile-time constants in every call.
+template <int LOGS, int LK, u32 STEP, u32 N, u32 IT = 0, class F>
+__device__ __forceinline__ void for_brev_rows(F&& f) {
+    if constexpr (IT < N) {
+        constexpr u32 c = brev_const(IT * STEP, LOGS);
+        f(IT, swz_lo<LK>(c), swz_hi<LK>(c));
+        for_brev_rows<LOGS, LK, STEP, N, IT + 1>(f);
+    }
+}
 template <int LK>
 __device__ __forceinline__ u32 swz_hash(u32 r) {  // r < 2^11
     if (LK == 1) return __popc(r >> 1) & 1;
@@ -118,17 +140,18 @@ __device__ __forceinline__ void tile_round(u64* __restrict__ s, const u64* __res
     constexpr bool LAST = LOGSPAN == 0;
     constexpr u32 TASKS = (1u << LOGS) * LANES / 16;
     if (R == 4) {
-        // radix-16 on one lane
+        // radix-16 on one lane (the task loops stay rolled: unrolled, the 2^11 pass was slower and the 2^8 one much slower)
+#pragma unroll 1
         for (u32 task = tid; task < TASKS; task += NTT2_THREADS) {
             const u32 lane = task % LANES, bf = task / LANES;
             const u32 lo = bf & (SPAN - 1), base = ((bf >> LOGSPAN) << (LOGSPAN + 4)) + lo;
-            const u32 hb = swz_hash<LK>(base);
+            const u32 bh = base ^ swz_hash<LK>(base);
+            u64* pr[1 << LK];
+#pragma unroll
+            for (int v = 0; v < (1 << LK); v++) pr[v] = s + ((bh ^ v) * LANES + lane);
             u64 x[16];
 #pragma unroll
-            for (int q = 0; q < 16; q++) {
-                const u32 row = (base + ((u32)q << LOGSPAN)) ^ (hb ^ swz_const<LK>((u32)q << LOGSPAN));
-                x[q] = s[row * LANES + lane];
-            }
+            for (int q = 0; q < 16; q++) x[q] = pr[swz_lo<LK>((u32)q << LOGSPAN)][swz_hi<LK>((u32)q << LOGSPAN) * LANES];
             if (K == 0 && pre) {
 #pragma unroll
                 for (int q = 0; q < 16; q++) x[q] = gl_mul(x[q], __ldg(pre + base + ((u32)q << LOGSPAN)));
@@ -144,23 +167,23 @@ __device__ __forceinline__ void tile_round(u64* __restrict__ s, const u64* __res
                 }
             }
 #pragma unroll
-            for (int q = 0; q < 16; q++) {
-                const u32 row = (base + ((u32)q << LOGSPAN)) ^ (hb ^ swz_const<LK>((u32)q << LOGSPAN));
-                s[row * LANES + lane] = x[q];
-            }
+            for (int q = 0; q < 16; q++) pr[swz_lo<LK>((u32)q << LOGSPAN)][swz_hi<LK>((u32)q << LOGSPAN) * LANES] = x[q];
         }
     } else {
         // radix-8 on two adjacent lanes
         constexpr int LP = LANES / 2;
+#pragma unroll 1
         for (u32 task = tid; task < TASKS; task += NTT2_THREADS) {
             const u32 lp = task % LP, bf = task / LP;
             const u32 lo = bf & (SPAN - 1), base = ((bf >> LOGSPAN) << (LOGSPAN + 3)) + lo;
-            const u32 hb = swz_hash<LK>(base);
+            const u32 bh = base ^ swz_hash<LK>(base);
+            ulonglong2* pr[1 << LK];
+#pragma unroll
+            for (int v = 0; v < (1 << LK); v++) pr[v] = reinterpret_cast<ulonglong2*>(s + ((bh ^ v) * LANES + 2 * lp));
             u64 xa[8], xb[8];
 #pragma unroll
             for (int q = 0; q < 8; q++) {
-                const u32 row = (base + ((u32)q << LOGSPAN)) ^ (hb ^ swz_const<LK>((u32)q << LOGSPAN));
-                const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(s + row * LANES + 2 * lp);
+                const ulonglong2 v = pr[swz_lo<LK>((u32)q << LOGSPAN)][swz_hi<LK>((u32)q << LOGSPAN) * (LANES / 2)];
                 xa[q] = v.x;
                 xb[q] = v.y;
             }
@@ -185,10 +208,7 @@ __device__ __forceinline__ void tile_round(u64* __restrict__ s, const u64* __res
                 }
             }
 #pragma unroll
-            for (int q = 0; q < 8; q++) {
-                const u32 row = (base + ((u32)q << LOGSPAN)) ^ (hb ^ swz_const<LK>((u32)q << LOGSPAN));
-                *reinterpret_cast<ulonglong2*>(s + row * LANES + 2 * lp) = make_ulonglong2(xa[q], xb[q]);
-            }
+            for (int q = 0; q < 8; q++) pr[swz_lo<LK>((u32)q << LOGSPAN)][swz_hi<LK>((u32)q << LOGSPAN) * (LANES / 2)] = make_ulonglong2(xa[q], xb[q]);
         }
     }
 }
@@ -341,6 +361,32 @@ __global__ void __launch_bounds__(NTT2_THREADS, NTT2_MINB) ntt2_pass_kernel(cons
         const bool post = p.has_post, scale = !p.has_post && p.cconst != 1, vec = p.vec_out;
         const u32 inv_mask = p.inverse ? (S - 1) : 0;  // jf = inverse ? (S - j) mod S : j
         constexpr u32 ROWS_PER_IT = NTT2_THREADS / LP;
+        if (!p.inverse && vec && T == 1) {
+            // Forward transform, 128-bit stores, one tile column (every LDE): output row j = j0 + it ROWS_PER_IT is tile row
+            // brev(j0) | brev(it ROWS_PER_IT), two bit fields apart, so with the linear row hash it sits at
+            // prow(brev(j0)) ^ prow(brev(it ROWS_PER_IT)), the second a compile-time constant. As in the rounds, 2^LK row pointers and
+            // compile-time offsets replace the per-row bit reversal and hash, and the output and twiddle rows advance by constants.
+            const u32 j0 = tid / LP, r0 = __brev(j0) >> (32 - LOGS), rh = r0 ^ swz_hash<LK>(r0);
+            const ulonglong2* pr[1 << LK];
+#pragma unroll
+            for (int v = 0; v < (1 << LK); v++) pr[v] = reinterpret_cast<const ulonglong2*>(s + ((rh ^ v) * LANES + l0));
+            const u64* cj = ctw + j0;
+            u64* oj = o0 + (u64)j0 * jstride;
+            const u64 ostep = (u64)ROWS_PER_IT * jstride;
+            for_brev_rows<LOGS, LK, ROWS_PER_IT, S / ROWS_PER_IT>([&](u32 it, u32 lo, u32 hi) {
+                ulonglong2 v = pr[lo][hi * (LANES / 2)];
+                if (post) {
+                    const u64 f = cj[it * ROWS_PER_IT];
+                    v.x = gl_mul(v.x, f);
+                    v.y = gl_mul(v.y, f);
+                } else if (scale) {
+                    v.x = gl_mul(v.x, p.cconst);
+                    v.y = gl_mul(v.y, p.cconst);
+                }
+                if (ok0) *reinterpret_cast<ulonglong2*>(oj + it * ostep) = v;
+            });
+            return;
+        }
 #pragma unroll 4
         for (u32 j = tid / LP; j < S; j += ROWS_PER_IT) {
             const u32 jf = inv_mask ? ((S - j) & inv_mask) : j;
