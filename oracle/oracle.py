@@ -358,19 +358,46 @@ def build_fib_trace(k, n):
     return tr, res
 
 
-def prove_fib(trace, results, opts):
+# ---- dishonest proofs (oracle/wf_prover.cpp, "dishonest proofs") ----
+# Targets of a Tamper. The LDE targets put the delta into the committed and opened rows of one column only; FRI_LAYER k
+# adds it to layer k before it is committed (0 = the DEEP codeword; k = the number of layers: the remainder's codeword) and
+# folds on from there; REMAINDER adds it to one serialized coefficient; REMAINDER_LONG puts `index` zero coefficients in
+# front of the remainder; the FLIP_* targets flip bit (delta[0] mod 8) of byte `row` of a section's opened values after the
+# proof is written (FLIP_FRI: of layer `index`).
+MAIN_LDE, AUX_LDE, CONSTRAINT_LDE, FRI_LAYER, REMAINDER, REMAINDER_LONG, FLIP_TRACE, FLIP_AUX, FLIP_CONSTRAINT, FLIP_FRI = range(10)
+ALL_ROWS = (1 << 64) - 1
+
+
+def tamper(target, index=0, row=ALL_ROWS, delta=(1, 0, 0)):
+    """One tamper: delta is an element of E as up to three canonical words (base-field targets use word 0)."""
+    dl = [int(v) for v in delta] + [0] * (3 - len(delta))
+    return (int(target), int(index), int(row), *dl)
+
+
+def _prove(fn, args, tamper_list):
+    """Calls a proving entry point with its trailing tamper arguments. Returns the proof bytes, or (proof, positions) when
+    tamper_list is not None: the query positions the proof opens (sorted, distinct)."""
+    cap = 1 << 23
+    out = np.zeros(cap, dtype=np.uint8)
+    fn.restype = C.c_long
+    tl = [] if tamper_list is None else list(tamper_list)
+    t_ = np.array(tl, dtype=np.uint64).reshape(-1, 6) if tl else np.zeros((1, 6), dtype=np.uint64)
+    pos = np.zeros(256, dtype=np.uint64)
+    npos = C.c_size_t(0)
+    want_pos = tamper_list is not None
+    ln = fn(*args, out.ctypes.data_as(u8p), C.c_size_t(cap), t_.ctypes.data_as(u64p), C.c_size_t(len(tl)),
+            pos.ctypes.data_as(u64p) if want_pos else None, C.byref(npos) if want_pos else None)
+    if ln < 0:
+        raise RuntimeError(f"{fn.__name__} failed ({ln})")
+    proof = out[:ln].tobytes()
+    return (proof, pos[: npos.value].copy()) if want_pos else proof
+
+
+def prove_fib(trace, results, opts, tamper=None):
     t_, tp = _u64(trace)
     r_, rp = _u64(results)
     k, n = t_.shape[0] // 2, t_.shape[1]
-    cap = 1 << 23
-    out = np.zeros(cap, dtype=np.uint8)
-    L = lib()
-    L.wfo_prove_fib.restype = C.c_long
-    ln = L.wfo_prove_fib(tp, C.c_size_t(k), C.c_size_t(n), rp, opts.ctypes.data_as(C.POINTER(C.c_uint32)),
-                         out.ctypes.data_as(u8p), C.c_size_t(cap))
-    if ln < 0:
-        raise RuntimeError("prove_fib failed")
-    return out[:ln].tobytes()
+    return _prove(lib().wfo_prove_fib, (tp, C.c_size_t(k), C.c_size_t(n), rp, opts.ctypes.data_as(C.POINTER(C.c_uint32))), tamper)
 
 
 def verify_fib(proof: bytes, k, results, hash_id=BLAKE3):
@@ -379,18 +406,11 @@ def verify_fib(proof: bytes, k, results, hash_id=BLAKE3):
     return lib().wfo_verify_fib(pp, C.c_size_t(len(proof)), C.c_size_t(k), rp, C.c_int(hash_id))
 
 
-def prove_air(desc, trace, opts):
+def prove_air(desc, trace, opts, tamper=None):
     d_, dp = _u64(desc)
     t_, tp = _u64(trace)
-    cap = 1 << 23
-    out = np.zeros(cap, dtype=np.uint8)
-    L = lib()
-    L.wfo_prove_air.restype = C.c_long
-    ln = L.wfo_prove_air(dp, C.c_size_t(d_.size), tp, C.c_size_t(t_.shape[1]), opts.ctypes.data_as(C.POINTER(C.c_uint32)),
-                         out.ctypes.data_as(u8p), C.c_size_t(cap))
-    if ln < 0:
-        raise RuntimeError(f"prove_air failed ({ln})")
-    return out[:ln].tobytes()
+    return _prove(lib().wfo_prove_air, (dp, C.c_size_t(d_.size), tp, C.c_size_t(t_.shape[1]),
+                                        opts.ctypes.data_as(C.POINTER(C.c_uint32))), tamper)
 
 
 AUX_BUILDER = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64))
@@ -412,19 +432,12 @@ def aux_callback(builder, aw, nr, n, d):
     return AUX_BUILDER(cb)
 
 
-def prove_air_aux(desc, trace, opts, builder, aw, nr):
+def prove_air_aux(desc, trace, opts, builder, aw, nr, tamper=None):
     d_, dp = _u64(desc)
     t_, tp = _u64(trace)
-    cap = 1 << 23
-    out = np.zeros(cap, dtype=np.uint8)
-    L = lib()
-    L.wfo_prove_air_aux.restype = C.c_long
     cb = aux_callback(builder, aw, nr, t_.shape[1], int(opts[3]))
-    ln = L.wfo_prove_air_aux(dp, C.c_size_t(d_.size), tp, C.c_size_t(t_.shape[1]), opts.ctypes.data_as(C.POINTER(C.c_uint32)),
-                             cb, None, out.ctypes.data_as(u8p), C.c_size_t(cap))
-    if ln < 0:
-        raise RuntimeError(f"prove_air_aux failed ({ln})")
-    return out[:ln].tobytes()
+    return _prove(lib().wfo_prove_air_aux, (dp, C.c_size_t(d_.size), tp, C.c_size_t(t_.shape[1]),
+                                            opts.ctypes.data_as(C.POINTER(C.c_uint32)), cb, None), tamper)
 
 
 def values_callback(values_fn, nr, nvals, d):
@@ -442,20 +455,13 @@ def values_callback(values_fn, nr, nvals, d):
     return AUX_BUILDER(cb)
 
 
-def prove_air_aux_dyn(desc, trace, opts, builder, values_fn, aw, nr, nvals):
+def prove_air_aux_dyn(desc, trace, opts, builder, values_fn, aw, nr, nvals, tamper=None):
     d_, dp = _u64(desc)
     t_, tp = _u64(trace)
-    cap = 1 << 23
-    out = np.zeros(cap, dtype=np.uint8)
-    L = lib()
-    L.wfo_prove_air_aux_dyn.restype = C.c_long
     d = int(opts[3])
     cb, cv = aux_callback(builder, aw, nr, t_.shape[1], d), values_callback(values_fn, nr, nvals, d)
-    ln = L.wfo_prove_air_aux_dyn(dp, C.c_size_t(d_.size), tp, C.c_size_t(t_.shape[1]), opts.ctypes.data_as(C.POINTER(C.c_uint32)),
-                                 cb, cv, None, out.ctypes.data_as(u8p), C.c_size_t(cap))
-    if ln < 0:
-        raise RuntimeError(f"prove_air_aux_dyn failed ({ln})")
-    return out[:ln].tobytes()
+    return _prove(lib().wfo_prove_air_aux_dyn, (dp, C.c_size_t(d_.size), tp, C.c_size_t(t_.shape[1]),
+                                                opts.ctypes.data_as(C.POINTER(C.c_uint32)), cb, cv, None), tamper)
 
 
 def verify_air_dyn(desc, proof: bytes, hash_id, values_fn, nr, nvals, d):

@@ -432,8 +432,12 @@ struct ProofParts {
     std::vector<u8> bytes;
 };
 
-static void queries_for(const Field& F, int h, const u64* rows_mat, size_t row_words, const std::vector<u8>& leaves,
-                        const std::vector<u8>& nodes, size_t N, const std::vector<u64>& pos, Writer& w) {
+// Byte range of a section of opened values in the proof (offset, length).
+struct Section { size_t off = 0, len = 0; };
+
+// returns where the opened values were written
+static Section queries_for(const Field& F, int h, const u64* rows_mat, size_t row_words, const std::vector<u8>& leaves,
+                           const std::vector<u8>& nodes, size_t N, const std::vector<u64>& pos, Writer& w) {
     (void)F;
     // air/src/proof/queries.rs:51-78,138-146 + trace_lde/default/mod.rs:284-297
     Writer vals;
@@ -442,8 +446,82 @@ static void queries_for(const Field& F, int h, const u64* rows_mat, size_t row_w
     long pl = merkle_prove_batch(leaves.data(), nodes.data(), N, pos.data(), pos.size(), lv.data(), pr.data(), pr.size(), digest_len(h));
     if (pl < 0) abort();
     (void)h;
-    w.usize(vals.b.size()); w.bytes(vals.b.data(), vals.b.size());
+    w.usize(vals.b.size());
+    Section s{w.b.size(), vals.b.size()};
+    w.bytes(vals.b.data(), vals.b.size());
     w.usize((u64)pl); w.bytes(pr.data(), (size_t)pl);
+    return s;
+}
+
+// ---- dishonest proofs -----------------------------------------------------------------------------
+// The oracle is test infrastructure, so it cheats on request: a proof whose every opening verifies and that is still wrong
+// is the only kind that reaches the verifier's FRI folding and remainder checks. A tamper names a target, an index, a row
+// (or every row) and a delta in E (d words, each < p; base-field targets use word 0):
+//   T_MAIN_LDE / T_AUX_LDE / T_CONSTRAINT_LDE, column `index`: the committed and opened rows of that LDE carry the delta;
+//     constraint evaluation, the OOD frame and the DEEP polynomial use the honest values.
+//   T_FRI_LAYER, layer `index` (0 = the DEEP codeword, index = number of layers: the remainder's codeword), row = position in
+//     the layer's domain: the delta is added before the layer is committed, and the next layer is folded from it.
+//   T_REMAINDER: the delta is added to serialized remainder coefficient `index` before it is hashed into the transcript.
+//   T_REMAINDER_LONG: `index` (>= 1) zero coefficients are put in front of the remainder (its highest degrees: the
+//     polynomial keeps its values, only its length is wrong).
+//   T_FLIP_TRACE / T_FLIP_AUX / T_FLIP_CONSTRAINT / T_FLIP_FRI (layer `index`): once the proof is written, bit
+//     (delta[0] mod 8) of byte `row` (ALL_ROWS: byte 0) of that section's opened values is flipped.
+enum { T_MAIN_LDE = 0, T_AUX_LDE, T_CONSTRAINT_LDE, T_FRI_LAYER, T_REMAINDER, T_REMAINDER_LONG,
+       T_FLIP_TRACE, T_FLIP_AUX, T_FLIP_CONSTRAINT, T_FLIP_FRI };
+constexpr u64 ALL_ROWS = ~(u64)0;
+struct Tamper { u64 target, index, row, delta[3]; };
+struct Tampers {
+    std::vector<Tamper> list;
+    std::vector<u64> positions;   // out: the query positions the proof opens
+};
+
+// the matrix [rows][cols * d] as committed: `m` itself, or a copy carrying the deltas of `target`
+static const u64* committed(const Tampers* tp, int target, const std::vector<u64>& m, size_t rows, size_t cols, int d,
+                            std::vector<u64>& copy) {
+    if (!tp) return m.data();
+    for (const Tamper& t : tp->list) {
+        if ((int)t.target != target) continue;
+        if (copy.empty()) copy = m;
+        const size_t r0 = t.row == ALL_ROWS ? 0 : t.row, r1 = t.row == ALL_ROWS ? rows : t.row + 1;
+        for (size_t r = r0; r < r1; r++)
+            for (int k = 0; k < d; k++) copy[(r * cols + t.index) * d + k] = f_add(copy[(r * cols + t.index) * d + k], t.delta[k]);
+    }
+    return copy.empty() ? m.data() : copy.data();
+}
+// the deltas of FRI layer `layer` on its evaluations [len][d]
+static void tamper_layer(const Tampers* tp, size_t layer, std::vector<u64>& ev, size_t len, int d) {
+    if (!tp) return;
+    for (const Tamper& t : tp->list) {
+        if (t.target != T_FRI_LAYER || t.index != layer) continue;
+        const size_t r0 = t.row == ALL_ROWS ? 0 : t.row, r1 = t.row == ALL_ROWS ? len : t.row + 1;
+        for (size_t r = r0; r < r1; r++) for (int k = 0; k < d; k++) ev[r * d + k] = f_add(ev[r * d + k], t.delta[k]);
+    }
+}
+// false when a tamper names nothing of this proof (a column, layer, row or byte that does not exist)
+static bool tampers_fit(const Tampers& tp, size_t c, size_t aw, size_t kc, size_t N, size_t nf, size_t nl, size_t rs) {
+    for (const Tamper& t : tp.list) {
+        for (int k = 0; k < 3; k++) if (t.delta[k] >= P) return false;
+        const bool all = t.row == ALL_ROWS;
+        switch (t.target) {
+            case T_MAIN_LDE: if (t.index >= c || (!all && t.row >= N)) return false; break;
+            case T_AUX_LDE: if (t.index >= aw || (!all && t.row >= N)) return false; break;
+            case T_CONSTRAINT_LDE: if (t.index >= kc || (!all && t.row >= N)) return false; break;
+            case T_FRI_LAYER: {
+                if (t.index > nl) return false;
+                size_t len = N;
+                for (u64 i = 0; i < t.index; i++) len /= nf;
+                if (!all && t.row >= len) return false;
+                break;
+            }
+            case T_REMAINDER: if (t.index >= rs || !all) return false; break;
+            case T_REMAINDER_LONG: if (t.index < 1 || t.index > 64 || !all) return false; break;
+            case T_FLIP_AUX: if (!aw) return false; break;
+            case T_FLIP_FRI: if (t.index >= nl) return false; break;
+            case T_FLIP_TRACE: case T_FLIP_CONSTRAINT: break;
+            default: return false;
+        }
+    }
+    return true;
 }
 
 struct StageTimer {
@@ -471,8 +549,9 @@ static bool apply_aux_values(Air& air, const std::vector<EE>& rnd, int d) {
     return true;
 }
 
+// tp: the tampers of a dishonest proof (nullptr: an honest one); an empty result when one of them does not fit the proof
 static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]*/, AuxBuilder aux_builder = nullptr,
-                                  void* aux_user = nullptr) {
+                                  void* aux_user = nullptr, Tampers* tp = nullptr) {
     FibAir air = air_in;  // the aux assertion values may be rewritten from the random elements (get_aux_assertions)
     StageTimer tm;
     const Opts& o = air.o;
@@ -480,6 +559,12 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
     Field F{(int)o.ext};
     const int d = F.d;
     const size_t n = air.n, N = air.lde_size(), c = air.width(), b = o.blowup, aw = air.aw;
+    if (tp) {
+        size_t nl = 0, dom = N, rs = n;
+        while (dom > (size_t)(o.rem_max_deg + 1) * b) { dom /= o.folding; rs /= o.folding; nl++; }
+        if (!tampers_fit(*tp, c, aw, air.num_comp_cols(), N, o.folding, nl, rs)) return {};
+    }
+    std::vector<u64> lde_t, alde_t, clde_t;   // the committed copies of tampered LDEs
     // channel (prover/src/channel.rs:57-82)
     std::vector<u64> seed = context_elements(air);
     for (u64 r : air.pub_inputs) seed.push_back(r);
@@ -491,8 +576,9 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
     interpolate_columns(polys.data(), c, n, 1);
     std::vector<u64> lde(N * c);
     lde_rows(polys.data(), c, n, 1, b, lde.data());
+    const u64* lde_c = committed(tp, T_MAIN_LDE, lde, N, c, 1, lde_t);
     std::vector<u8> t_leaves(N * 32), t_nodes(N * 32);
-    hash_rows(h, lde.data(), N, c, o.part_words(c, 1), t_leaves.data());  // row_matrix.rs:191 with E = BaseField
+    hash_rows(h, lde_c, N, c, o.part_words(c, 1), t_leaves.data());  // row_matrix.rs:191 with E = BaseField
     merkle_nodes(h, t_leaves.data(), N, t_nodes.data());
     commitments.bytes(t_nodes.data() + 32, digest_len(h));
     coin.reseed(t_nodes.data() + 32);
@@ -500,6 +586,7 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
     // 1b. auxiliary segment (lib.rs:309-349, air/src/air/mod.rs:292-306, trace_lde/default/mod.rs:140-166)
     std::vector<EE> rnd;
     std::vector<u64> apolys, alde;
+    const u64* alde_c = nullptr;
     std::vector<u8> a_leaves, a_nodes;
     if (aw) {
         for (size_t i = 0; i < air.nr; i++) rnd.push_back(coin.draw(F));
@@ -511,8 +598,9 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
         interpolate_columns(apolys.data(), aw, n, d);
         alde.resize(N * aw * d);
         lde_rows(apolys.data(), aw, n, d, b, alde.data());
+        alde_c = committed(tp, T_AUX_LDE, alde, N, aw, d, alde_t);
         a_leaves.resize(N * 32); a_nodes.resize(N * 32);
-        hash_rows(h, alde.data(), N, aw * d, o.part_words(aw, d), a_leaves.data());
+        hash_rows(h, alde_c, N, aw * d, o.part_words(aw, d), a_leaves.data());
         merkle_nodes(h, a_leaves.data(), N, a_nodes.data());
         commitments.bytes(a_nodes.data() + 32, digest_len(h));
         coin.reseed(a_nodes.data() + 32);
@@ -614,8 +702,9 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
     for (size_t j = 0; j < kc; j++) memcpy(&cpolys[j * n * d], &cp[j * n * d], n * d * 8);
     std::vector<u64> clde(N * kc * d);
     lde_rows(cpolys.data(), kc, n, d, b, clde.data());
+    const u64* clde_c = committed(tp, T_CONSTRAINT_LDE, clde, N, kc, d, clde_t);
     std::vector<u8> c_leaves(N * 32), c_nodes(N * 32);
-    hash_rows(h, clde.data(), N, kc * d, o.part_words(kc, d), c_leaves.data());
+    hash_rows(h, clde_c, N, kc * d, o.part_words(kc, d), c_leaves.data());
     merkle_nodes(h, c_leaves.data(), N, c_nodes.data());
     commitments.bytes(c_nodes.data() + 32, digest_len(h));
     coin.reseed(c_nodes.data() + 32);
@@ -715,6 +804,7 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
     size_t cur_len = N;
     const size_t nf = o.folding, max_rem = (size_t)(o.rem_max_deg + 1) * b;
     while (cur_len > max_rem) {
+        tamper_layer(tp, layers.size(), cur, cur_len, d);
         Layer L;
         L.rows = cur_len / nf;
         L.tv.resize(cur_len * d);
@@ -733,11 +823,18 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
     }
     std::vector<u64> remainder;
     {
+        tamper_layer(tp, layers.size(), cur, cur_len, d);
         auto itw = get_inv_twiddles(cur_len);
         interpolate_poly_with_offset(cur.data(), cur_len, d, itw.data(), GENERATOR);
         size_t rs = cur_len / b;
         remainder.resize(rs * d);
         for (size_t i = 0; i < rs; i++) for (int k = 0; k < d; k++) remainder[i * d + k] = cur[(rs - 1 - i) * d + k];
+        if (tp)
+            for (const Tamper& t : tp->list) {
+                if (t.target == T_REMAINDER)
+                    for (int k = 0; k < d; k++) remainder[t.index * d + k] = f_add(remainder[t.index * d + k], t.delta[k]);
+                if (t.target == T_REMAINDER_LONG) remainder.insert(remainder.begin(), t.index * d, 0);
+            }
         u8 dg[32];
         hash_elements(h, remainder.data(), remainder.size(), dg);
         commitments.bytes(dg, digest_len(h));
@@ -758,9 +855,10 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
     write_context(w, air);
     w.u8_((u8)pos.size());
     w.u16_((uint16_t)commitments.b.size()); w.bytes(commitments.b.data(), commitments.b.size());
-    queries_for(F, h, lde.data(), c, t_leaves, t_nodes, N, pos, w);          // trace queries: main segment
-    if (aw) queries_for(F, h, alde.data(), aw * d, a_leaves, a_nodes, N, pos, w);  // aux segment (trace_lde/default/mod.rs:199-218)
-    queries_for(F, h, clde.data(), kc * d, c_leaves, c_nodes, N, pos, w);    // constraint queries
+    std::vector<Section> sec(T_FLIP_FRI + layers.size());   // opened values of T_FLIP_TRACE .. T_FLIP_FRI + layer
+    sec[T_FLIP_TRACE] = queries_for(F, h, lde_c, c, t_leaves, t_nodes, N, pos, w);          // trace queries: main segment
+    if (aw) sec[T_FLIP_AUX] = queries_for(F, h, alde_c, aw * d, a_leaves, a_nodes, N, pos, w);  // aux segment (trace_lde/default/mod.rs:199-218)
+    sec[T_FLIP_CONSTRAINT] = queries_for(F, h, clde_c, kc * d, c_leaves, c_nodes, N, pos, w);    // constraint queries
     w.u16_((uint16_t)ood_t.b.size()); w.bytes(ood_t.b.data(), ood_t.b.size());
     w.u16_((uint16_t)ood_q.b.size()); w.bytes(ood_q.b.data(), ood_q.b.size());
     // FriProof (fri/src/prover/mod.rs:254-319, fri/src/proof.rs:149-163,275-285)
@@ -778,7 +876,9 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
             std::vector<u8> lv(p.size() * 32), pr(64 + p.size() * 40 * 33);
             long pl = merkle_prove_batch(L.leaves.data(), L.nodes.data(), L.rows, p.data(), p.size(), lv.data(), pr.data(), pr.size(), digest_len(h));
             if (pl < 0) abort();
-            w.u32_((u32)vals.b.size()); w.bytes(vals.b.data(), vals.b.size());
+            w.u32_((u32)vals.b.size());
+            sec[T_FLIP_FRI + (&L - layers.data())] = Section{w.b.size(), vals.b.size()};
+            w.bytes(vals.b.data(), vals.b.size());
             w.u32_((u32)pl); w.bytes(pr.data(), (size_t)pl);
             dom /= nf;
         }
@@ -787,6 +887,16 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
     w.u8_(0);
     w.u64_(nonce);
     tm.mark("queries_and_proof");
+    if (tp) {
+        for (const Tamper& t : tp->list) {
+            if (t.target < T_FLIP_TRACE) continue;
+            const Section s = sec[t.target == T_FLIP_FRI ? T_FLIP_FRI + t.index : t.target];
+            const u64 at = t.row == ALL_ROWS ? 0 : t.row;
+            if (at >= s.len) return {};
+            w.b[s.off + at] ^= (u8)(1u << (t.delta[0] & 7));
+        }
+        tp->positions = pos;
+    }
     return w.b;
 }
 
@@ -1184,14 +1294,32 @@ static Opts make_opts(const uint32_t* v) {
     if (o.hash_rate == 0) o.hash_rate = 1;
     return o;
 }
-// trace: [2k][n] canonical words; results: k words. Returns proof length (bytes written to out), or -1.
-long wfo_prove_fib(const uint64_t* trace, size_t k, size_t n, const uint64_t* results, const uint32_t* opts, uint8_t* out,
-                   size_t cap) {
-    Air air = fib_air(k, n, results, make_opts(opts));
-    std::vector<u8> p = prove_fib(air, trace);
+// Every proving entry point ends in these arguments: `tamper` [ntamper][6] words {target, index, row, delta[3]} (the
+// Tamper list of a dishonest proof, see T_* above; ntamper = 0 for an honest proof) and, when `positions` is not null,
+// the query positions the proof opens (at most num_queries words) with their count in *npositions.
+static long prove_entry(const Air& air, const uint64_t* trace, AuxBuilder builder, void* user, const uint64_t* tamper,
+                        size_t ntamper, uint64_t* positions, size_t* npositions, uint8_t* out, size_t cap) {
+    Tampers tp;
+    for (size_t i = 0; i < ntamper; i++) {
+        const uint64_t* t = tamper + 6 * i;
+        tp.list.push_back(Tamper{t[0], t[1], t[2], {t[3], t[4], t[5]}});
+    }
+    std::vector<u8> p = prove_fib(air, trace, builder, user, ntamper || positions ? &tp : nullptr);
+    if (p.empty()) return -4;
     if (p.size() > cap) return -1;
     memcpy(out, p.data(), p.size());
+    if (positions) {
+        memcpy(positions, tp.positions.data(), tp.positions.size() * 8);
+        *npositions = tp.positions.size();
+    }
     return (long)p.size();
+}
+// trace: [2k][n] canonical words; results: k words. Returns proof length (bytes written to out), -1 when it does not fit,
+// -4 for a tamper that does not fit the proof.
+long wfo_prove_fib(const uint64_t* trace, size_t k, size_t n, const uint64_t* results, const uint32_t* opts, uint8_t* out,
+                   size_t cap, const uint64_t* tamper, size_t ntamper, uint64_t* positions, size_t* npositions) {
+    Air air = fib_air(k, n, results, make_opts(opts));
+    return prove_entry(air, trace, nullptr, nullptr, tamper, ntamper, positions, npositions, out, cap);
 }
 // 0 = accepted; otherwise the failed check (V_* above)
 int wfo_verify_fib(const uint8_t* proof, size_t len, size_t k, const uint64_t* results, int hash_id) {
@@ -1205,39 +1333,32 @@ int wfo_verify_fib(const uint8_t* proof, size_t len, size_t k, const uint64_t* r
 }
 // generic AIR (flat description, see parse_air): trace [w][n]
 long wfo_prove_air(const uint64_t* desc, size_t desc_len, const uint64_t* trace, size_t n, const uint32_t* opts, uint8_t* out,
-                   size_t cap) {
+                   size_t cap, const uint64_t* tamper, size_t ntamper, uint64_t* positions, size_t* npositions) {
     Air air;
     if (!parse_air(desc, desc_len, air)) return -2;
     air.n = n; air.o = make_opts(opts);
     if (air.aw) return -3;  // multi-segment AIRs go through wfo_prove_air_aux
-    std::vector<u8> p = prove_fib(air, trace);
-    if (p.size() > cap) return -1;
-    memcpy(out, p.data(), p.size());
-    return (long)p.size();
+    return prove_entry(air, trace, nullptr, nullptr, tamper, ntamper, positions, npositions, out, cap);
 }
 // multi-segment AIR: `builder` fills the aux columns [aw][n][d] from the drawn random elements [nr][d]
 long wfo_prove_air_aux(const uint64_t* desc, size_t desc_len, const uint64_t* trace, size_t n, const uint32_t* opts,
-                       int (*builder)(void*, const uint64_t*, uint64_t*), void* user, uint8_t* out, size_t cap) {
+                       int (*builder)(void*, const uint64_t*, uint64_t*), void* user, uint8_t* out, size_t cap,
+                       const uint64_t* tamper, size_t ntamper, uint64_t* positions, size_t* npositions) {
     Air air;
     if (!parse_air(desc, desc_len, air)) return -2;
     air.n = n; air.o = make_opts(opts);
-    std::vector<u8> p = prove_fib(air, trace, builder, user);
-    if (p.size() > cap) return -1;
-    memcpy(out, p.data(), p.size());
-    return (long)p.size();
+    return prove_entry(air, trace, builder, user, tamper, ntamper, positions, npositions, out, cap);
 }
 // same with Air::get_aux_assertions as a callback on the random elements (prover and verifier must be given the same one)
 long wfo_prove_air_aux_dyn(const uint64_t* desc, size_t desc_len, const uint64_t* trace, size_t n, const uint32_t* opts,
                            int (*builder)(void*, const uint64_t*, uint64_t*), int (*values_fn)(void*, const uint64_t*, uint64_t*),
-                           void* user, uint8_t* out, size_t cap) {
+                           void* user, uint8_t* out, size_t cap, const uint64_t* tamper, size_t ntamper, uint64_t* positions,
+                           size_t* npositions) {
     Air air;
     if (!parse_air(desc, desc_len, air)) return -2;
     air.n = n; air.o = make_opts(opts);
     air.aux_values_fn = values_fn; air.aux_values_user = user;
-    std::vector<u8> p = prove_fib(air, trace, builder, user);
-    if (p.size() > cap) return -1;
-    memcpy(out, p.data(), p.size());
-    return (long)p.size();
+    return prove_entry(air, trace, builder, user, tamper, ntamper, positions, npositions, out, cap);
 }
 int wfo_verify_air_dyn(const uint64_t* desc, size_t desc_len, const uint8_t* proof, size_t len, int hash_id,
                        int (*values_fn)(void*, const uint64_t*, uint64_t*), void* user) {
