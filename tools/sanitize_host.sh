@@ -8,7 +8,7 @@ NVCC=/usr/local/cuda/bin/nvcc
 mkdir -p winterfell_b200/_var/asan
 ( cd winterfell_b200
   FLAGS="-gencode arch=compute_90a,code=sm_90a -O1 -g -std=c++17 -Xcompiler -fPIC,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer --use_fast_math -ccbin /usr/bin/g++ -w -I_build"
-  for f in ntt ntt2 commit fri layout capi prover jit; do $NVCC $FLAGS -c csrc/$f.cu -o _var/asan/$f.o & done; wait
+  for f in ntt ntt2 commit fri layout capi prover jit auxbuild validate verify; do $NVCC $FLAGS -c csrc/$f.cu -o _var/asan/$f.o & done; wait
   $NVCC -Wno-deprecated-gpu-targets -shared -Xlinker --version-script=exports.map -Xcompiler -fsanitize=address,-fsanitize=undefined \
         -o _var/asan/libwinterfell_b200.so _var/asan/*.o -lcudart -ldl -ccbin /usr/bin/g++ )
 export ASAN_OPTIONS=detect_leaks=0:halt_on_error=1:protect_shadow_gap=0 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1

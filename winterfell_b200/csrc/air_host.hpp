@@ -20,6 +20,9 @@ struct AirHost {
     std::vector<std::pair<u32, std::vector<u32>>> all_degrees() const {  // context.rs:268-271
         auto r = degrees; r.insert(r.end(), aux_degrees.begin(), aux_degrees.end()); return r;
     }
+    size_t num_constraints() const {  // transition then boundary constraints, main and aux (context.rs:205-207, :223-225)
+        return degrees.size() + aux_degrees.size() + asserts.size() + aux_asserts.size();
+    }
     std::vector<u64> pub_inputs;
     std::vector<std::pair<u32, std::vector<u32>>> degrees;
     std::vector<std::vector<u64>> periodic;
@@ -33,11 +36,7 @@ struct AirHost {
     std::vector<u64> fib_results;
     u32 log_ce_blowup() const {  // air/src/air/context.rs:87-100, transition/degree.rs min_blowup_factor
         u32 r = 1;
-        for (auto& dg : all_degrees()) {
-            u32 bound = dg.first + (u32)dg.second.size() - 1, l = 0;
-            while ((1u << l) < bound) l++;
-            r = std::max(r, std::max(l, 1u));
-        }
+        for (auto& dg : all_degrees()) r = std::max(r, log2_ceil(dg.first + dg.second.size() - 1));
         return r;
     }
     u32 num_comp_cols(size_t n) const {  // context.rs:265-285
@@ -225,10 +224,8 @@ static inline int validate_assertions(wf_ctx* ctx, const std::vector<AirAssertio
 // structure of the description, degrees against the blowup factor, periodic columns, assertion validity and overlaps
 // (the panics of Air::new / BoundaryConstraints::new / prepare_assertions in the reference, returned as a status).
 static inline int air_check_host(wf_ctx* ctx, const AirHost& air, uint32_t log_n, uint32_t blowup) {
-    u32 log_b = 0;
-    while ((1u << log_b) < blowup) log_b++;
     const size_t n = (size_t)1 << log_n;
-    if (air.log_ce_blowup() > log_b) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
+    if (air.log_ce_blowup() > log2_ceil(blowup)) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
     for (auto& col : air.periodic) if (col.size() > n) return wf_fail(ctx, WF_ERR_INVALID, "periodic column longer than the trace");
     CKI(validate_degrees(ctx, air.all_degrees(), n));
     CKI(validate_assertions(ctx, air.aux_asserts, n, 3, "aux assertion"));
@@ -267,16 +264,116 @@ static inline const char* air_structure_mismatch(const AirHost& a, const AirHost
     return layout(a.aux_asserts, b.aux_asserts, aux_r);
 }
 
+// ---- proof transcript and wire format: the rules the provers (prover.cu) and the verifier (verify.cu) must share ----
+// ProofOptions from the nine option words of the C ABI: opts[8] = hash_id | num_partitions << 8 | hash_rate << 16
+// (ProofOptions::with_partitions, air/src/options.rs:193-200); 0 in either field is the default PartitionOptions::new(1, 1)
+static inline Options options_from_words(const uint32_t* opts) {
+    Options o;
+    o.num_queries = opts[0]; o.blowup = opts[1]; o.grinding = opts[2]; o.ext = opts[3]; o.folding = opts[4];
+    o.rem_max_deg = opts[5]; o.batch_c = opts[6]; o.batch_d = opts[7]; o.hash_id = (int)(opts[8] & 0xff);
+    o.num_partitions = (opts[8] >> 8) & 0xff; o.hash_rate = (opts[8] >> 16) & 0xff;
+    if (o.num_partitions == 0) o.num_partitions = 1;
+    if (o.hash_rate == 0) o.hash_rate = 1;
+    return o;
+}
+// ProofOptions::new / with_partitions asserts (air/src/options.rs:132-190, :410-417). The extension degree is left to the
+// caller: the verifier answers a bad one with WF_VERIFY_CONTEXT, after its other checks
+static inline bool options_in_range(const Options& o) {
+    auto pow2 = [](u64 v) { return v && !(v & (v - 1)); };
+    return o.num_queries >= 1 && o.num_queries <= 255 && pow2(o.blowup) && o.blowup >= 2 && o.blowup <= 128 && o.grinding <= 32 &&
+           pow2(o.folding) && o.folding >= 2 && o.folding <= 16 && o.rem_max_deg <= 255 && pow2((u64)o.rem_max_deg + 1) &&
+           o.batch_c <= 2 && o.batch_d <= 2 && o.num_partitions >= 1 && o.num_partitions <= 16 && o.hash_rate >= 1;
+}
+
+// the public coin's seed: Context::to_elements (context.rs:119-136; TraceInfo::to_elements, trace_info.rs:209-238), then
+// the public inputs (prover/src/channel.rs:57-82)
+static inline std::vector<u64> context_seed(const AirHost& air, size_t n, const Options& o) {
+    const u64 c = air.w, ti0 = air.aw ? (((((c << 8) | 1) << 8) | air.aw) << 8) | air.nr : c << 8;
+    std::vector<u64> seed = {ti0, (u64)n, 1, 0xFFFFFFFFULL, (u64)air.num_constraints(),
+                             ((u64)o.ext << 24) | ((u64)o.folding << 16) | ((u64)o.rem_max_deg << 8) | o.blowup, o.grinding, o.num_queries};
+    seed.insert(seed.end(), air.pub_inputs.begin(), air.pub_inputs.end());
+    return seed;
+}
+// Context::write_into (context.rs:142-151): TraceInfo, modulus, ProofOptions, then the number of constraints.
+// parse_proof (verify.cu) reads it back.
+static inline void write_context(ByteVec& w, const AirHost& air, u32 log_n, const Options& o) {
+    w.u8_((u8)air.w); w.u8_((u8)air.aw); w.u8_((u8)air.nr); w.u8_((u8)log_n); w.u16_(0);
+    w.u8_(8); w.u64_(GL_P);
+    w.u8_((u8)o.num_queries); w.u8_((u8)o.blowup); w.u8_((u8)o.grinding); w.u8_((u8)o.ext); w.u8_((u8)o.folding);
+    w.u8_((u8)o.rem_max_deg); w.u8_((u8)o.batch_c); w.u8_((u8)o.batch_d); w.u8_((u8)o.num_partitions); w.u8_((u8)o.hash_rate);
+    w.usize(air.num_constraints());
+}
+
+template <int D>
+static inline GlExt<D> draw_ext(PublicCoin& coin) {
+    GlExt<D> r = ext_zero<D>();
+    coin.draw(D, r.v);
+    return r;
+}
 // air/src/air/coefficients.rs:201-218: Linear / Algebraic / Horner batching of the coefficients drawn from the coin
 template <int D>
 static inline std::vector<GlExt<D>> draw_coeffs(PublicCoin& coin, u32 method, size_t n) {
-    auto draw = [&]() { GlExt<D> r = ext_zero<D>(); coin.draw(D, r.v); return r; };
     std::vector<GlExt<D>> r;
-    if (method == 0) { for (size_t i = 0; i < n; i++) r.push_back(draw()); return r; }
-    GlExt<D> a = draw(), x = ext_from_base<D>(1);
+    if (method == 0) { for (size_t i = 0; i < n; i++) r.push_back(draw_ext<D>(coin)); return r; }
+    GlExt<D> a = draw_ext<D>(coin), x = ext_from_base<D>(1);
     for (size_t i = 0; i < n; i++) { r.push_back(x); x = ext_mul(x, a); }
     if (method == 2) std::reverse(r.begin(), r.end());
     return r;
+}
+
+// Columns over E from the evaluations of their base-component columns (col_ext per column, 1 or D):
+// H_j = sum_q phi^q * (component column q of j)
+template <int D>
+static inline std::vector<GlExt<D>> ext_from_components(const std::vector<GlExt<D>>& evals, u32 col_ext = D) {
+    std::vector<GlExt<D>> r(evals.size() / col_ext);
+    for (size_t j = 0; j < r.size(); j++) {
+        GlExt<D> acc = ext_zero<D>();
+        for (u32 q = 0; q < col_ext; q++) {
+            GlExt<D> basis = ext_zero<D>();
+            basis.v[q] = 1;
+            acc = ext_add(acc, ext_mul(basis, evals[j * col_ext + q]));
+        }
+        r[j] = acc;
+    }
+    return r;
+}
+
+// OodFrame (air/src/proof/ood_frame.rs:59-72, :95-108) of the trace and the quotient columns, written to ood_t / ood_q when
+// given; returns merge_ood_evaluations (:335-349), the hash of cur (trace, quotient) then next (trace, quotient) that the coin
+// is reseeded with (prover/src/channel.rs:109-112)
+template <int D>
+static inline Digest ood_frames(int hash_id, const std::vector<GlExt<D>>& t_cur, const std::vector<GlExt<D>>& t_nxt,
+                                const std::vector<GlExt<D>>& q_cur, const std::vector<GlExt<D>>& q_nxt, ByteVec* ood_t = nullptr,
+                                ByteVec* ood_q = nullptr) {
+    auto put = [](ByteVec& w, const std::vector<GlExt<D>>& v) { for (auto& e : v) for (int q = 0; q < D; q++) w.u64_(e.v[q]); };
+    if (ood_t) { ood_t->u8_(2); put(*ood_t, t_cur); put(*ood_t, t_nxt); }
+    if (ood_q) { ood_q->u8_(2); put(*ood_q, q_cur); put(*ood_q, q_nxt); }
+    ByteVec m;
+    put(m, t_cur); put(m, q_cur); put(m, t_nxt); put(m, q_nxt);
+    return hh_hash_elements(hash_id, (const u64*)m.v.data(), m.v.size() / 8);
+}
+
+// The aux assertion values of Air::get_aux_assertions(aux_rand_elements) (air/src/air/mod.rs:279) as a callback sees them:
+// [value][D] words out of the [value][3] of AirHost::aux_asserts, times R = 2^64 mod p when `mont`
+static inline std::vector<u64> get_aux_assertion_words(const AirHost& air, int D, bool mont) {
+    std::vector<u64> vals;
+    for (auto& a : air.aux_asserts)
+        for (size_t i = 0; i < a.values.size() / 3; i++)
+            for (int k = 0; k < D; k++) vals.push_back(mont ? gl_mul(a.values[i * 3 + k], 0xFFFFFFFFULL) : a.values[i * 3 + k]);
+    return vals;
+}
+// ... and back. A Montgomery word goes through gl_from_mont; a canonical one must be < p, else false (values part written)
+static inline bool set_aux_assertion_words(AirHost& air, const u64* vals, int D, bool mont) {
+    size_t q = 0;
+    for (auto& a : air.aux_asserts)
+        for (size_t i = 0; i < a.values.size() / 3; i++, q++)
+            for (int k = 0; k < 3; k++) {
+                u64 v = k < D ? vals[q * D + k] : 0;
+                if (mont) v = gl_from_mont(v);
+                else if (v >= GL_P) return false;
+                a.values[i * 3 + k] = v;
+            }
+    return true;
 }
 
 // validate.cu: Trace::validate (prover/src/trace/mod.rs:86-201) and ConstraintEvaluationTable::validate_transition_degrees

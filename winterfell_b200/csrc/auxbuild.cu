@@ -281,8 +281,7 @@ template <int D>
 static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u32 w, const std::vector<std::vector<u64>>& periodic,
                        const u64* rnd, u32 nr, wf_mat** out) {
     const size_t n = main->m.rows;
-    u32 log_n = 0;
-    while (((size_t)1 << log_n) < n) log_n++;
+    const u32 log_n = log2_ceil(n);
     const u32 np = (u32)periodic.size();
     // one upload: constants | random elements | periodic tables | programs (u32 pairs) -- pageable, staged before return
     std::vector<u64> up(b.consts);

@@ -880,8 +880,7 @@ int wf_tree_to_host(wf_ctx* ctx, const wf_tree* t, uint8_t* leaves, uint8_t* nod
 // that all the gathers of a proof (trace rows, constraint rows, every FRI layer) share ONE index
 // upload, ONE result download and ONE stream synchronisation (GatherBatch).
 int wf_open_plan(wf_ctx* ctx, size_t n, const uint64_t* positions, size_t k, OpenPlan& pl) {
-    pl.depth = 0;
-    while (((size_t)1 << pl.depth) < n) pl.depth++;
+    pl.depth = log2_ceil(n);
     if (k == 0) return wf_fail(ctx, WF_ERR_INVALID, "no positions");
     std::map<size_t, size_t> index_map;
     for (size_t i = 0; i < k; i++) {
@@ -964,8 +963,7 @@ int GatherBatch::add_opening_sharded(wf_ctx* ctx, const wf_tree* t, size_t n_glo
     CKI(wf_open_plan(ctx, n_global, pos.data(), pos.size(), j.plan));
     if (t) j.plan.digest_bytes = WF_DIGEST_BYTES(t->hash_id);   // (the host-only planning export passes no tree)
     const size_t n_local = n_global / (size_t)world;
-    u32 log_w = 0;
-    while ((1 << log_w) < world) log_w++;
+    const u32 log_w = log2_ceil((size_t)world);
     j.idx.assign(j.plan.want.size(), ~(u64)0);
     for (size_t s = 0; s < j.plan.want.size(); s++) {
         const u64 e = j.plan.want[s];
@@ -1106,9 +1104,7 @@ int wf_fri_build_layers(wf_ctx* ctx, int hash_id, const wf_mat* evals, int d, ui
         u64 alpha[3] = {0, 0, 0};
         draw_alpha(user, alpha);
         const u64* master;
-        u32 ll = 0;
-        while (((size_t)1 << ll) < len) ll++;
-        CKI(wf_get_twiddles(ctx, ll, &master));
+        CKI(wf_get_twiddles(ctx, log2_ceil(len), &master));
         void* nxt;
         CKI(g.tmp.alloc(m * ld * 8, &nxt));
         if (ld > d) CK(cudaMemsetAsync(nxt, 0, m * ld * 8, ctx->st));
@@ -1180,9 +1176,7 @@ int wf_fri_build_layers_coin(wf_ctx* ctx, int hash_id, const wf_mat* evals, int 
         CK(fri_coin_step(hash_id, (u64*)dstate, t->nodes + 4, d, (u64*)dalpha, (u64*)dlog + 8 * layer, ctx->st));
         ctx->launches += 2 + merkle_launches(m);
         const u64* master;
-        u32 ll = 0;
-        while (((size_t)1 << ll) < len) ll++;
-        CKI(wf_get_twiddles(ctx, ll, &master));
+        CKI(wf_get_twiddles(ctx, log2_ceil(len), &master));
         void* nxt;
         CKI(g.tmp.alloc(m * ld * 8, &nxt));
         if (ld > d) CK(cudaMemsetAsync(nxt, 0, m * ld * 8, ctx->st));
@@ -1256,12 +1250,7 @@ int wf_fri_queue_proof(wf_ctx* ctx, wf_fri* f, const std::vector<u64>& positions
     std::vector<u64> pos = positions;
     for (auto& L : f->layers) {
         size_t m = L.len / f->folding;
-        std::vector<u64> fp;  // fold_positions (fri/src/folding/mod.rs:159-176)
-        for (u64 p : pos) {
-            u64 q = p % m;
-            if (std::find(fp.begin(), fp.end(), q) == fp.end()) fp.push_back(q);
-        }
-        pos = fp;
+        pos = fold_positions(pos, m);
         // queried values: row `position` of the transposed layer = v[pos + j*m], j < folding
         std::vector<u64> gpos(pos.size() * f->folding);
         for (size_t i = 0; i < pos.size(); i++)
@@ -1276,18 +1265,21 @@ int wf_fri_queue_proof(wf_ctx* ctx, wf_fri* f, const std::vector<u64>& positions
     }
     return WF_OK;
 }
-void wf_fri_finish_proof(const wf_fri* f, const GatherBatch& gb, const FriProofPlan& plan, ByteVec& bv) {
-    // FriProof / FriProofLayer wire format (fri/src/proof.rs:149-163, 275-285)
-    bv.u8_((u8)f->layers.size());
-    for (size_t l = 0; l < f->layers.size(); l++) {
-        size_t nvals = plan.nq[l] * f->folding * f->d;
+void wf_fri_finish_proof(const wf_fri* f, const GatherBatch& gb, const FriProofPlan& plan, ByteVec& bv, const FriProofPlan* before) {
+    // FriProof / FriProofLayer wire format (fri/src/proof.rs:149-163, 275-285): per layer the queried values, then the paths
+    auto layer = [&](const FriProofPlan& p, size_t l) {
+        const size_t nvals = p.nq[l] * f->folding * f->d;
         ByteVec paths;
-        wf_open_finish(gb.digs[plan.dig_ids[l]].plan, gb.digest_result(plan.dig_ids[l]), nullptr, paths);
+        wf_open_finish(gb.digs[p.dig_ids[l]].plan, gb.digest_result(p.dig_ids[l]), nullptr, paths);
         bv.u32_((u32)(nvals * 8));
-        bv.bytes(gb.row_result(plan.row_ids[l]), nvals * 8);
+        bv.bytes(gb.row_result(p.row_ids[l]), nvals * 8);
         bv.u32_((u32)paths.v.size());
         bv.bytes(paths.v.data(), paths.v.size());
-    }
+    };
+    const size_t nb = before ? before->nq.size() : 0;
+    bv.u8_((u8)(nb + f->layers.size()));
+    for (size_t l = 0; l < nb; l++) layer(*before, l);
+    for (size_t l = 0; l < f->layers.size(); l++) layer(plan, l);
     bv.u16_((uint16_t)(f->remainder.size() * 8));
     bv.bytes(f->remainder.data(), f->remainder.size() * 8);
     bv.u8_(0);  // log2(num_partitions = 1)

@@ -1,6 +1,7 @@
 // fri.cu — FRI commit-phase kernels (K11 in SURVEY.md §2.1): leaf hashing of the transposed layer
 // and the degree-respecting projection. See fri.cuh for the reference citations.
 #include "fri.cuh"
+#include "internal.hpp"
 
 #include "blake3.cuh"
 #include "commit.cuh"
@@ -126,9 +127,7 @@ template <int D>
 static cudaError_t fold_dispatch(const u64* evals, size_t len, int ld, int nf, const u64* alpha, const u64* d_alpha,
                                  const u64* master, u64* next, int next_ld, cudaStream_t st, size_t i0, u32 logL_global) {
     size_t m = len / nf;
-    u32 logL = 0;
-    while (((size_t)1 << logL) < len) logL++;
-    if (logL_global) logL = logL_global;
+    const u32 logL = logL_global ? logL_global : log2_ceil(len);
     GlExt<D> a;
     for (int c = 0; c < D; c++) a.v[c] = alpha ? alpha[c] : 0;
     unsigned blocks = (unsigned)((m + 255) / 256);

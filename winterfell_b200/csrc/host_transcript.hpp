@@ -8,6 +8,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "blake3.cuh"
@@ -127,6 +128,22 @@ struct PublicCoin {
         return out.size() == num;
     }
 };
+
+// the query positions over a domain of `domain` points (prover/src/channel.rs:150-163, verifier/src/lib.rs:284-292):
+// draw_integers, then sorted and deduplicated. false when the coin cannot draw them.
+static inline bool query_positions(PublicCoin& coin, size_t num_queries, size_t domain, u64 nonce, std::vector<u64>& pos) {
+    if (!coin.draw_integers(num_queries, domain, nonce, pos)) return false;
+    std::sort(pos.begin(), pos.end());
+    pos.erase(std::unique(pos.begin(), pos.end()), pos.end());
+    return true;
+}
+// fold_positions (fri/src/folding/mod.rs:159-176): the positions' rows in a layer of row_len rows, first occurrences in order
+static inline std::vector<u64> fold_positions(const std::vector<u64>& pos, size_t row_len) {
+    std::vector<u64> r;
+    for (u64 p : pos)
+        if (std::find(r.begin(), r.end(), p % row_len) == r.end()) r.push_back(p % row_len);
+    return r;
+}
 
 // ByteWriter (utils/core/src/serde/byte_writer.rs)
 struct ByteVec {

@@ -65,13 +65,15 @@ struct wf_tree {
     u64* nodes;   // nleaves x 4 words
 };
 
+// the least l with 2^l >= n (0 for n <= 1)
+static inline u32 log2_ceil(size_t n) { return n <= 1 ? 0 : 64 - (u32)__builtin_clzll((unsigned long long)(n - 1)); }
+
 // Small host-side transforms for transcript-sized data (FRI remainder, periodic column tables):
 // plain radix-2 on `n` elements of `d` interleaved components. inverse: a_j = (1/n) sum v_i w^(-ij),
 // then coefficient j scaled by offset^-j (fft/serial.rs:84-101 interpolate_poly_with_offset);
 // forward: coefficient j scaled by offset^j first, then v_i = sum a_j w^(ij) (evaluation over offset*<w>).
 static inline void wf_host_dft(std::vector<u64>& v, size_t n, int d, bool inverse, u64 offset) {
-    u32 log_n = 0;
-    while (((size_t)1 << log_n) < n) log_n++;
+    const u32 log_n = log2_ceil(n);
     u64 w0 = n > 1 ? gl_root_of_unity(log_n) : 1;
     if (inverse) w0 = gl_inv(w0);
     if (!inverse && offset != 1) {
@@ -209,7 +211,9 @@ struct wf_fri {
 // FriProver::build_proof split the same way: queue the gathers, then serialise
 struct FriProofPlan { std::vector<size_t> row_ids, dig_ids; std::vector<size_t> nq; };
 int wf_fri_queue_proof(wf_ctx* ctx, wf_fri* f, const std::vector<u64>& positions, GatherBatch& gb, FriProofPlan& plan);
-void wf_fri_finish_proof(const wf_fri* f, const GatherBatch& gb, const FriProofPlan& plan, ByteVec& out);
+// before: the gathers of layers that come ahead of f's own (the layers a sharded proof folds on its shards), or nullptr
+void wf_fri_finish_proof(const wf_fri* f, const GatherBatch& gb, const FriProofPlan& plan, ByteVec& out,
+                         const FriProofPlan* before = nullptr);
 int wf_tree_open_many_bytes(wf_ctx* ctx, const wf_tree* t, const uint64_t* positions, size_t k, uint8_t* leaves_out,
                             ByteVec& proof);
 

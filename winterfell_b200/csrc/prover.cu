@@ -727,23 +727,16 @@ static AirHost fib_air_host(u32 k, size_t n, const u64* results) {
     return a;
 }
 
-template <int D>
 struct Channel {  // ProverChannel (prover/src/channel.rs)
     PublicCoin coin;
     ByteVec commitments;
-    Channel(int h, const std::vector<u64>& seed) : coin(h, seed.data(), seed.size()) {}
+    explicit Channel(int h, const std::vector<u64>& seed) : coin(h, seed.data(), seed.size()) {}
     void commit(const u8 root[32]) {  // commit_trace / commit_constraints / commit_fri_layer
         commitments.bytes(root, WF_DIGEST_BYTES(coin.hash_id));   // ByteDigest<N>::write_into: N bytes
         Digest d;
         memcpy(d.b, root, 32);
         coin.reseed(d);
     }
-    GlExt<D> draw() {
-        GlExt<D> r = ext_zero<D>();
-        coin.draw(D, r.v);
-        return r;
-    }
-    std::vector<GlExt<D>> draw_coeffs(u32 method, size_t n) { return ::draw_coeffs<D>(coin, method, n); }
 };
 
 template <int D>
@@ -800,11 +793,6 @@ int ood_eval(wf_ctx* ctx, const std::vector<const wf_mat*>& mats, const GlExt<D>
         off += (size_t)cols * 2 * D;
     }
     return WF_OK;
-}
-
-template <int D>
-void write_elems(ByteVec& w, const std::vector<GlExt<D>>& v) {
-    for (auto& e : v) for (int q = 0; q < D; q++) w.u64_(e.v[q]);
 }
 
 // Queries::new (air/src/proof/queries.rs:51-78) + Serializable (:138-146), from batched gathers
@@ -1142,8 +1130,7 @@ int deep_compose_polys(wf_ctx* ctx, const wf_mat* polys, const wf_mat* apolys, c
                        const std::vector<GlExt<D>>& dc, const GlExt<D>& z, const GlExt<D>& zg, wf_mat** out) {
     const u32 c = polys->m.cols, aw = apolys ? apolys->m.cols / D : 0, ct = c + aw;
     const size_t n = polys->m.rows, ntiles = (n + SYN_TILE - 1) / SYN_TILE;
-    u32 log_n = 0;
-    while (((size_t)1 << log_n) < n) log_n++;
+    const u32 log_n = log2_ceil(n);
     DevScratch tmp(ctx);
     u64* d_dt;
     CKI(upload_ext<D>(ctx, dc, 0, ct + kc, &d_dt));
@@ -1204,13 +1191,10 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     const AirHost& air = aux_assertions ? air_dyn : air_in;
     const int h = o.hash_id;
     const size_t n = (size_t)1 << log_n;
-    u32 log_b = 0;
-    while ((1u << log_b) < o.blowup) log_b++;
+    const u32 log_b = log2_ceil(o.blowup);
     const size_t N = n << log_b;
     const u32 c = air.w, kc = air.num_comp_cols(n), log_ceb = air.log_ce_blowup();
-    const u32 aw = air.aw, n_atr = (u32)air.aux_degrees.size(), n_aas = (u32)air.aux_asserts.size();
-    const u32 n_mtr = (u32)air.degrees.size(), n_mas = (u32)air.asserts.size();
-    const u32 n_tr = n_mtr + n_atr, n_as = n_mas + n_aas;  // context.rs:205-207, :223-225
+    const u32 aw = air.aw;
     if (aw && !aux_builder && !aux_build) return wf_fail(ctx, WF_ERR_INVALID, "multi-segment AIR needs an aux trace builder");
     const bool validate = ctx->validate && !air.is_fib;   // wf_ctx_set_validation; the FibSmall path is not checked
     if (log_ceb > log_b) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
@@ -1218,14 +1202,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     CKI(validate_degrees(ctx, air.all_degrees(), n));
     CKI(validate_assertions(ctx, air.aux_asserts, n, 3, "aux assertion"));
     CKI(validate_assertions(ctx, air.asserts, n, 1, "assertion"));
-    // ---- channel seed: Context::to_elements || pub inputs (channel.rs:57-82, context.rs:119-136) ----
-    // TraceInfo::to_elements (air/src/air/trace_info.rs:209-238)
-    const u64 ti0 = aw ? ((((((u64)c << 8) | 1) << 8) | aw) << 8) | air.nr : ((u64)c << 8);
-    std::vector<u64> seed = {ti0, (u64)n, 1, 0xFFFFFFFFULL, (u64)(n_tr + n_as),
-                             ((u64)o.ext << 24) | ((u64)o.folding << 16) | ((u64)o.rem_max_deg << 8) | o.blowup,
-                             o.grinding, o.num_queries};
-    for (u64 v : air.pub_inputs) seed.push_back(v);
-    Channel<D> ch(h, seed);
+    Channel ch(h, context_seed(air, n, o));
 
     // ---- 1. trace commitment (lib.rs:497-522) ----
     wf_mat *trace = nullptr, *polys = nullptr, *lde = nullptr, *atrace = nullptr, *apolys = nullptr, *alde = nullptr, *comp = nullptr,
@@ -1259,7 +1236,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     //          DefaultTraceLde::set_aux_trace trace_lde/default/mod.rs:140-166) ----
     std::vector<u64> rnd_flat;  // [nr][D], canonical
     if (aw) {
-        for (u32 i = 0; i < air.nr; i++) { GlExt<D> e = ch.draw(); for (int q = 0; q < D; q++) rnd_flat.push_back(e.v[q]); }
+        for (u32 i = 0; i < air.nr; i++) { GlExt<D> e = draw_ext<D>(ch.coin); for (int q = 0; q < D; q++) rnd_flat.push_back(e.v[q]); }
         std::vector<u64> rnd_user = rnd_flat;
         if (mont) for (u64& v : rnd_user) v = gl_mul(v, 0xFFFFFFFFULL);  // x * R, R = 2^64 mod p
         std::vector<u64> aux_host;  // [aw][n][D]: ColMatrix<E>, one Vec<E> per column
@@ -1275,23 +1252,10 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
             if (aux_builder(aux_user, rnd_user.data(), aux_host.data()) != 0) return wf_fail(ctx, WF_ERR_INVALID, "aux trace builder failed");
         }
         if (aux_assertions) {
-            size_t total = 0;
-            for (auto& a : air_dyn.aux_asserts) total += a.values.size() / 3;
-            std::vector<u64> vals(total * D);
-            size_t q = 0;
-            for (auto& a : air_dyn.aux_asserts)
-                for (size_t i = 0; i < a.values.size() / 3; i++, q++)
-                    for (int k = 0; k < D; k++) vals[q * D + k] = mont ? gl_mul(a.values[i * 3 + k], 0xFFFFFFFFULL) : a.values[i * 3 + k];
+            std::vector<u64> vals = get_aux_assertion_words(air_dyn, D, mont);
             if (aux_assertions(aux_user, rnd_user.data(), vals.data()) != 0) return wf_fail(ctx, WF_ERR_INVALID, "aux assertion callback failed");
-            q = 0;
-            for (auto& a : air_dyn.aux_asserts)
-                for (size_t i = 0; i < a.values.size() / 3; i++, q++)
-                    for (int k = 0; k < 3; k++) {
-                        u64 v = k < D ? vals[q * D + k] : 0;
-                        if (mont) v = gl_from_mont(v);
-                        else if (v >= GL_P) return wf_fail(ctx, WF_ERR_INVALID, "aux assertion value is not a canonical field element");
-                        a.values[i * 3 + k] = v;
-                    }
+            if (!set_aux_assertion_words(air_dyn, vals.data(), D, mont))
+                return wf_fail(ctx, WF_ERR_INVALID, "aux assertion value is not a canonical field element");
         }
         if (!aux_build) {
             // E column j -> D base columns j*D + q (rows of the LDE then serialise exactly like [E] rows)
@@ -1318,7 +1282,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     // ---- 2. constraint evaluation (lib.rs:373-378) ----
     // coefficient order: main transition, aux transition (transition/mod.rs:63-72), main assertions,
     // aux assertions (boundary/mod.rs:108-110)
-    std::vector<GlExt<D>> cc = ch.draw_coeffs(o.batch_c, n_tr + n_as);
+    std::vector<GlExt<D>> cc = draw_coeffs<D>(ch.coin, o.batch_c, air.num_constraints());
     CKI(eval_constraints<D>(ctx, air, lde, alde, cc, rnd_flat, log_n, log_b, &comp));
     if (validate) {   // validate_transition_degrees (evaluator/default.rs:114) on the prover's own LDEs
         TraceReport rep;
@@ -1333,7 +1297,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     ch.commit(root);
 
     // ---- 4. out-of-domain frames (lib.rs:392-401) ----
-    GlExt<D> z = ch.draw();
+    GlExt<D> z = draw_ext<D>(ch.coin);
     GlExt<D> zg = ext_mul_base(z, gl_root_of_unity(log_n));
     std::vector<std::vector<GlExt<D>>> ood;
     {
@@ -1341,40 +1305,19 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
         if (aw) mats.push_back(apolys);
         CKI(ood_eval<D>(ctx, mats, z, zg, ood));
     }
-    std::vector<GlExt<D>>&t_cur = ood[0], &t_nxt = ood[1], &qb_cur = ood[2], &qb_nxt = ood[3];  // qb_*: per base component column
-    // H_j(z) = sum_comp phi^comp * (component column evaluated at z)
-    auto combine = [&](const std::vector<GlExt<D>>& comp_evals) {
-        std::vector<GlExt<D>> r(comp_evals.size() / D);
-        for (u32 j = 0; j < r.size(); j++) {
-            GlExt<D> acc = ext_zero<D>();
-            for (int q = 0; q < D; q++) {
-                GlExt<D> basis = ext_zero<D>();
-                basis.v[q] = 1;
-                acc = ext_add(acc, ext_mul(basis, comp_evals[j * D + q]));
-            }
-            r[j] = acc;
-        }
-        return r;
-    };
-    std::vector<GlExt<D>> q_cur = combine(qb_cur), q_nxt = combine(qb_nxt);
+    std::vector<GlExt<D>>&t_cur = ood[0], &t_nxt = ood[1];
+    std::vector<GlExt<D>> q_cur = ext_from_components<D>(ood[2]), q_nxt = ext_from_components<D>(ood[3]);
     if (aw) {  // trace frame rows = main columns then aux columns (ood_frame.rs:40-72)
-        auto a_cur = combine(ood[4]), a_nxt = combine(ood[5]);
+        auto a_cur = ext_from_components<D>(ood[4]), a_nxt = ext_from_components<D>(ood[5]);
         t_cur.insert(t_cur.end(), a_cur.begin(), a_cur.end());
         t_nxt.insert(t_nxt.end(), a_nxt.begin(), a_nxt.end());
     }
     const u32 ct = c + aw;
-    ByteVec ood_t, ood_q;  // OodFrame (air/src/proof/ood_frame.rs:59-72, :95-108)
-    ood_t.u8_(2); write_elems<D>(ood_t, t_cur); write_elems<D>(ood_t, t_nxt);
-    ood_q.u8_(2); write_elems<D>(ood_q, q_cur); write_elems<D>(ood_q, q_nxt);
-    {
-        ByteVec m;  // merge_ood_evaluations (:335-349): cur(trace, quotient), next(trace, quotient)
-        write_elems<D>(m, t_cur); write_elems<D>(m, q_cur); write_elems<D>(m, t_nxt); write_elems<D>(m, q_nxt);
-        Digest dg = hh_hash_elements(h, (const u64*)m.v.data(), m.v.size() / 8);
-        ch.coin.reseed(dg);  // channel.rs:109-112 (not added to the commitments)
-    }
+    ByteVec ood_t, ood_q;
+    ch.coin.reseed(ood_frames<D>(h, t_cur, t_nxt, q_cur, q_nxt, &ood_t, &ood_q));  // not added to the commitments
     wf_mark(ctx, "ood_frames");
     // ---- 5. DEEP composition (lib.rs:403-440), coefficient form ----
-    std::vector<GlExt<D>> dc = ch.draw_coeffs(o.batch_d, ct + kc);
+    std::vector<GlExt<D>> dc = draw_coeffs<D>(ch.coin, o.batch_d, ct + kc);
     CKI(deep_compose_polys<D>(ctx, polys, apolys, cpolys, kc, log_b, dc, z, zg, &deep));
     wf_mark(ctx, "deep_composition");
     // ---- 6. FRI (lib.rs:442-448) ----
@@ -1390,18 +1333,11 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     CKI(grind_on_device(ctx, h, ch.coin.seed, o.grinding, &nonce));
     if (ch.coin.check_leading_zeros(nonce) < o.grinding) return wf_fail(ctx, WF_ERR_STATE, "grinding self-check failed");
     std::vector<u64> pos;
-    if (!ch.coin.draw_integers(o.num_queries, N, nonce, pos)) return wf_fail(ctx, WF_ERR_STATE, "failed to draw query positions");
-    std::sort(pos.begin(), pos.end());
-    pos.erase(std::unique(pos.begin(), pos.end()), pos.end());
+    if (!query_positions(ch.coin, o.num_queries, N, nonce, pos)) return wf_fail(ctx, WF_ERR_STATE, "failed to draw query positions");
     wf_mark(ctx, "grinding");
     // ---- 8. proof object (lib.rs:464-489; air/src/proof/mod.rs:189-200) ----
     ByteVec w;
-    // Context (context.rs:142-151): TraceInfo, modulus, ProofOptions, num_constraints
-    w.u8_((u8)c); w.u8_((u8)aw); w.u8_((u8)air.nr); w.u8_((u8)log_n); w.u16_(0);
-    w.u8_(8); w.u64_(GL_P);
-    w.u8_((u8)o.num_queries); w.u8_((u8)o.blowup); w.u8_((u8)o.grinding); w.u8_((u8)o.ext); w.u8_((u8)o.folding);
-    w.u8_((u8)o.rem_max_deg); w.u8_((u8)o.batch_c); w.u8_((u8)o.batch_d); w.u8_((u8)o.num_partitions); w.u8_((u8)o.hash_rate);
-    w.usize(n_tr + n_as);
+    write_context(w, air, log_n, o);
     w.u8_((u8)pos.size());
     w.u16_((uint16_t)ch.commitments.v.size());
     w.bytes(ch.commitments.v.data(), ch.commitments.v.size());
@@ -1448,7 +1384,6 @@ struct ShardCtx {
     wf_ctx* ctx;
     const wf_comm* cm;
     int G, r;
-    u32 logG;
     double bytes_sent = 0, bytes_overlapped = 0, ncoll = 0, ms_small = 0;
     bool forked = false;
     // exchanges issued between fork() and join() run on the communicator's stream, behind the ctx stream's tail at fork time
@@ -1572,13 +1507,11 @@ static int shard_tree_finish(ShardCtx& sc, int h, ShardTree& t, Digest* root) {
 template <int D>
 int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* local_cols, const uint64_t* d_local, int mont, u32 k,
                       u32 log_n, const u64* results, const Options& o, std::vector<u8>& proof_out, double* stats) {
-    ShardCtx sc{ctx, cm, cm->world, cm->rank, 0};
+    ShardCtx sc{ctx, cm, cm->world, cm->rank};
     const int G = sc.G, r = sc.r;
-    while ((1 << sc.logG) < G) sc.logG++;
     const int h = o.hash_id;
     const size_t n = (size_t)1 << log_n;
-    u32 log_b = 0;
-    while ((1u << log_b) < o.blowup) log_b++;
+    const u32 log_b = log2_ceil(o.blowup);
     const size_t N = n << log_b, b = o.blowup;
     const u32 c = 2 * k, cl = c / (u32)G, nsl = cl / 8, nsg = c / 8;
     const size_t rows_per = N / (size_t)G;
@@ -1588,12 +1521,7 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     const u32 kc = air.num_comp_cols(n), log_ceb = air.log_ce_blowup();
     const size_t ce = n << log_ceb, ce_per = ce / (size_t)G;
     if (rows_per < 64 * b || ce_per < 64) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "trace too short to shard over %d ranks", G);
-    const u32 n_tr = (u32)air.degrees.size(), n_as = (u32)air.asserts.size();
-    std::vector<u64> seed = {(u64)c << 8, (u64)n, 1, 0xFFFFFFFFULL, (u64)(n_tr + n_as),
-                             ((u64)o.ext << 24) | ((u64)o.folding << 16) | ((u64)o.rem_max_deg << 8) | o.blowup,
-                             o.grinding, o.num_queries};
-    for (u64 v : air.pub_inputs) seed.push_back(v);
-    Channel<D> ch(h, seed);  // every rank replays the whole transcript
+    Channel ch(h, context_seed(air, n, o));  // every rank replays the whole transcript
 
     wf_mat *trace = nullptr, *polys = nullptr, *lde = nullptr, *shard = nullptr, *comp_l = nullptr, *comp = nullptr, *cpolys = nullptr,
            *clde = nullptr, *deep = nullptr, *fri_in = nullptr, *tstage = nullptr;
@@ -1707,7 +1635,7 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     wf_mark(ctx, "trace_commit");
     ch.commit(root.b);
     // ---- 4. constraint evaluation over my CE rows ----
-    std::vector<GlExt<D>> cc = ch.draw_coeffs(o.batch_c, n_tr + n_as);
+    std::vector<GlExt<D>> cc = draw_coeffs<D>(ch.coin, o.batch_c, air.num_constraints());
     CKI(eval_constraints<D>(ctx, air, shard, nullptr, cc, {}, log_n, log_b, &comp_l, (size_t)r * ce_per, ce_per));
     wf_mark(ctx, "constraint_eval");
     // ---- 5. composition polynomial: all-gather the CE evaluations (a few hundred MiB at most), interpolate + extend on
@@ -1778,7 +1706,7 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     wf_mark(ctx, "composition_commit");
     ch.commit(root.b);
     // ---- 6. out-of-domain frames: my columns' polynomials, all-gathered; composition columns are replicated ----
-    GlExt<D> z = ch.draw();
+    GlExt<D> z = draw_ext<D>(ch.coin);
     GlExt<D> zg = ext_mul_base(z, gl_root_of_unity(log_n));
     std::vector<std::vector<GlExt<D>>> ood;
     CKI(ood_eval<D>(ctx, {polys, cpolys}, z, zg, ood));
@@ -1791,32 +1719,12 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
         for (u32 j = 0; j < c; j++)
             for (int q = 0; q < D; q++) { t_cur[j].v[q] = all[((size_t)j * 2) * D + q]; t_nxt[j].v[q] = all[((size_t)j * 2 + 1) * D + q]; }
     }
-    auto combine = [&](const std::vector<GlExt<D>>& comp_evals) {  // H_j(z) from its base-component columns
-        std::vector<GlExt<D>> rr(comp_evals.size() / D);
-        for (u32 j = 0; j < rr.size(); j++) {
-            GlExt<D> acc = ext_zero<D>();
-            for (int q = 0; q < D; q++) {
-                GlExt<D> basis = ext_zero<D>();
-                basis.v[q] = 1;
-                acc = ext_add(acc, ext_mul(basis, comp_evals[j * D + q]));
-            }
-            rr[j] = acc;
-        }
-        return rr;
-    };
-    std::vector<GlExt<D>> q_cur = combine(ood[2]), q_nxt = combine(ood[3]);
+    std::vector<GlExt<D>> q_cur = ext_from_components<D>(ood[2]), q_nxt = ext_from_components<D>(ood[3]);
     ByteVec ood_t, ood_q;
-    ood_t.u8_(2); write_elems<D>(ood_t, t_cur); write_elems<D>(ood_t, t_nxt);
-    ood_q.u8_(2); write_elems<D>(ood_q, q_cur); write_elems<D>(ood_q, q_nxt);
-    {
-        ByteVec m;
-        write_elems<D>(m, t_cur); write_elems<D>(m, q_cur); write_elems<D>(m, t_nxt); write_elems<D>(m, q_nxt);
-        Digest dg = hh_hash_elements(h, (const u64*)m.v.data(), m.v.size() / 8);
-        ch.coin.reseed(dg);
-    }
+    ch.coin.reseed(ood_frames<D>(h, t_cur, t_nxt, q_cur, q_nxt, &ood_t, &ood_q));
     wf_mark(ctx, "ood_frames");
     // ---- 7. DEEP composition over my LDE rows (evaluation form is row-local) ----
-    std::vector<GlExt<D>> dc = ch.draw_coeffs(o.batch_d, c + kc);
+    std::vector<GlExt<D>> dc = draw_coeffs<D>(ch.coin, o.batch_d, c + kc);
     GlExt<D> Sz = ext_zero<D>(), Szg = ext_zero<D>();
     for (u32 j = 0; j < c; j++) { Sz = ext_add(Sz, ext_mul(dc[j], t_cur[j])); Szg = ext_add(Szg, ext_mul(dc[j], t_nxt[j])); }
     for (u32 j = 0; j < kc; j++) { Sz = ext_add(Sz, ext_mul(dc[c + j], q_cur[j])); Szg = ext_add(Szg, ext_mul(dc[c + j], q_nxt[j])); }
@@ -1864,9 +1772,8 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
         slayers.push_back(sl);
         CKI(shard_tree_finish(sc, h, slayers.back().tree, &root));
         ch.commit(root.b);              // commit_fri_layer, then draw_fri_alpha (prover/src/channel.rs:215-234)
-        GlExt<D> alpha = ch.draw();
-        u32 logL = 0;
-        while (((size_t)1 << logL) < L) logL++;
+        GlExt<D> alpha = draw_ext<D>(ch.coin);
+        const u32 logL = log2_ceil(L);
         const u64* master;
         CKI(wf_get_twiddles(ctx, logL, &master));
         void* nx;
@@ -1896,17 +1803,11 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     CKI(grind_on_device(ctx, h, ch.coin.seed, o.grinding, &nonce));
     if (ch.coin.check_leading_zeros(nonce) < o.grinding) return wf_fail(ctx, WF_ERR_STATE, "grinding self-check failed");
     std::vector<u64> pos;
-    if (!ch.coin.draw_integers(o.num_queries, N, nonce, pos)) return wf_fail(ctx, WF_ERR_STATE, "failed to draw query positions");
-    std::sort(pos.begin(), pos.end());
-    pos.erase(std::unique(pos.begin(), pos.end()), pos.end());
+    if (!query_positions(ch.coin, o.num_queries, N, nonce, pos)) return wf_fail(ctx, WF_ERR_STATE, "failed to draw query positions");
     wf_mark(ctx, "grinding");
     // ---- 10. proof object: every rank queues the same gathers, contributes what it holds, the words are summed ----
     ByteVec w;
-    w.u8_((u8)c); w.u8_(0); w.u8_(0); w.u8_((u8)log_n); w.u16_(0);
-    w.u8_(8); w.u64_(GL_P);
-    w.u8_((u8)o.num_queries); w.u8_((u8)o.blowup); w.u8_((u8)o.grinding); w.u8_((u8)o.ext); w.u8_((u8)o.folding);
-    w.u8_((u8)o.rem_max_deg); w.u8_((u8)o.batch_c); w.u8_((u8)o.batch_d); w.u8_((u8)o.num_partitions); w.u8_((u8)o.hash_rate);
-    w.usize(n_tr + n_as);
+    write_context(w, air, log_n, o);
     w.u8_((u8)pos.size());
     w.u16_((uint16_t)ch.commitments.v.size());
     w.bytes(ch.commitments.v.data(), ch.commitments.v.size());
@@ -1925,24 +1826,23 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     size_t tr_dig, cr_dig;
     CKI(gb.add_opening_sharded(ctx, ttree.local, N, G, r, pos, &tr_dig, &top_t));
     CKI(gb.add_opening_sharded(ctx, ctree.local, N, G, r, pos, &cr_dig, &top_c));
-    struct SQ { size_t row_id, dig_id, nq; std::vector<std::pair<size_t, u64>> top; };
-    std::vector<SQ> sq;
+    FriProofPlan splan;   // the sharded layers' gathers, and per layer the slots of the nodes above the subtree roots
+    std::vector<std::vector<std::pair<size_t, u64>>> top_f(slayers.size());
     std::vector<u64> fpos = pos;
-    for (auto& sl : slayers) {  // FriProver::build_proof (fri/src/prover/mod.rs:254-319) on the sharded layers
-        std::vector<u64> fp;    // fold_positions (fri/src/folding/mod.rs:159-176)
-        for (u64 p : fpos) { u64 q = p % sl.m_g; if (std::find(fp.begin(), fp.end(), q) == fp.end()) fp.push_back(q); }
-        fpos = fp;
+    for (size_t l = 0; l < slayers.size(); l++) {  // FriProver::build_proof (fri/src/prover/mod.rs:254-319) on the sharded layers
+        const SLayer& sl = slayers[l];
+        fpos = fold_positions(fpos, sl.m_g);
         std::vector<u64> gpos(fpos.size() * nf, NONE);
         for (size_t i = 0; i < fpos.size(); i++)
             if ((int)(fpos[i] / sl.m_l) == r)
                 for (u32 j = 0; j < nf; j++) gpos[i * nf + j] = (u64)j * sl.m_l + fpos[i] % sl.m_l;
         SegMatrix lm;
         lm.base = sl.vals; lm.rows = (size_t)nf * sl.m_l; lm.cols = (u32)D; lm.W = ld; lm.seg_stride = lm.rows * ld;
-        SQ e;
-        e.row_id = gb.add_rows(lm, gpos);
-        CKI(gb.add_opening_sharded(ctx, sl.tree.local, sl.m_g, G, r, fpos, &e.dig_id, &e.top));
-        e.nq = fpos.size();
-        sq.push_back(e);
+        size_t dig_id;
+        splan.row_ids.push_back(gb.add_rows(lm, gpos));
+        CKI(gb.add_opening_sharded(ctx, sl.tree.local, sl.m_g, G, r, fpos, &dig_id, &top_f[l]));
+        splan.dig_ids.push_back(dig_id);
+        splan.nq.push_back(fpos.size());
     }
     FriProofPlan fplan;
     {
@@ -1959,35 +1859,12 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     };
     patch(tr_dig, top_t, ttree);
     patch(cr_dig, top_c, ctree);
-    for (size_t i = 0; i < sq.size(); i++) patch(sq[i].dig_id, sq[i].top, slayers[i].tree);
+    for (size_t l = 0; l < slayers.size(); l++) patch(splan.dig_ids[l], top_f[l], slayers[l].tree);
     write_queries(gb, tr_rows, tr_dig, pos.size() * c, w);
     write_queries(gb, cr_rows, cr_dig, pos.size() * kc * D, w);
     w.u16_((uint16_t)ood_t.v.size()); w.bytes(ood_t.v.data(), ood_t.v.size());
     w.u16_((uint16_t)ood_q.v.size()); w.bytes(ood_q.v.data(), ood_q.v.size());
-    {   // FriProof (fri/src/proof.rs:149-163, 275-285): sharded layers, then the replicated ones
-        w.u8_((u8)(slayers.size() + fri->layers.size()));
-        for (size_t l = 0; l < sq.size(); l++) {
-            const size_t nvals = sq[l].nq * nf * D;
-            ByteVec paths;
-            wf_open_finish(gb.digs[sq[l].dig_id].plan, gb.digest_result(sq[l].dig_id), nullptr, paths);
-            w.u32_((u32)(nvals * 8));
-            w.bytes(gb.row_result(sq[l].row_id), nvals * 8);
-            w.u32_((u32)paths.v.size());
-            w.bytes(paths.v.data(), paths.v.size());
-        }
-        for (size_t l = 0; l < fri->layers.size(); l++) {
-            const size_t nvals = fplan.nq[l] * fri->folding * fri->d;
-            ByteVec paths;
-            wf_open_finish(gb.digs[fplan.dig_ids[l]].plan, gb.digest_result(fplan.dig_ids[l]), nullptr, paths);
-            w.u32_((u32)(nvals * 8));
-            w.bytes(gb.row_result(fplan.row_ids[l]), nvals * 8);
-            w.u32_((u32)paths.v.size());
-            w.bytes(paths.v.data(), paths.v.size());
-        }
-        w.u16_((uint16_t)(fri->remainder.size() * 8));
-        w.bytes(fri->remainder.data(), fri->remainder.size() * 8);
-        w.u8_(0);
-    }
+    wf_fri_finish_proof(fri, gb, fplan, w, &splan);   // the sharded layers, then the replicated ones
     w.u64_(nonce);
     wf_mark(ctx, "queries_and_proof");
     proof_out.swap(w.v);
@@ -2012,18 +1889,9 @@ extern "C" int wf_grind(wf_ctx* ctx, int hash_id, const uint8_t seed[32], uint32
 }
 
 static int parse_options(wf_ctx* ctx, const uint32_t* opts, Options& o) {
-    o.num_queries = opts[0]; o.blowup = opts[1]; o.grinding = opts[2]; o.ext = opts[3]; o.folding = opts[4];
-    o.rem_max_deg = opts[5]; o.batch_c = opts[6]; o.batch_d = opts[7]; o.hash_id = (int)(opts[8] & 0xff);
-    // ProofOptions::with_partitions (air/src/options.rs:193-200): opts[8] = hash_id | num_partitions << 8 | hash_rate << 16;
-    // 0 in either field is the default PartitionOptions::new(1, 1)
-    o.num_partitions = (opts[8] >> 8) & 0xff; o.hash_rate = (opts[8] >> 16) & 0xff;
-    if (o.num_partitions == 0) o.num_partitions = 1;
-    if (o.hash_rate == 0) o.hash_rate = 1;
+    o = options_from_words(opts);
     if (o.num_partitions > 16) return wf_fail(ctx, WF_ERR_INVALID, "at most 16 partitions (air/src/options.rs:413-414)");
-    if (o.blowup < 2 || o.blowup > 128 || (o.blowup & (o.blowup - 1)) || o.num_queries == 0 || o.num_queries > 255 || o.batch_c > 2 ||
-        o.batch_d > 2 || o.grinding > 32 || o.rem_max_deg > 255 || ((o.rem_max_deg + 1) & o.rem_max_deg) ||
-        (o.folding != 2 && o.folding != 4 && o.folding != 8 && o.folding != 16) || o.ext < 1 || o.ext > 3)
-        return wf_fail(ctx, WF_ERR_INVALID, "bad proof options");  // ProofOptions::new asserts (air/src/options.rs:132-190)
+    if (!options_in_range(o) || o.ext < 1 || o.ext > 3) return wf_fail(ctx, WF_ERR_INVALID, "bad proof options");
     if (!WF_HASH_IS_KNOWN(o.hash_id)) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "unknown hash %d", o.hash_id);
     return WF_OK;
 }
@@ -2316,8 +2184,7 @@ extern "C" int wf_eval_constraints(wf_ctx* ctx, const uint64_t* air_desc, size_t
         return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     AirHost air;
     if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
-    u32 log_b = 0;
-    while ((1u << log_b) < blowup) log_b++;
+    const u32 log_b = log2_ceil(blowup);
     const size_t N = (size_t)1 << (log_n + log_b);
     if (air.log_ce_blowup() > log_b) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
     if (main_lde->m.rows != N || main_lde->m.cols != air.w) return wf_fail(ctx, WF_ERR_INVALID, "main LDE shape does not match the AIR");
@@ -2340,18 +2207,14 @@ extern "C" int wf_composition_commit(wf_ctx* ctx, int hash_id, const wf_mat* com
                                      uint32_t num_cols, wf_mat** polys, wf_mat** lde, wf_tree** tree) {
     if (!ctx || !comp_trace || !polys || !lde || !tree || ext < 1 || ext > 3 || num_cols == 0 || blowup < 2 || (blowup & (blowup - 1)))
         return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
-    u32 log_b = 0;
-    while ((1u << log_b) < blowup) log_b++;
-    return composition_commit(ctx, hash_id, comp_trace, log_n, log_b, (int)ext, num_cols, polys, lde, tree);
+    return composition_commit(ctx, hash_id, comp_trace, log_n, log2_ceil(blowup), (int)ext, num_cols, polys, lde, tree);
 }
 extern "C" int wf_composition_commit_partitioned(wf_ctx* ctx, int hash_id, const wf_mat* comp_trace, uint32_t log_n, uint32_t blowup,
                                                  uint32_t ext, uint32_t num_cols, uint32_t partition_size, wf_mat** polys, wf_mat** lde,
                                                  wf_tree** tree) {
     if (!ctx || !comp_trace || !polys || !lde || !tree || ext < 1 || ext > 3 || num_cols == 0 || blowup < 2 || (blowup & (blowup - 1)))
         return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
-    u32 log_b = 0;
-    while ((1u << log_b) < blowup) log_b++;
-    return composition_commit(ctx, hash_id, comp_trace, log_n, log_b, (int)ext, num_cols, polys, lde, tree, partition_size);
+    return composition_commit(ctx, hash_id, comp_trace, log_n, log2_ceil(blowup), (int)ext, num_cols, polys, lde, tree, partition_size);
 }
 
 template <int D>
@@ -2363,16 +2226,8 @@ static int evaluate_at_entry(wf_ctx* ctx, const wf_mat* polys, u32 col_ext, cons
     CKI(ood_eval<D>(ctx, {polys}, a, b, ev));
     for (int pt = 0; pt < 2; pt++) {
         uint64_t* o = pt ? o1 : o0;
-        const size_t cols = ev[pt].size() / col_ext;
-        for (size_t j = 0; j < cols; j++) {
-            GlExt<D> acc = ext_zero<D>();
-            for (u32 q = 0; q < col_ext; q++) {  // column of E = sum_q phi^q * (component column q)
-                GlExt<D> basis = ext_zero<D>();
-                basis.v[q] = 1;
-                acc = ext_add(acc, ext_mul(basis, ev[pt][j * col_ext + q]));
-            }
-            for (int q = 0; q < D; q++) o[j * D + q] = acc.v[q];
-        }
+        const std::vector<GlExt<D>> cols = ext_from_components<D>(ev[pt], col_ext);
+        for (size_t j = 0; j < cols.size(); j++) for (int q = 0; q < D; q++) o[j * D + q] = cols[j].v[q];
     }
     return WF_OK;
 }
@@ -2392,8 +2247,7 @@ template <int D>
 static int deep_entry(wf_ctx* ctx, const wf_mat* lde, const wf_mat* alde, const wf_mat* clde, u32 log_n, const uint64_t* zw,
                       const uint64_t* coeffs, const uint64_t* ood_cur, const uint64_t* ood_next, wf_mat** out) {
     const u32 c = lde->m.cols, aw = alde ? alde->m.cols / D : 0, kc = clde->m.cols / D, tot = c + aw + kc;
-    u32 log_N = 0;
-    while (((size_t)1 << log_N) < lde->m.rows) log_N++;
+    const u32 log_N = log2_ceil(lde->m.rows);
     if (log_n > log_N) return wf_fail(ctx, WF_ERR_INVALID, "trace length exceeds the LDE domain");
     std::vector<GlExt<D>> dc(tot);
     GlExt<D> z = ext_zero<D>(), Sz = ext_zero<D>(), Szg = ext_zero<D>();
@@ -2436,8 +2290,7 @@ extern "C" int wf_deep_compose_polys(wf_ctx* ctx, uint32_t ext, const wf_mat* ma
         cons_polys->m.rows != main_polys->m.rows || (aux_polys && (aux_polys->m.cols % ext || aux_polys->m.rows != main_polys->m.rows)))
         return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     const size_t n = main_polys->m.rows;
-    u32 log_n = 0;
-    while (((size_t)1 << log_n) < n) log_n++;
+    const u32 log_n = log2_ceil(n);
     if (n < 8 || (n & (n - 1))) return wf_fail(ctx, WF_ERR_INVALID, "rows must be a power of two >= 8");
     if (log_blowup < 1 || log_blowup > 7 || log_n + log_blowup > 32) return wf_fail(ctx, WF_ERR_INVALID, "bad blowup");
     switch (ext) {

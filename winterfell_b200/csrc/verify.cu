@@ -248,7 +248,8 @@ struct Parsed {
     u64 nonce = 0;
 };
 
-// Proof::from_bytes with the oracle's order of checks: WF_VERIFY_ACCEPT when the bytes parse
+// Proof::from_bytes with the oracle's order of checks: WF_VERIFY_ACCEPT when the bytes parse. The Context it starts with is
+// the inverse of write_context (air_host.hpp)
 u32 parse_proof(const AirHost& air, int hash_id, const u8* proof, size_t len, Parsed& pp) {
     Reader r{proof, len};
     const u8 mw = r.u8_(), aw = r.u8_(), ar = r.u8_(), logn = r.u8_();
@@ -264,20 +265,13 @@ u32 parse_proof(const AirHost& air, int hash_id, const u8* proof, size_t len, Pa
     o.hash_id = hash_id;
     const u64 ncons = r.usize();
     if (!r.ok) return WF_VERIFY_MALFORMED;
-    // ProofOptions::new / with_partitions asserts (air/src/options.rs:143-172, :410-417), TraceInfo::read_from (2^logn >= 8)
-    // and the two-adicity of the field
-    auto pow2 = [](u64 v) { return v && !(v & (v - 1)); };
-    if (o.num_queries == 0 || !pow2(o.blowup) || o.blowup < 2 || o.blowup > 128 || o.grinding > 32 || !pow2(o.folding) || o.folding < 2 ||
-        o.folding > 16 || !pow2((u64)o.rem_max_deg + 1) || o.batch_c > 2 || o.batch_d > 2 || o.num_partitions < 1 || o.num_partitions > 16 ||
-        o.hash_rate < 1)
-        return WF_VERIFY_MALFORMED;
-    u32 lb = 0;
-    while ((1u << lb) < o.blowup) lb++;
+    // the options' asserts, TraceInfo::read_from (2^logn >= 8) and the two-adicity of the field
+    if (!options_in_range(o)) return WF_VERIFY_MALFORMED;
+    const u32 lb = log2_ceil(o.blowup);
     if (logn < 3 || logn + lb > 32) return WF_VERIFY_MALFORMED;
     pp.logn = logn;
     const size_t n = (size_t)1 << logn, N = n << lb;
-    const u64 n_tr = air.degrees.size() + air.aux_degrees.size(), n_as = air.asserts.size() + air.aux_asserts.size();
-    if (mw != air.w || ncons != n_tr + n_as || o.ext < 1 || o.ext > 3) return WF_VERIFY_CONTEXT;
+    if (mw != air.w || ncons != air.num_constraints() || o.ext < 1 || o.ext > 3) return WF_VERIFY_CONTEXT;
     const size_t d = o.ext, ct = air.w + air.aw, kc = air.num_comp_cols(n), nseg = air.aw ? 2 : 1;
     pp.nuq = r.u8_();
     const u64 clen = r.le(2);
@@ -527,46 +521,32 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
     if (call.aux_assertions) air_dyn = air_in;
     const AirHost& air = call.aux_assertions ? air_dyn : air_in;
     const size_t n = (size_t)1 << pp.logn;
-    u32 lb = 0;
-    while ((1u << lb) < o.blowup) lb++;
+    const u32 lb = log2_ceil(o.blowup);
     const size_t N = n << lb;
     const u32 c = air.w, aw = air.aw, ct = c + aw, kc = air.num_comp_cols(n), nl = pp.nl;
     const u32 n_mtr = (u32)air.degrees.size(), n_tr = n_mtr + (u32)air.aux_degrees.size();
-    const u32 n_mas = (u32)air.asserts.size(), n_as = n_mas + (u32)air.aux_asserts.size();
+    const u32 n_mas = (u32)air.asserts.size();
     const u64 g = gl_root_of_unity(pp.logn);
     const size_t nseg = aw ? 2 : 1;
     // ---- transcript (lib.rs:149-260) ----
-    const u64 ti0 = aw ? ((((((u64)c << 8) | 1) << 8) | aw) << 8) | air.nr : ((u64)c << 8);
-    std::vector<u64> seed = {ti0, (u64)n, 1, 0xFFFFFFFFULL, (u64)(n_tr + n_as),
-                             ((u64)o.ext << 24) | ((u64)o.folding << 16) | ((u64)o.rem_max_deg << 8) | o.blowup, o.grinding, o.num_queries};
-    for (u64 v : air.pub_inputs) seed.push_back(v);
+    const std::vector<u64> seed = context_seed(air, n, o);
     PublicCoin coin(h, seed.data(), seed.size());
-    auto draw = [&]() { GlExt<D> e = ext_zero<D>(); coin.draw(D, e.v); return e; };
     coin.reseed(pp.cm[0]);
     std::vector<GlExt<D>> rnd;
     if (aw) {  // lib.rs:170-184
-        for (u32 i = 0; i < air.nr; i++) rnd.push_back(draw());
+        for (u32 i = 0; i < air.nr; i++) rnd.push_back(draw_ext<D>(coin));
         coin.reseed(pp.cm[1]);
         if (call.aux_assertions) {  // Air::get_aux_assertions(aux_rand_elements)
-            std::vector<u64> rw, vals;
+            std::vector<u64> rw, vals = get_aux_assertion_words(air_dyn, D, false);
             for (auto& e : rnd) for (int k = 0; k < D; k++) rw.push_back(e.v[k]);
-            for (auto& a : air_dyn.aux_asserts)
-                for (size_t i = 0; i < a.values.size() / 3; i++) for (int k = 0; k < D; k++) vals.push_back(a.values[i * 3 + k]);
             if (call.aux_assertions(call.aux_user, j, rw.data(), vals.data()) != 0)
                 return wf_fail(call.ctx, WF_ERR_INVALID, "proof %u: aux assertion callback failed", j);
-            size_t q = 0;
-            for (auto& a : air_dyn.aux_asserts)
-                for (size_t i = 0; i < a.values.size() / 3; i++, q++)
-                    for (int k = 0; k < 3; k++) {
-                        const u64 v = k < D ? vals[q * D + k] : 0;
-                        if (v >= GL_P) { fail = fail_word(0, WF_VERIFY_MALFORMED); return WF_OK; }
-                        a.values[i * 3 + k] = v;
-                    }
+            if (!set_aux_assertion_words(air_dyn, vals.data(), D, false)) { fail = fail_word(0, WF_VERIFY_MALFORMED); return WF_OK; }
         }
     }
-    const std::vector<GlExt<D>> cc = draw_coeffs<D>(coin, o.batch_c, n_tr + n_as);
+    const std::vector<GlExt<D>> cc = draw_coeffs<D>(coin, o.batch_c, air.num_constraints());
     coin.reseed(pp.cm[nseg]);
-    const GlExt<D> z = draw();
+    const GlExt<D> z = draw_ext<D>(coin);
     std::vector<GlExt<D>> t_cur(ct), t_nxt(ct), q_cur(kc), q_nxt(kc);
     for (u32 i = 0; i < ct; i++) { t_cur[i] = read_elem<D>(pp.ood_t.p + 1, i); t_nxt[i] = read_elem<D>(pp.ood_t.p + 1, ct + i); }
     for (u32 i = 0; i < kc; i++) { q_cur[i] = read_elem<D>(pp.ood_q.p + 1, i); q_nxt[i] = read_elem<D>(pp.ood_q.p + 1, kc + i); }
@@ -605,19 +585,13 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
         for (u32 i = 0; i < kc; i++) res2 = ext_add(res2, ext_mul(ext_pow(z, (u64)i * n), q_cur[i]));
         if (memcmp(res.v, res2.v, sizeof(res.v))) { fail = fail_word(0, WF_VERIFY_OOD); return WF_OK; }
     }
-    {
-        std::vector<u64> m;   // merge_ood_evaluations: cur (trace, quotient), next (trace, quotient)
-        for (auto* v : {&t_cur, &q_cur, &t_nxt, &q_nxt}) for (auto& e : *v) for (int k = 0; k < D; k++) m.push_back(e.v[k]);
-        coin.reseed(hh_hash_elements(h, m.data(), m.size()));
-    }
+    coin.reseed(ood_frames<D>(h, t_cur, t_nxt, q_cur, q_nxt));
     const std::vector<GlExt<D>> dc = draw_coeffs<D>(coin, o.batch_d, ct + kc);
     std::vector<GlExt<D>> alphas;   // FriVerifier::new (fri/src/verifier/mod.rs:48-90)
-    for (u32 i = 0; i <= nl; i++) { coin.reseed(pp.cm[nseg + 1 + i]); alphas.push_back(draw()); }
+    for (u32 i = 0; i <= nl; i++) { coin.reseed(pp.cm[nseg + 1 + i]); alphas.push_back(draw_ext<D>(coin)); }
     if (coin.check_leading_zeros(pp.nonce) < o.grinding) { fail = fail_word(0, WF_VERIFY_POW); return WF_OK; }
     std::vector<u64> pos;
-    if (!coin.draw_integers(o.num_queries, N, pp.nonce, pos)) { fail = fail_word(0, WF_VERIFY_MALFORMED); return WF_OK; }
-    std::sort(pos.begin(), pos.end());
-    pos.erase(std::unique(pos.begin(), pos.end()), pos.end());
+    if (!query_positions(coin, o.num_queries, N, pp.nonce, pos)) { fail = fail_word(0, WF_VERIFY_MALFORMED); return WF_OK; }
     if (pos.size() != pp.nuq) { fail = fail_word(0, WF_VERIFY_MALFORMED); return WF_OK; }
 
     // ---- device work ----
@@ -657,14 +631,12 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
     }
     // FRI (fri/src/verifier/mod.rs:210-331)
     const u32 nf = o.folding;
-    u32 nf_log = 0;
-    while ((1u << nf_log) < nf) nf_log++;
+    const u32 nf_log = log2_ceil(nf);
     std::vector<u64> positions = pos;
     size_t dom = N;
     for (u32 depth = 0; depth < nl; depth++) {
         const size_t row_len = dom / nf;
-        std::vector<u64> fpos;   // fold_positions (fri/src/folding/mod.rs:159-176): first occurrences, in order
-        for (u64 p : positions) if (std::find(fpos.begin(), fpos.end(), p % row_len) == fpos.end()) fpos.push_back(p % row_len);
+        const std::vector<u64> fpos = fold_positions(positions, row_len);
         const u32 layer = fri_layer_rank(depth);
         if (pp.fri_log_parts) {   // map_positions_to_indexes (fri/src/utils.rs:9-33)
             if (pp.fri_log_parts >= 32) { fail = fail_word(layer, WF_VERIFY_MALFORMED); return WF_OK; }
@@ -685,8 +657,7 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
             per_row[row].push_back({cur[i], (u32)(positions[i] / row_len)});
         }
         std::vector<u32> next(fpos.size());
-        u32 log_dom = 0;
-        while (((size_t)1 << log_dom) < dom) log_dom++;
+        const u32 log_dom = log2_ceil(dom);
         for (size_t i = 0; i < fpos.size(); i++) {
             Plan::Fold f{};
             f.it.proof = pidx; f.it.depth = depth; f.it.log_dom = log_dom; f.it.out = next[i] = pl.nevals++;
@@ -703,19 +674,17 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
     size_t mdp1 = n;   // max_degree_plus_1 after folding (verifier/mod.rs:296-300)
     for (u32 i = 0; i < nl; i++) mdp1 /= nf;
     if (rn > mdp1) { fail = fail_word(R_REMAINDER, WF_VERIFY_FRI_REMAINDER); return WF_OK; }
-    u32 log_dom = 0;
-    while (((size_t)1 << log_dom) < dom) log_dom++;
+    const u32 log_dom = log2_ceil(dom);
     for (size_t i = 0; i < positions.size(); i++) pl.rems.push_back({pidx, cur[i], log_dom, 0, positions[i]});
     return WF_OK;
 }
 
 // AcceptableOptions::OptionSet (verifier/src/lib.rs:355-359): everything ProofOptions holds
-bool options_match(const Options& o, const uint32_t* a) {
-    u32 np = (a[8] >> 8) & 0xff, hr = (a[8] >> 16) & 0xff;
-    if (np == 0) np = 1;
-    if (hr == 0) hr = 1;
-    return o.num_queries == a[0] && o.blowup == a[1] && o.grinding == a[2] && o.ext == a[3] && o.folding == a[4] && o.rem_max_deg == a[5] &&
-           o.batch_c == a[6] && o.batch_d == a[7] && o.num_partitions == np && o.hash_rate == hr;
+bool options_match(const Options& o, const uint32_t* words) {
+    const Options a = options_from_words(words);
+    return o.num_queries == a.num_queries && o.blowup == a.blowup && o.grinding == a.grinding && o.ext == a.ext && o.folding == a.folding &&
+           o.rem_max_deg == a.rem_max_deg && o.batch_c == a.batch_c && o.batch_d == a.batch_d && o.num_partitions == a.num_partitions &&
+           o.hash_rate == a.hash_rate;
 }
 
 size_t align2(size_t words) { return (words + 1) & ~(size_t)1; }
