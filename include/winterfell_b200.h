@@ -475,6 +475,9 @@ int wf_fri_fold_dev(wf_ctx* ctx, const uint64_t* d_evals, size_t len, int ext_de
  * d_out holds 22 n words. */
 #define WF_FIELD_TEST_SHIFTS {1, 3, 6, 12, 24, 31, 32, 33, 48, 63, 64, 65, 72, 80, 84, 90, 95, 96}
 int wf_field_ops_dev(wf_ctx* ctx, const uint64_t* d_a, const uint64_t* d_b, size_t n, uint64_t* d_out);
+/* the device's power-of-two multiply for every compile-time shift: d_out[k*n + i] = a[i] * 2^k for k = 0..96
+ * (a: n canonical words, device). d_out holds 97 n words. */
+int wf_field_shifts_dev(wf_ctx* ctx, const uint64_t* d_a, size_t n, uint64_t* d_out);
 /* extension-field arithmetic of the device code (ExtensibleField<2> / <3> for BaseElement, math/src/field/f64/mod.rs:401-499;
  * inverses extensions/quadratic.rs:81-94, cubic.rs:81-97): a, b = n elements of `ext` (2 | 3) canonical words each (device);
  * d_out = 6 blocks of n elements: a*b, 1/a (0 for 0), frobenius(a), a.mul_base(b[0]), a+b, a-b. */

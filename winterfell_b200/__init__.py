@@ -112,6 +112,7 @@ _SIGS = [
     ("wf_merkle_dev", C.c_int, [vp, C.c_int, vp, C.c_size_t, vp]),
     ("wf_fri_fold_dev", C.c_int, [vp, vp, C.c_size_t, C.c_int, C.c_uint32, u64p, vp]),
     ("wf_field_ops_dev", C.c_int, [vp, vp, vp, C.c_size_t, vp]),
+    ("wf_field_shifts_dev", C.c_int, [vp, vp, C.c_size_t, vp]),
     ("wf_ext_ops_dev", C.c_int, [vp, C.c_uint32, vp, vp, C.c_size_t, vp]),
     ("wf_ctx_set_jit", C.c_int, [vp, C.c_int]),
     ("wf_ctx_jit_stats", C.c_int, [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
@@ -621,6 +622,10 @@ class Context:
 
     def field_ops_dev(self, d_a, d_b, n, d_out):
         self.check(self.L.wf_field_ops_dev(self.h, vp(d_a), vp(d_b), n, vp(d_out)))
+
+    def field_shifts_dev(self, d_a, n, d_out):
+        """d_out[k*n + i] = a[i] * 2^k for k = 0..96 (97 n words)"""
+        self.check(self.L.wf_field_shifts_dev(self.h, vp(d_a), n, vp(d_out)))
 
     def set_jit(self, on):
         """constraint kernels compiled per AIR with NVRTC (default on) vs the built-in interpreter"""

@@ -10,6 +10,7 @@
 #include <set>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "internal.hpp"
@@ -386,6 +387,16 @@ __global__ void field_ops_kernel(const u64* a, const u64* b, size_t n, u64* out)
     field_shift_store<63>(x, out, n, i, 9);  field_shift_store<64>(x, out, n, i, 10); field_shift_store<65>(x, out, n, i, 11);
     field_shift_store<72>(x, out, n, i, 12); field_shift_store<80>(x, out, n, i, 13); field_shift_store<84>(x, out, n, i, 14);
     field_shift_store<90>(x, out, n, i, 15); field_shift_store<95>(x, out, n, i, 16); field_shift_store<96>(x, out, n, i, 17);
+}
+// out[k n + i] = a[i] * 2^k for every K = 0..96: each shift amount is its own instantiation of gl_shl_dev<K>
+template <int... K>
+__device__ __forceinline__ void field_shifts_all(u64 x, u64* out, size_t n, size_t i, std::integer_sequence<int, K...>) {
+    ((out[(size_t)K * n + i] = gl_mul_2exp<K>(x)), ...);
+}
+__global__ void field_shifts_kernel(const u64* a, size_t n, u64* out) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    field_shifts_all(a[i], out, n, i, std::make_integer_sequence<int, 97>{});
 }
 
 // extension-field KAT kernel: out[0] = a * b, out[1] = a^-1, out[2] = frobenius(a), out[3] = a.mul_base(b[0]),
@@ -1337,6 +1348,14 @@ int wf_merkle_dev(wf_ctx* ctx, int hash_id, const uint8_t* d_leaves, size_t nlea
 int wf_field_ops_dev(wf_ctx* ctx, const uint64_t* d_a, const uint64_t* d_b, size_t n, uint64_t* d_out) {
     if (!ctx || !d_a || !d_b || !d_out || n == 0) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     field_ops_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->st>>>(d_a, d_b, n, d_out);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return WF_OK;
+}
+// every shift amount the network could use, K = 0..96, on crafted operands: out[k n + i] = a[i] * 2^k
+int wf_field_shifts_dev(wf_ctx* ctx, const uint64_t* d_a, size_t n, uint64_t* d_out) {
+    if (!ctx || !d_a || !d_out || n == 0) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    field_shifts_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->st>>>(d_a, n, d_out);
     ctx->launches++;
     CK(cudaGetLastError());
     return WF_OK;
