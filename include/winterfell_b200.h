@@ -478,6 +478,17 @@ int wf_field_ops_dev(wf_ctx* ctx, const uint64_t* d_a, const uint64_t* d_b, size
 /* the device's power-of-two multiply for every compile-time shift: d_out[k*n + i] = a[i] * 2^k for k = 0..96
  * (a: n canonical words, device). d_out holds 97 n words. */
 int wf_field_shifts_dev(wf_ctx* ctx, const uint64_t* d_a, size_t n, uint64_t* d_out);
+/* the Rescue arithmetic of the Rp64_256 / RpJive64_256 kernels (rp64.cuh, rpjive.cuh) on ANY 64-bit words a, b (n of each,
+ * device, n a multiple of 24), through the same device functions the kernels call. d_out holds 10 blocks of n words:
+ * gl_mul_weak(a, b), gl_sqr_weak(a), rp64_exp7(a) (congruent to the exact results, below 2^64 only), then x^(1/7) by
+ * rp64_inv7_group<G> on consecutive groups of G words of a for each G in WF_RESCUE_TEST_GROUPS (weak as well), then rp64_mds on
+ * consecutive groups of 12 words of a and rpj_mds on groups of 8 (canonical). */
+#define WF_RESCUE_TEST_GROUPS {1, 2, 3, 4, 6}
+int wf_rescue_ops_dev(wf_ctx* ctx, const uint64_t* d_a, const uint64_t* d_b, size_t n, uint64_t* d_out);
+/* the device's permutation, merge and merge_with_int of hash_id (WF_HASH_RP64_256: states of W = 12 words,
+ * WF_HASH_RPJIVE64_256: W = 8) on n states of any words (device) and n values: d_out = [n][W] permuted states, then [n][4]
+ * merge of words 0..8 of each state as two digests, then [n][4] merge_with_int(words 0..4, values[i]). */
+int wf_rescue_permute_dev(wf_ctx* ctx, int hash_id, const uint64_t* d_states, const uint64_t* d_values, size_t n, uint64_t* d_out);
 /* extension-field arithmetic of the device code (ExtensibleField<2> / <3> for BaseElement, math/src/field/f64/mod.rs:401-499;
  * inverses extensions/quadratic.rs:81-94, cubic.rs:81-97): a, b = n elements of `ext` (2 | 3) canonical words each (device);
  * d_out = 6 blocks of n elements: a*b, 1/a (0 for 0), frobenius(a), a.mul_base(b[0]), a+b, a-b. */

@@ -920,8 +920,22 @@ struct Reader {
     }
 };
 
+// ElementDigest::read_from (rp64_256/digest.rs:61-69, rp64_256_jive/digest.rs:61-69) reads each digest word through
+// BaseElement::new, which reduces a word w >= p to w - p: a Rescue commitment or Merkle path node stands for its reduced digest.
+// ByteDigest (BLAKE3, SHA3) is taken as it is.
+static void reduce_digest(int h, u8* dg) {
+    if (h != WFO_HASH_RP64_256 && h != WFO_HASH_RPJIVE64_256) return;
+    for (int k = 0; k < 4; k++) { u64 w; memcpy(&w, dg + 8 * k, 8); if (w >= P) w -= P; memcpy(dg + 8 * k, &w, 8); }
+}
+// BaseElement::read_from refuses a word >= p (math/src/field/f64/mod.rs:673-681)
+static bool words_canonical(const u8* b, size_t len) {
+    for (size_t at = 0; at + 8 <= len; at += 8) { u64 w; memcpy(&w, b + at, 8); if (w >= P) return false; }
+    return true;
+}
+
 struct BatchProof { u8 depth; std::vector<std::vector<std::array<u8, 32>>> nodes; };
-static bool read_batch_proof(Reader& r, BatchProof& bp, size_t dlen = 32) {
+static bool read_batch_proof(Reader& r, BatchProof& bp, int h) {
+    const size_t dlen = digest_len(h);
     bp.depth = r.u8_();
     u64 nv = r.usize();
     if (!r.ok || nv > 100000 || bp.depth < 1 || bp.depth > 40) return false;   // a tree of 2^depth leaves; callers shift by it
@@ -930,7 +944,7 @@ static bool read_batch_proof(Reader& r, BatchProof& bp, size_t dlen = 32) {
         u64 ln = r.usize();
         if (!r.ok || ln > 64) return false;
         v.resize(ln);
-        for (auto& dg : v) { const u8* q = r.take(dlen); if (!q) return false; dg.fill(0); memcpy(dg.data(), q, dlen); }
+        for (auto& dg : v) { const u8* q = r.take(dlen); if (!q) return false; dg.fill(0); memcpy(dg.data(), q, dlen); reduce_digest(h, dg.data()); }
     }
     return r.ok;
 }
@@ -1056,7 +1070,7 @@ static int verify_fib(const u8* proof, size_t len, FibAir air /* options + resul
     const size_t dl = digest_len(h), ncm = nseg + 1 + nlayers + 1;
     if (clen != dl * ncm) return V_MALFORMED;
     std::vector<u8> cm32(32 * ncm, 0);   // the commitments in 32-byte slots (zero padded, as ByteDigest::as_bytes)
-    for (size_t i = 0; i < ncm; i++) memcpy(cm32.data() + 32 * i, cm + dl * i, dl);
+    for (size_t i = 0; i < ncm; i++) { memcpy(cm32.data() + 32 * i, cm + dl * i, dl); reduce_digest(h, cm32.data() + 32 * i); }
     cm = cm32.data();
     const u8* trace_root = cm; const u8* aux_root = cm + 32;  // air/src/proof/commitments.rs:66-100
     const u8* cons_root = cm + 32 * nseg; const u8* fri_roots = cm + 32 * (nseg + 1);
@@ -1087,6 +1101,16 @@ static int verify_fib(const u8* proof, size_t len, FibAir air /* options + resul
     const u8 fri_log_parts = r.u8_();   // FriProof::num_partitions, stored as a power of two (fri/src/proof.rs:36,101-103)
     u64 nonce = r.le(8);
     if (!r.ok || r.pos != len || reml % (8 * d)) return V_MALFORMED;
+    // VerifierChannel::new (verifier/src/channel.rs:92-118) reads every field element of the proof with BaseElement::read_from
+    // and turns a word >= p into ProofDeserializationError: the opened values (air/src/proof/table.rs:60-65), the OOD frames
+    // (ood_frame.rs:140,157, after their frame-size byte), the FRI layer values and the remainder (fri/src/proof.rs:185,321)
+    {
+        bool ok = words_canonical(tq_vals.data(), tq_vals.size()) && words_canonical(aq_vals.data(), aq_vals.size()) &&
+                  words_canonical(cq_vals.data(), cq_vals.size()) && words_canonical(ot + 1, otl - 1) && words_canonical(oq + 1, oql - 1) &&
+                  words_canonical(rem, reml);
+        for (auto& v : fv) ok = ok && words_canonical(v.data(), v.size());
+        if (!ok) return V_MALFORMED;
+    }
 
     // transcript (lib.rs:149-260)
     std::vector<u64> seed = context_elements(air);
@@ -1168,7 +1192,7 @@ static int verify_fib(const u8* proof, size_t len, FibAir air /* options + resul
         for (size_t i = 0; i < pos.size(); i++) hash_rows(h, (const u64*)(vals.data() + i * row_words * 8), 1, row_words, part, lv[i].data());
         Reader pr_r{pr.data(), pr.size()};
         BatchProof bp;
-        if (!read_batch_proof(pr_r, bp, digest_len(h)) || pr_r.pos != pr.size() || ((size_t)1 << bp.depth) != N) return false;
+        if (!read_batch_proof(pr_r, bp, h) || pr_r.pos != pr.size() || ((size_t)1 << bp.depth) != N) return false;
         u8 got[32];
         return batch_root(h, bp, pos, lv, got) && !memcmp(got, root, 32);
     };
@@ -1225,7 +1249,7 @@ static int verify_fib(const u8* proof, size_t len, FibAir air /* options + resul
             for (size_t i = 0; i < fpos.size(); i++) hash_elements(h, (const u64*)(vals.data() + i * nf * d * 8), nf * d, lv[i].data());
             Reader pr_r{fp[depth].data(), fp[depth].size()};
             BatchProof bp;
-            if (!read_batch_proof(pr_r, bp, digest_len(h)) || pr_r.pos != fp[depth].size() || ((size_t)1 << bp.depth) != dom / nf) return V_FRI_LAYER;
+            if (!read_batch_proof(pr_r, bp, h) || pr_r.pos != fp[depth].size() || ((size_t)1 << bp.depth) != dom / nf) return V_FRI_LAYER;
             u8 got[32];
             if (!batch_root(h, bp, fpos, lv, got) || memcmp(got, fri_roots + 32 * depth, 32)) return V_FRI_LAYER;
             // get_query_values
@@ -1430,7 +1454,7 @@ int wfo_merkle_verify_batch(int hash_id, const uint8_t root[32], const uint64_t*
                             const uint8_t* proof, size_t proof_len) {
     Reader r{proof, proof_len};
     BatchProof bp;
-    if (!read_batch_proof(r, bp, digest_len(hash_id)) || r.pos != proof_len) return 1;
+    if (!read_batch_proof(r, bp, hash_id) || r.pos != proof_len) return 1;
     std::vector<u64> idx(indexes, indexes + k);
     std::vector<std::array<u8, 32>> lv(k);
     for (size_t i = 0; i < k; i++) memcpy(lv[i].data(), leaves + 32 * i, 32);

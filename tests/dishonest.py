@@ -236,3 +236,104 @@ def flip_set(proof, seed):
     zero_rate = bytearray(proof)
     zero_rate[24] = 0   # ProofOptions::hash_rate: the last of the ten option bytes after the 15-byte trace info + modulus
     return muts + [bytes(wrap), bytes(zero_rate), proof]
+
+
+# ---- proofs carrying words of p or more ----
+MALFORMED = 1
+
+
+def _usize(b, pos):
+    first = b[pos]
+    ln = 9 if first == 0 else (first & -first).bit_length()
+    if ln == 9:
+        return int.from_bytes(b[pos + 1:pos + 9], "little"), pos + 9
+    return int.from_bytes(b[pos:pos + ln], "little") >> ln, pos + ln
+
+
+def proof_fields(proof, hash_id, two_segments):
+    """byte offsets of the proof's parts (the layout parse_proof reads): {name: (offset, length)} for 'commitments',
+    'trace values' / 'trace path', ['aux values' / 'aux path'], 'constraint values' / 'constraint path', 'ood trace',
+    'ood quotient', 'fri values 0' / 'fri path 0' .., 'remainder'"""
+    b = proof
+    pos = 4
+    meta = int.from_bytes(b[pos:pos + 2], "little")
+    pos += 2 + meta
+    pos += 1 + b[pos]                 # field modulus bytes
+    pos += 10                         # options
+    _, pos = _usize(b, pos)           # number of constraints
+    pos += 1                          # unique queries
+    out = {}
+    clen = int.from_bytes(b[pos:pos + 2], "little")
+    out["commitments"] = (pos + 2, clen)
+    pos += 2 + clen
+    for seg in ["trace"] + (["aux"] if two_segments else []) + ["constraint"]:
+        for part in ("values", "path"):
+            n, pos = _usize(b, pos)
+            out[f"{seg} {part}"] = (pos, n)
+            pos += n
+    for name in ("ood trace", "ood quotient"):
+        n = int.from_bytes(b[pos:pos + 2], "little")
+        out[name] = (pos + 3, n - 1)  # after the frame-size byte
+        pos += 2 + n
+    nl = b[pos]
+    pos += 1
+    for i in range(nl):
+        for part in ("values", "path"):
+            n = int.from_bytes(b[pos:pos + 4], "little")
+            out[f"fri {part} {i}"] = (pos + 4, n)
+            pos += 4 + n
+    n = int.from_bytes(b[pos:pos + 2], "little")
+    out["remainder"] = (pos + 2, n)
+    assert pos + 2 + n + 1 + 8 == len(b)
+    return out
+
+
+def _first_path_digest(proof, off, n):
+    """offset of the first digest of a batch Merkle opening: depth byte, vint count, per node vector a vint length"""
+    pos = off + 1
+    nv, pos = _usize(proof, pos)
+    for _ in range(nv):
+        ln, pos = _usize(proof, pos)
+        if ln:
+            return pos
+    return None
+
+
+def _put(proof, at, word):
+    b = bytearray(proof)
+    b[at:at + 8] = int(word).to_bytes(8, "little")
+    return bytes(b)
+
+
+def noncanonical_cases(hash_id, ext):
+    """An honest two-segment proof with one word replaced by a word of p or more. BaseElement::read_from refuses it in every
+    field element the verifier reads (math/src/field/f64/mod.rs:673-681): an opened main, aux or constraint value, an OOD
+    value, a FRI layer value, a remainder coefficient all give ProofDeserializationError (1). A Rescue digest word is read
+    through BaseElement::new (rp64_256/digest.rs:61-69, rp64_256_jive/digest.rs:61-69), which reduces it: 2^64 - 1 stands for
+    2^32 - 2, a different digest, so a commitment or path node changed so fails the check its digest meets (`want` None: the
+    oracle decides). Words p + w for a digest word w < 2^32 - 1 would change nothing; honest digests almost never have one,
+    so that is covered at the merge level. Byte digests (BLAKE3, SHA3) are bytes: the same replacement fails the same way."""
+    opts = O.make_opts(num_queries=12, blowup=8, ext=ext, folding=4, rem_max_deg=3, hash_id=hash_id)
+    pv = Prover("perm_rap", 64)
+    proof, pos = pv.prove(opts)
+    f = proof_fields(proof, hash_id, True)
+    top = 2**64 - 1
+    spec = [("honest", proof, ACCEPT)]
+    for name, word_index, w in (("trace values", 0, top), ("trace values", -1, P), ("aux values", 1, top),
+                                ("constraint values", -1, P + 5), ("ood trace", 0, top), ("ood trace", -1, P),
+                                ("ood quotient", 2, top), ("fri values 0", 3, P), ("remainder", -1, top)):
+        off, n = f[name]
+        k = word_index % (n // 8)
+        spec.append((f"{name} word {k} = {w:#x}", _put(proof, off + 8 * k, w), MALFORMED))
+    if ext > 1:   # the last coordinate of the first extension element of the remainder
+        off, _ = f["remainder"]
+        spec.append((f"remainder coordinate {ext - 1} = p", _put(proof, off + 8 * (ext - 1), P), MALFORMED))
+    if hash_id in (1, 2):
+        off, _ = f["commitments"]
+        spec.append(("trace commitment word 1 = 2^64 - 1", _put(proof, off + 8, top), None))
+        spec.append(("constraint commitment word 0 = 2^64 - 1", _put(proof, off + 64, top), None))
+        at = _first_path_digest(proof, *f["trace path"])
+        spec.append(("trace path node word 0 = 2^64 - 1", _put(proof, at, top), None))
+        at = _first_path_digest(proof, *f["fri path 0"])
+        spec.append(("FRI path node word 3 = 2^64 - 1", _put(proof, at + 24, top), None))
+    return [Case(f"h={hash_id} ext={ext} {name}", ("perm_rap", 64), pv.desc, p, want, hash_id, pos, None) for name, p, want in spec]

@@ -113,6 +113,8 @@ _SIGS = [
     ("wf_fri_fold_dev", C.c_int, [vp, vp, C.c_size_t, C.c_int, C.c_uint32, u64p, vp]),
     ("wf_field_ops_dev", C.c_int, [vp, vp, vp, C.c_size_t, vp]),
     ("wf_field_shifts_dev", C.c_int, [vp, vp, C.c_size_t, vp]),
+    ("wf_rescue_ops_dev", C.c_int, [vp, vp, vp, C.c_size_t, vp]),
+    ("wf_rescue_permute_dev", C.c_int, [vp, C.c_int, vp, vp, C.c_size_t, vp]),
     ("wf_ext_ops_dev", C.c_int, [vp, C.c_uint32, vp, vp, C.c_size_t, vp]),
     ("wf_ctx_set_jit", C.c_int, [vp, C.c_int]),
     ("wf_ctx_jit_stats", C.c_int, [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
@@ -626,6 +628,14 @@ class Context:
     def field_shifts_dev(self, d_a, n, d_out):
         """d_out[k*n + i] = a[i] * 2^k for k = 0..96 (97 n words)"""
         self.check(self.L.wf_field_shifts_dev(self.h, vp(d_a), n, vp(d_out)))
+
+    def rescue_ops_dev(self, d_a, d_b, n, d_out):
+        """the Rescue S-box / MDS arithmetic on any 64-bit words (10 n words, include/winterfell_b200.h)"""
+        self.check(self.L.wf_rescue_ops_dev(self.h, vp(d_a), vp(d_b), n, vp(d_out)))
+
+    def rescue_permute_dev(self, hash_id, d_states, d_values, n, d_out):
+        """permute / merge / merge_with_int of HASH_RP64_256 (12-word states) or HASH_RPJIVE64_256 (8-word states)"""
+        self.check(self.L.wf_rescue_permute_dev(self.h, hash_id, vp(d_states), vp(d_values), n, vp(d_out)))
 
     def set_jit(self, on):
         """constraint kernels compiled per AIR with NVRTC (default on) vs the built-in interpreter"""

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "internal.hpp"
+#include "alg_hash.cuh"
 
 void wf_mark(wf_ctx* ctx, const char* name) {
     if (!ctx->profiling) return;
@@ -397,6 +398,60 @@ __global__ void field_shifts_kernel(const u64* a, size_t n, u64* out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     field_shifts_all(a[i], out, n, i, std::make_integer_sequence<int, 97>{});
+}
+
+// the Rescue S-box and MDS arithmetic on arbitrary 64-bit words, through the functions the hash kernels call (layout in
+// include/winterfell_b200.h, wf_rescue_ops_dev). One thread per element, per group of G, 12 or 8 elements.
+__global__ void rescue_weak_kernel(const u64* a, const u64* b, size_t n, u64* out) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    out[i] = gl_mul_weak(a[i], b[i]);
+    out[n + i] = gl_sqr_weak(a[i]);
+    out[2 * n + i] = rp64_exp7(a[i]);
+}
+template <int G>
+__global__ void rescue_inv7_kernel(const u64* a, size_t n, u64* out) {
+    size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n / G) return;
+    u64 s[G];
+#pragma unroll
+    for (int e = 0; e < G; e++) s[e] = a[t * G + e];
+    rp64_inv7_group<G>(s);
+#pragma unroll
+    for (int e = 0; e < G; e++) out[t * G + e] = s[e];
+}
+__global__ void rescue_mds_kernel(const u64* a, size_t n, u64* out12, u64* out8) {
+    size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n / 12) {
+        u64 s[12];
+        for (int e = 0; e < 12; e++) s[e] = a[t * 12 + e];
+        rp64_mds(s);
+        for (int e = 0; e < 12; e++) out12[t * 12 + e] = s[e];
+    }
+    if (t < n / 8) {
+        u64 s[8];
+        for (int e = 0; e < 8; e++) s[e] = a[t * 8 + e];
+        rpj_mds(s);
+        for (int e = 0; e < 8; e++) out8[t * 8 + e] = s[e];
+    }
+}
+// permute, merge and merge_with_int of one hasher on n states of W words (wf_rescue_permute_dev)
+template <int HASH, int W>
+__global__ void rescue_permute_kernel(const u64* in, const u64* values, size_t n, u64* out) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    u64 s[W];
+#pragma unroll
+    for (int e = 0; e < W; e++) s[e] = in[i * W + e];
+    u64 m[4], mi[4];
+    alg_merge<HASH>(s, m);
+    alg_merge_with_int<HASH>(s, values[i], mi);
+    if (HASH == WF_HASH_RP64_256) rp64_permute(s);
+    else rpj_permute(s);
+#pragma unroll
+    for (int e = 0; e < W; e++) out[i * W + e] = s[e];
+#pragma unroll
+    for (int e = 0; e < 4; e++) { out[n * W + i * 4 + e] = m[e]; out[n * (W + 4) + i * 4 + e] = mi[e]; }
 }
 
 // extension-field KAT kernel: out[0] = a * b, out[1] = a^-1, out[2] = frobenius(a), out[3] = a.mul_base(b[0]),
@@ -1356,6 +1411,32 @@ int wf_field_ops_dev(wf_ctx* ctx, const uint64_t* d_a, const uint64_t* d_b, size
 int wf_field_shifts_dev(wf_ctx* ctx, const uint64_t* d_a, size_t n, uint64_t* d_out) {
     if (!ctx || !d_a || !d_out || n == 0) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     field_shifts_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->st>>>(d_a, n, d_out);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return WF_OK;
+}
+// the hashers' weakly reduced S-box arithmetic and their MDS products on any 64-bit words: uniform data almost never reaches a
+// weak word in [p, 2^64), the borrow of gl_mul_weak or the carries of the MDS sums, so tests feed crafted operands
+int wf_rescue_ops_dev(wf_ctx* ctx, const uint64_t* d_a, const uint64_t* d_b, size_t n, uint64_t* d_out) {
+    if (!ctx || !d_a || !d_b || !d_out || n == 0 || n % 24) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    const unsigned blocks = (unsigned)((n + 127) / 128);
+    rescue_weak_kernel<<<blocks, 128, 0, ctx->st>>>(d_a, d_b, n, d_out);
+    rescue_inv7_kernel<1><<<blocks, 128, 0, ctx->st>>>(d_a, n, d_out + 3 * n);
+    rescue_inv7_kernel<2><<<blocks, 128, 0, ctx->st>>>(d_a, n, d_out + 4 * n);
+    rescue_inv7_kernel<3><<<blocks, 128, 0, ctx->st>>>(d_a, n, d_out + 5 * n);
+    rescue_inv7_kernel<4><<<blocks, 128, 0, ctx->st>>>(d_a, n, d_out + 6 * n);
+    rescue_inv7_kernel<6><<<blocks, 128, 0, ctx->st>>>(d_a, n, d_out + 7 * n);
+    rescue_mds_kernel<<<blocks, 128, 0, ctx->st>>>(d_a, n, d_out + 8 * n, d_out + 9 * n);
+    ctx->launches += 7;
+    CK(cudaGetLastError());
+    return WF_OK;
+}
+int wf_rescue_permute_dev(wf_ctx* ctx, int hash_id, const uint64_t* d_states, const uint64_t* d_values, size_t n, uint64_t* d_out) {
+    if (!ctx || !d_states || !d_values || !d_out || n == 0) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    const unsigned blocks = (unsigned)((n + 127) / 128);
+    if (hash_id == WF_HASH_RP64_256) rescue_permute_kernel<WF_HASH_RP64_256, 12><<<blocks, 128, 0, ctx->st>>>(d_states, d_values, n, d_out);
+    else if (hash_id == WF_HASH_RPJIVE64_256) rescue_permute_kernel<WF_HASH_RPJIVE64_256, 8><<<blocks, 128, 0, ctx->st>>>(d_states, d_values, n, d_out);
+    else return wf_fail(ctx, WF_ERR_INVALID, "hash %d has no Rescue permutation", hash_id);
     ctx->launches++;
     CK(cudaGetLastError());
     return WF_OK;

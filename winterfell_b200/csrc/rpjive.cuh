@@ -62,14 +62,16 @@ GL_HD void rpj_permute(u64 s[8]) {
     }
 }
 
-// Jive compression of an 8-element state (apply_jive_summation :337-350)
+// Jive compression of an 8-element state (apply_jive_summation :337-350). The input may hold any 64-bit words: the reference
+// reads a digest word w >= p as w - p (ElementDigest::read_from, rp64_256_jive/digest.rs:61-69), and gl_add needs canonical
+// operands, so the sum reduces its inputs first (the permutation takes any word).
 GL_HD void rpj_compress(const u64 in[8], u64 out[4]) {
-    u64 s[8];
+    u64 s[8], c[8];
 #pragma unroll
-    for (int i = 0; i < 8; i++) s[i] = in[i];
+    for (int i = 0; i < 8; i++) { s[i] = in[i]; c[i] = in[i] >= GL_P ? in[i] - GL_P : in[i]; }
     rpj_permute(s);
 #pragma unroll
-    for (int i = 0; i < 4; i++) out[i] = gl_add(gl_add(in[i], in[4 + i]), gl_add(s[i], s[4 + i]));
+    for (int i = 0; i < 4; i++) out[i] = gl_add(gl_add(c[i], c[4 + i]), gl_add(s[i], s[4 + i]));
 }
 // merge of two digests given as 8 canonical elements (:186-196)
 GL_HD void rpj_merge(const u64 in[8], u64 out[4]) { rpj_compress(in, out); }

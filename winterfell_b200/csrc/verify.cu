@@ -237,6 +237,32 @@ struct Reader {  // ByteReader (utils/core/src/serde/byte_reader.rs)
     }
 };
 struct Bytes { const u8* p = nullptr; size_t n = 0; };
+
+// A digest of Rp64_256 / RpJive64_256 is read word by word through BaseElement::new, which reduces a word w >= p to w - p
+// (ElementDigest::read_from, rp64_256/digest.rs:61-69, rp64_256_jive/digest.rs:61-69): such a commitment or Merkle path node
+// stands for the reduced digest. The byte digests are taken as they are.
+void read_digest(int hash_id, const u8* q, Digest& dg) {
+    memcpy(dg.b, q, WF_DIGEST_BYTES(hash_id));
+    if (hash_id != WF_HASH_RP64_256 && hash_id != WF_HASH_RPJIVE64_256) return;
+    for (int k = 0; k < 4; k++) {
+        u64 w;
+        memcpy(&w, dg.b + 8 * k, 8);
+        if (w >= GL_P) w -= GL_P;
+        memcpy(dg.b + 8 * k, &w, 8);
+    }
+}
+// Every field element of a proof is read through BaseElement::read_from, which refuses a word >= p (math/src/field/f64/
+// mod.rs:673-681): the opened values (air/src/proof/table.rs:60-65), the OOD frames (ood_frame.rs:140,157), the FRI layer
+// values and the remainder (fri/src/proof.rs:185,321). VerifierChannel::new reports each as ProofDeserializationError
+// (verifier/src/channel.rs:92-118), after the acceptable options and the AIR (verifier/src/lib.rs:82-140).
+bool all_canonical(const Bytes& b, size_t skip = 0) {
+    for (size_t at = skip; at + 8 <= b.n; at += 8) {
+        u64 w;
+        memcpy(&w, b.p + at, 8);
+        if (w >= GL_P) return false;
+    }
+    return true;
+}
 struct Parsed {
     u32 logn = 0;
     Options o{};
@@ -284,7 +310,7 @@ u32 parse_proof(const AirHost& air, int hash_id, const u8* proof, size_t len, Pa
     const size_t dl = WF_DIGEST_BYTES(hash_id), ncm = nseg + 1 + pp.nl + 1;
     if (clen != dl * ncm) return WF_VERIFY_MALFORMED;
     pp.cm.assign(ncm, Digest{});
-    for (size_t i = 0; i < ncm; i++) memcpy(pp.cm[i].b, cm + dl * i, dl);
+    for (size_t i = 0; i < ncm; i++) read_digest(hash_id, cm + dl * i, pp.cm[i]);
     auto read_q = [&](Bytes& v, Bytes& pr) {
         v.n = r.usize(); v.p = r.take(v.n);
         if (!r.ok) return false;
@@ -310,6 +336,14 @@ u32 parse_proof(const AirHost& air, int hash_id, const u8* proof, size_t len, Pa
     pp.nonce = r.le(8);
     if (!r.ok || r.pos != len || pp.rem.n % (8 * d)) return WF_VERIFY_MALFORMED;
     return WF_VERIFY_ACCEPT;
+}
+bool values_canonical(const Parsed& pp) {
+    for (const Bytes* b : {&pp.tq_v, &pp.aq_v, &pp.cq_v, &pp.rem})
+        if (!all_canonical(*b)) return false;
+    if (!all_canonical(pp.ood_t, 1) || !all_canonical(pp.ood_q, 1)) return false;   // after the frame-size byte
+    for (const Bytes& b : pp.fv)
+        if (!all_canonical(b)) return false;
+    return true;
 }
 
 // ---- host: the batch plan ----
@@ -350,13 +384,13 @@ struct Plan {
 
     // BatchMerkleProof::get_root (crypto/src/merkle/proofs.rs:110-205) as a merge schedule. false: the opening does not parse,
     // has the wrong depth or does not open the given indexes (what makes the oracle's check fail before any hash is compared)
-    bool opening(const Bytes& path, size_t dl, size_t nleaves, const std::vector<u64>& idx, const std::vector<u32>& leaf_refs,
+    bool opening(const Bytes& path, int hash_id, size_t nleaves, const std::vector<u64>& idx, const std::vector<u32>& leaf_refs,
                  u32* root_ref) {
         Reader r{path.p, path.n};
         const u8 depth = r.u8_();
         const u64 nv = r.usize();
         if (!r.ok || nv > 100000 || depth < 1 || depth > 40) return false;
-        const size_t up0 = up.size();
+        const size_t dl = WF_DIGEST_BYTES(hash_id), up0 = up.size();
         auto undo = [&]() { up.resize(up0); return false; };
         std::vector<std::vector<u32>> nodes_of(nv);
         for (auto& v : nodes_of) {
@@ -366,7 +400,7 @@ struct Plan {
                 const u8* q = r.take(dl);
                 if (!q) return undo();
                 Digest dg{};
-                memcpy(dg.b, q, dl);
+                read_digest(hash_id, q, dg);
                 v.push_back(upload(dg));
             }
         }
@@ -612,12 +646,11 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
     }
     const u32 pidx = (u32)pl.pds.size();
     pl.pds.push_back(pd);
-    const size_t dl = WF_DIGEST_BYTES(h);
     // trace / constraint queries (verifier/src/channel.rs:206-260); rows hashed in partitions (channel.rs:431-453)
     std::vector<u32> t_refs, a_refs, c_refs;
     u32 root;
     auto open = [&](const Bytes& v, const Bytes& p, u32 words, u32 part, const Digest& want, u32 rank, u32 code, std::vector<u32>& refs) {
-        if (!pl.rows(v, pos.size(), words, part, refs) || !pl.opening(p, dl, N, pos, refs, &root)) { fail = fail_word(rank, code); return false; }
+        if (!pl.rows(v, pos.size(), words, part, refs) || !pl.opening(p, h, N, pos, refs, &root)) { fail = fail_word(rank, code); return false; }
         pl.cmps.push_back({j, fail_word(rank, code), root, pl.upload(want)});
         return true;
     };
@@ -645,7 +678,7 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
                 if ((p % P_) * psize + (p - p % P_) / P_ != p) { fail = fail_word(layer, WF_VERIFY_FRI_LAYER); return WF_OK; }
         }
         std::vector<u32> refs;
-        if (!pl.rows(pp.fv[depth], fpos.size(), nf * D, 0, refs) || !pl.opening(pp.fp[depth], dl, row_len, fpos, refs, &root)) {
+        if (!pl.rows(pp.fv[depth], fpos.size(), nf * D, 0, refs) || !pl.opening(pp.fp[depth], h, row_len, fpos, refs, &root)) {
             fail = fail_word(layer, WF_VERIFY_FRI_LAYER);
             return WF_OK;
         }
@@ -725,6 +758,7 @@ extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* 
             wf_ctx note{};
             if (air_check_host(&note, airs[j], pp.logn, pp.o.blowup) != WF_OK) v = WF_VERIFY_CONTEXT;
         }
+        if (v == WF_VERIFY_ACCEPT && !values_canonical(pp)) v = WF_VERIFY_MALFORMED;
         if (v != WF_VERIFY_ACCEPT) { fail[j] = fail_word(0, v); continue; }
         int r = pp.o.ext == 1 ? host_part<1>(call, j, airs[j], pp, pl, fail[j])
               : pp.o.ext == 2 ? host_part<2>(call, j, airs[j], pp, pl, fail[j]) : host_part<3>(call, j, airs[j], pp, pl, fail[j]);
