@@ -384,7 +384,9 @@ int wf_mat_evaluate_at(wf_ctx* ctx, const wf_mat* polys, uint32_t ext, uint32_t 
                        uint64_t* out0, uint64_t* out1);
 /* DeepCompositionPoly::{add_trace_polys, add_composition_poly, evaluate} (prover/src/composer/mod.rs:67-210):
  * DEEP composition evaluated over the LDE domain, N x ext. coeffs / ood_cur / ood_next: [width + aux_width +
- * composition columns][ext] in that order (DeepCompositionCoefficients, TraceOodFrame + QuotientOodFrame rows). */
+ * composition columns][ext] in that order (DeepCompositionCoefficients, TraceOodFrame + QuotientOodFrame rows).
+ * WF_ERR_INVALID when z or z*g lies on the LDE domain 7 <w_N> (a base-field point with (point / 7)^N = 1): some row's
+ * denominator x - z vanishes there. wf_deep_compose_polys is exact at such a point. */
 int wf_deep_compose(wf_ctx* ctx, uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const wf_mat* cons_lde, uint32_t log_n,
                     const uint64_t* z, const uint64_t* coeffs, const uint64_t* ood_cur, const uint64_t* ood_next, wf_mat** out);
 /* The same DEEP composition from the COEFFICIENT matrices, as the reference builds it: S = sum_j coeffs_j p_j over the n
@@ -493,6 +495,10 @@ int wf_rescue_permute_dev(wf_ctx* ctx, int hash_id, const uint64_t* d_states, co
  * inverses extensions/quadratic.rs:81-94, cubic.rs:81-97): a, b = n elements of `ext` (2 | 3) canonical words each (device);
  * d_out = 6 blocks of n elements: a*b, 1/a (0 for 0), frobenius(a), a.mul_base(b[0]), a+b, a-b. */
 int wf_ext_ops_dev(wf_ctx* ctx, uint32_t ext, const uint64_t* d_a, const uint64_t* d_b, size_t n, uint64_t* d_out);
+/* the delayed-reduction dot product of the OOD, DEEP-sum and constraint kernels (GlAcc: acc_zero / acc_mad / acc_reduce,
+ * gl64.cuh) on n rows of k terms (1 <= k < 2^31): d_x, d_y = [n][k] ANY 64-bit words (device). d_out = [n][6] words: the raw
+ * 160-bit accumulator sum_j x_j y_j as w0..w4 (32-bit words, w0 lowest, one per output word), then its reduction mod p. */
+int wf_acc_ops_dev(wf_ctx* ctx, const uint64_t* d_x, const uint64_t* d_y, uint32_t k, size_t n, uint64_t* d_out);
 
 /* ---- host-side helpers of the product (transcript arithmetic; no GPU needed) ------------------- */
 /* H::hash_elements / merge / merge_with_int on the host (crypto/src/hash/mod.rs:31-64) */

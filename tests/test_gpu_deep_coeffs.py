@@ -12,6 +12,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import combine_model as M
 import winterfell_b200 as wf
 
 P = wf.P
@@ -73,17 +74,6 @@ def test_coefficient_form_matches_evaluation_form(ctx, oracle, ext, c, aw, kc, l
             o.free()
 
 
-def _host_syn_div(oracle, s, b, ext):
-    """syn_div(p, 1, b) of polynom/mod.rs:498-505, serially: q_i = s_(i+1) + b q_(i+1), q_(n-1) = 0."""
-    mul = (lambda x, y: oracle.ext_mul(x, y)) if ext > 1 else (lambda x, y: np.array([oracle.mul(int(x[0]), int(y[0]))], dtype=np.uint64))
-    q = np.zeros_like(s)
-    acc = np.zeros(ext, dtype=np.uint64)
-    for i in range(len(s) - 1, 0, -1):
-        acc = np.array([(int(u) + int(v)) % P for u, v in zip(s[i], mul(b, acc))], dtype=np.uint64)
-        q[i - 1] = acc
-    return q
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("ext,log_n", [(1, 3), (3, 3), (2, 11), (3, 12), (1, 13)])
 def test_division_matches_serial_syn_div(ctx, oracle, ext, log_n):
@@ -106,7 +96,7 @@ def test_division_matches_serial_syn_div(ctx, oracle, ext, log_n):
             s[i] = [(int(u) + int(v)) % P for u, v in zip(s[i], t)]
     zg = oracle.ext_mul(z, np.array([oracle.root_of_unity(log_n)] + [0] * (ext - 1), dtype=np.uint64)) if ext > 1 \
         else np.array([oracle.mul(int(z[0]), oracle.root_of_unity(log_n))], dtype=np.uint64)
-    qz, qzg = _host_syn_div(oracle, s, z, ext), _host_syn_div(oracle, s, zg, ext)
+    qz, qzg = M.host_syn_div(oracle, s, z, ext), M.host_syn_div(oracle, s, zg, ext)
     want = np.array([[(int(u) + int(v)) % P for u, v in zip(a, b)] for a, b in zip(qz, qzg)], dtype=np.uint64)
     assert np.array_equal(coef[:n], want)
     assert not coef[n:].any()

@@ -116,6 +116,7 @@ _SIGS = [
     ("wf_rescue_ops_dev", C.c_int, [vp, vp, vp, C.c_size_t, vp]),
     ("wf_rescue_permute_dev", C.c_int, [vp, C.c_int, vp, vp, C.c_size_t, vp]),
     ("wf_ext_ops_dev", C.c_int, [vp, C.c_uint32, vp, vp, C.c_size_t, vp]),
+    ("wf_acc_ops_dev", C.c_int, [vp, vp, vp, C.c_uint32, C.c_size_t, vp]),
     ("wf_ctx_set_jit", C.c_int, [vp, C.c_int]),
     ("wf_ctx_jit_stats", C.c_int, [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     ("wf_jit_compile_air", C.c_int, [u64p, C.c_size_t, C.c_uint32, C.POINTER(C.c_size_t), C.c_char_p, C.c_size_t]),
@@ -648,6 +649,10 @@ class Context:
 
     def ext_ops_dev(self, ext, d_a, d_b, n, d_out):
         self.check(self.L.wf_ext_ops_dev(self.h, ext, vp(d_a), vp(d_b), n, vp(d_out)))
+
+    def acc_ops_dev(self, d_x, d_y, k, n, d_out):
+        """n delayed-reduction dot products of k terms: d_out = [n][6] words, w0..w4 of the accumulator and its reduction"""
+        self.check(self.L.wf_acc_ops_dev(self.h, vp(d_x), vp(d_y), k, n, vp(d_out)))
 
     def fri_fold_dev(self, d_evals, length, ext_degree, folding, alpha, d_next):
         a_, ap = _u64(alpha)

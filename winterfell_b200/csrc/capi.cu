@@ -470,6 +470,18 @@ __global__ void ext_ops_kernel(const u64* a, const u64* b, size_t n, u64* out) {
         for (int q = 0; q < D; q++) out[((size_t)k * n + i) * D + q] = r[k].v[q];
 }
 
+// delayed-reduction dot products (wf_acc_ops_dev): n rows of k terms through acc_zero / acc_mad / acc_reduce, the accumulator
+// of the OOD, DEEP-sum and FibSmall constraint kernels. out[i] = w0..w4 of the raw accumulator, then its reduction.
+__global__ void acc_ops_kernel(const u64* x, const u64* y, u32 k, size_t n, u64* out) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    GlAcc a = acc_zero();
+    for (u32 j = 0; j < k; j++) acc_mad(a, x[i * k + j], y[i * k + j]);
+    u64* o = out + i * 6;
+    o[0] = a.w0; o[1] = a.w1; o[2] = a.w2; o[3] = a.w3; o[4] = a.w4;
+    o[5] = acc_reduce(a);
+}
+
 template <int K>
 static u64 m2e(u64 x) { return gl_mul_2exp<K>(x); }
 
@@ -1446,6 +1458,15 @@ int wf_ext_ops_dev(wf_ctx* ctx, uint32_t ext, const uint64_t* d_a, const uint64_
     const unsigned blocks = (unsigned)((n + 127) / 128);
     if (ext == 2) ext_ops_kernel<2><<<blocks, 128, 0, ctx->st>>>(d_a, d_b, n, d_out);
     else ext_ops_kernel<3><<<blocks, 128, 0, ctx->st>>>(d_a, d_b, n, d_out);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return WF_OK;
+}
+// the delayed-reduction accumulator on caller-chosen products: uniform data almost never reaches its carry ripples, a
+// reduction that lands on 0 or p - 1, or the borrow of the final subtraction of w4 2^128, so tests feed aimed sums
+int wf_acc_ops_dev(wf_ctx* ctx, const uint64_t* d_x, const uint64_t* d_y, uint32_t k, size_t n, uint64_t* d_out) {
+    if (!ctx || !d_x || !d_y || !d_out || n == 0 || k == 0 || k >= (1u << 31)) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    acc_ops_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->st>>>(d_x, d_y, k, n, d_out);
     ctx->launches++;
     CK(cudaGetLastError());
     return WF_OK;

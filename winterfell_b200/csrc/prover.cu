@@ -422,8 +422,7 @@ __global__ void __launch_bounds__(256, DEEP_DIV_MINB) deep_div_kernel(DeepParams
         den[2 * r] = deep_m<D>(pz, x, x2);
         den[2 * r + 1] = deep_m<D>(pzg, x, x2);
     }
-    // batch inversion in the base field; the norms are never zero (z is outside the base-field LDE domain with overwhelming
-    // probability; a zero would also break the reference's synthetic division)
+    // batch inversion in the base field; the norms are never zero (deep_compose refuses a z or z*g on the LDE domain)
     u64 pre[2 * ROWS], run = 1;
 #pragma unroll
     for (int q = 0; q < 2 * ROWS; q++) { pre[q] = run; run = gl_mul(run, den[q]); }
@@ -1095,6 +1094,16 @@ int deep_compose(wf_ctx* ctx, const wf_mat* lde, const wf_mat* alde, const wf_ma
     // nrows != 0: row-sharded call — the matrices hold LDE rows [row0, row0 + nrows) only
     const u32 c = lde->m.cols, aw = alde ? alde->m.cols / D : 0, ct = c + aw;
     const size_t N = nrows ? nrows : ((size_t)1 << log_N);
+    // x - z vanishes at a row x = 7 w_N^i only for z in the base field with (z / 7)^N = 1 (outside the base field the norm of x - z
+    // is nonzero); the batch inversion would then zero the inverses of a whole thread's rows, so such a point is refused
+    for (const GlExt<D>* w : {&z, &zg}) {
+        bool base = true;
+        for (int q = 1; q < D; q++) base = base && w->v[q] == 0;
+        if (base && gl_sqr_n(gl_mul(w->v[0], 2635249152773512046ULL), (int)log_N) == 1)  // 7^-1 mod p
+            return wf_fail(ctx, WF_ERR_INVALID, "DEEP point %s lies on the LDE domain: its denominators vanish", w == &z ? "z" : "z*g");
+    }
+    DeepPoint<D> pz, pzg;
+    if (!deep_point<D>(z, pz) || !deep_point<D>(zg, pzg)) return wf_fail(ctx, WF_ERR_STATE, "conjugates of the out-of-domain point are inconsistent");
     u64 *d_dt, *d_dq, *d_da;
     CKI(upload_ext<D>(ctx, dc, 0, ct + kc, &d_dt));  // one upload (one synchronisation) for all coefficients
     d_da = d_dt + (size_t)c * D;
@@ -1111,8 +1120,6 @@ int deep_compose(wf_ctx* ctx, const wf_mat* lde, const wf_mat* alde, const wf_ma
     deep_sum_kernel<D><<<(unsigned)((N + DEEP_SUM_THREADS - 1) / DEEP_SUM_THREADS), DEEP_SUM_THREADS, coef_bytes, ctx->st>>>(p);
     const size_t rows_per_thread = DEEP_ROWS;
     size_t threads = (N + rows_per_thread - 1) / rows_per_thread;
-    DeepPoint<D> pz, pzg;
-    if (!deep_point<D>(z, pz) || !deep_point<D>(zg, pzg)) return wf_fail(ctx, WF_ERR_STATE, "conjugates of the out-of-domain point are inconsistent");
     deep_div_kernel<D><<<(unsigned)((threads + 255) / 256), 256, 0, ctx->st>>>(p, pz, pzg, Sz, Szg);
     ctx->launches += 2;
     CK(cudaGetLastError());
