@@ -433,8 +433,13 @@ typedef struct wf_comm {
     int (*fork)(void* user);
     int (*join)(void* user);
 } wf_comm;
-/* FibSmall x k (as wf_prove_fib) sharded over comm->world GPUs: this rank passes ITS 2k/world columns (host columns, or
- * d_local = device column-major [2k/world][2^log_n]); 2k/world must be a multiple of 8 (whole 8-column segments).
+/* The main-trace columns [*first, *first + *count) that `rank` of `world` (a power of two) owns in a sharded proof of a trace
+ * of `width` (1..255) columns: contiguous runs of whole 8-column segments in rank order, the first (segments mod world) ranks
+ * one segment more than the others; the last segment may be partly filled and trailing ranks may own no column. Needs no
+ * device. WF_ERR_INVALID for a world that is not a power of two, a rank outside it or a width outside 1..255. */
+int wf_shard_columns(uint32_t width, uint32_t world, uint32_t rank, uint32_t* first, uint32_t* count);
+/* FibSmall x k (as wf_prove_fib) sharded over comm->world GPUs: this rank passes ITS columns, wf_shard_columns(2k, world,
+ * rank) (host columns, or d_local = device column-major [count][2^log_n]).
  * `results` and `opts` are the full proof's; every rank returns the same proof bytes.
  * stats (optional, 8 doubles): [0] bytes this rank sent through exchanges ordered on the ctx stream, [1] ms inside those,
  * [2] number of collectives, [3] ms inside all_gather_host + all_reduce_sum, [4] FRI layers folded on shards, [5] bytes sent
@@ -443,6 +448,23 @@ typedef struct wf_comm {
  * (the driver refused the mapping, or WF_PEER_PUSH=0). */
 int wf_prove_fib_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* const* local_cols, const uint64_t* d_local, int mont,
                          uint32_t k, uint32_t log_n, const uint64_t* results, const uint32_t* opts, uint8_t* proof,
+                         size_t* proof_len, double* stats);
+/* A user-described AIR (the description of wf_prove_air / wf_prove_air_aux_built) sharded over comm->world GPUs. Every rank
+ * passes the same description, options, log_n and aux build, plus its own block of main-trace columns: local_count =
+ * wf_shard_columns(width, world, rank)'s count, as host columns (local_cols, representation by `mont`) or device memory
+ * (d_local, column-major [local_count][2^log_n], canonical); a rank that owns no column passes local_count = 0 and may pass
+ * NULL for both. Single-segment AIR: aux_build = NULL, aux_assertions = NULL; every rank returns the bytes wf_prove_air gives
+ * for the whole trace. Two-segment AIR: aux_build is required (host-callback builders are not supported here); every rank
+ * gathers the whole main trace (n * width * 8 bytes of device memory per rank), builds the aux segment on the device with the
+ * transcript's random elements and returns the bytes wf_prove_air_aux_built gives; aux_assertions (may be NULL) is called on
+ * every rank with the same random elements, as there. stats as wf_prove_fib_sharded. wf_ctx_set_validation's checks are not
+ * run. Refusals (WF_ERR_INVALID / WF_ERR_UNSUPPORTED: a world that is not a power of two >= 2, a trace too short for the
+ * world, a description that fails wf_air_check, a bad aux build, a local_count that is not this rank's) happen before any
+ * device buffer is allocated, and every rank returns an error: the checks on shared values need no communication, and every
+ * rank's verdict on its own block is all-gathered before the first exchange. */
+int wf_prove_air_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build,
+                         size_t aux_build_len, wf_aux_assertions_fn aux_assertions, void* aux_user, const uint64_t* const* local_cols,
+                         const uint64_t* d_local, uint32_t local_count, int mont, uint32_t log_n, const uint32_t* opts, uint8_t* proof,
                          size_t* proof_len, double* stats);
 
 /* ---- constraint kernels compiled per AIR ---------------------------------------------------------------------------

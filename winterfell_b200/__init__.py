@@ -142,6 +142,9 @@ _SIGS = [
     ("wf_host_sharded_opening_plan", C.c_long, [C.c_size_t, C.c_int, C.c_int, u64p, C.c_size_t, u64p, u64p, C.c_size_t]),
     ("wf_prove_fib_sharded", C.c_int, [vp, vp, C.POINTER(u64p), vp, C.c_int, C.c_uint32, C.c_uint32, u64p, C.POINTER(C.c_uint32), u8p,
                                        C.POINTER(C.c_size_t), C.POINTER(C.c_double)]),
+    ("wf_shard_columns", C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    ("wf_prove_air_sharded", C.c_int, [vp, vp, u64p, C.c_size_t, u64p, C.c_size_t, AUX_BUILDER, vp, C.POINTER(u64p), vp, C.c_uint32,
+                                       C.c_int, C.c_uint32, C.POINTER(C.c_uint32), u8p, C.POINTER(C.c_size_t), C.POINTER(C.c_double)]),
 ]
 
 

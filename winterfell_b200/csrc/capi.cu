@@ -751,11 +751,13 @@ int wf_trace_lde_cosetwise(wf_ctx* ctx, const uint64_t* const* cols, const uint6
     u32 log_n;
     if (log2_exact(nrows, &log_n) || log_n < 1) return wf_fail(ctx, WF_ERR_INVALID, "rows must be a power of two >= 2");
     if (log_blowup > 7 || log_n + log_blowup > 32) return wf_fail(ctx, WF_ERR_INVALID, "bad blowup");
-    const int Wout = seg_width_for(ncols);
+    // a coset-major output may be wider than the columns need (a sharded proof's partly filled last segment is staged at width 8)
+    if (coset_major && (!*lde_out || (*lde_out)->m.rows != (nrows << log_blowup) || (*lde_out)->m.W < seg_width_for(ncols) ||
+                        (*lde_out)->m.cols != ncols))
+        return wf_fail(ctx, WF_ERR_INVALID, "coset-major output must be preallocated");
+    const int Wout = coset_major ? (*lde_out)->m.W : seg_width_for(ncols);
     const u32 nseg_out = (ncols + Wout - 1) / Wout;
     const u32 nb = 1u << log_blowup;
-    if (coset_major && (!*lde_out || (*lde_out)->m.rows != (nrows << log_blowup) || (*lde_out)->m.W != Wout || (*lde_out)->m.cols != ncols))
-        return wf_fail(ctx, WF_ERR_INVALID, "coset-major output must be preallocated");
     // cosets of one column chunk: all at once, or one by one with the callback when this is the last chunk
     auto extend = [&](const SegMatrix& pv, SegMatrix& ov, u32 out_col0, bool last) -> int {
         if (!after_coset || !last) {
@@ -783,7 +785,17 @@ int wf_trace_lde_cosetwise(wf_ctx* ctx, const uint64_t* const* cols, const uint6
         if (r != WF_OK) return r;
         if (!coset_major && !after_coset) return wf_mat_lde(ctx, *polys_out, log_blowup, lde_out);
         if (!coset_major) CKI(wf_mat_alloc(ctx, nrows << log_blowup, ncols, lde_out));
-        return extend((*polys_out)->m, (*lde_out)->m, 0, true);
+        const SegMatrix& pm = (*polys_out)->m;
+        if (pm.W == Wout) return extend(pm, (*lde_out)->m, 0, true);
+        for (u32 g = 0; g < pm.nseg(); g++) {   // narrower coefficient segments, each into its place in a wider output segment
+            SegMatrix pv = pm, ov = (*lde_out)->m;
+            pv.base += (size_t)g * pm.seg_stride;
+            pv.cols = std::min<u32>(pm.W, ncols - g * pm.W);
+            ov.base += (size_t)(g * pm.W / Wout) * ov.seg_stride;
+            ov.cols = pv.cols;
+            CKI(extend(pv, ov, g * pm.W % Wout, g + 1 == pm.nseg()));
+        }
+        return WF_OK;
     }
     if (!ctx->copy_st) {
         CK(cudaStreamCreateWithFlags(&ctx->copy_st, cudaStreamNonBlocking));

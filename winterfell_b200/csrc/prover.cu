@@ -840,14 +840,13 @@ static int sequence_table(wf_ctx* ctx, const u64* values, size_t L, u32 words_pe
 template <int D>
 int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const wf_mat* alde, const std::vector<GlExt<D>>& cc,
                      const std::vector<u64>& rnd_flat, u32 log_n, u32 log_b, wf_mat** out, size_t row0 = 0, size_t ce_rows = 0) {
-    // ce_rows != 0: row-sharded call — CE rows [row0, row0 + ce_rows) only; `lde` then holds the LDE rows of that range
-    // followed by `blowup` halo rows (FibEvalParams::row0)
+    // ce_rows != 0: row-sharded call — CE rows [row0, row0 + ce_rows) only; `lde` (and `alde`) then hold the LDE rows of that
+    // range followed by `blowup` halo rows (FibEvalParams::row0, GenEvalParams::row0)
     const size_t n = (size_t)1 << log_n;
     const u32 c = air.w, aw = air.aw, log_ceb = air.log_ce_blowup();
     const u32 n_atr = (u32)air.aux_degrees.size(), n_mtr = (u32)air.degrees.size(), n_mas = (u32)air.asserts.size();
     const u32 n_tr = n_mtr + n_atr;
     const size_t ce = n << log_ceb;
-    if (ce_rows && !air.is_fib) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "row-sharded constraint evaluation covers the FibSmall family");
     wf_mat* comp;
     CKI(wf_mat_alloc(ctx, ce_rows ? ce_rows : ce, D, &comp));
     if (comp->m.W > D) CK(cudaMemsetAsync(comp->m.base, 0, comp->m.words() * 8, ctx->st));
@@ -968,6 +967,7 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
         CKI(upload(eshift.data(), eshift.size() * 4, &dp)); p.e_shift = (u32*)dp;
         CKI(wf_get_twiddles(ctx, log_n + log_ceb, &p.tw_ce));
         CKI(upload(zt.data(), zt.size() * 8, &dp)); p.zt = (const u64*)dp;
+        p.row0 = row0; p.ce_rows = ce_rows;
         p.num_exempt = air.exemptions;
         for (u32 e = 0; e < air.exemptions; e++) p.exempt[e] = gl_pow(g_tr, n - air.exemptions + e);  // divisor.rs:31-41
         std::vector<u32> agoff = {0}, aecol, aetstride, aeshift;
@@ -1017,13 +1017,14 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
         const bool jit = ctx->jit_enabled &&
                          wf_jit_get_kernel(ctx, wf_jit_source(D, air.w, (u32)air.periodic.size(), air.num_regs, air.prog, air.consts, aw, air.nr,
                                                               air.aux_num_regs, air.aux_prog), &jk) == WF_OK;
+        const unsigned blocks = (unsigned)(((ce_rows ? ce_rows : ce) + 127) / 128);
         if (jit) {
             void* args[] = {&p};
-            CK(cudaLaunchKernel((const void*)jk, dim3((unsigned)((ce + 127) / 128)), dim3(128), args, 0, ctx->st));
+            CK(cudaLaunchKernel((const void*)jk, dim3(blocks), dim3(128), args, 0, ctx->st));
         } else if (aw) {
-            generic_constraints_kernel<D, true><<<(unsigned)((ce + 127) / 128), 128, 0, ctx->st>>>(p);
+            generic_constraints_kernel<D, true><<<blocks, 128, 0, ctx->st>>>(p);
         } else {
-            generic_constraints_kernel<D, false><<<(unsigned)((ce + 127) / 128), 128, 0, ctx->st>>>(p);
+            generic_constraints_kernel<D, false><<<blocks, 128, 0, ctx->st>>>(p);
         }
         ctx->launches++;
         CK(cudaGetLastError());
@@ -1374,7 +1375,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
 }
 
 // =================================================================================================
-// One proof sharded over several GPUs (include/winterfell_b200.h: wf_comm, wf_prove_fib_sharded)
+// One proof sharded over several GPUs (include/winterfell_b200.h: wf_comm, wf_prove_fib_sharded, wf_prove_air_sharded)
 // =================================================================================================
 // staging: [b cosets][rows_j][W] (per segment) -> natural order row j * b + k of the row shard
 __global__ void __launch_bounds__(256) coset_interleave_kernel(SegMatrix src, SegMatrix dst, size_t rows_j, u32 b) {
@@ -1511,32 +1512,161 @@ static int shard_tree_finish(ShardCtx& sc, int h, ShardTree& t, Digest* root) {
     return WF_OK;
 }
 
+// Columns [first, first + count) of a `w`-column trace that rank r of G owns (wf_shard_columns): contiguous runs of whole
+// 8-column segments, the first (segments mod G) ranks one segment more than the others; the last segment may be partly filled
+// and trailing ranks may own none. With a segment count divisible by G every rank owns the same number of whole segments.
+static void shard_segments(u32 w, u32 G, u32 r, u32& seg0, u32& nseg) {
+    const u32 S = (w + 7) / 8, base = S / G, extra = S % G;
+    seg0 = r * base + std::min(r, extra);
+    nseg = base + (r < extra ? 1u : 0u);
+}
+static void shard_columns(u32 w, u32 G, u32 r, u32& first, u32& count) {
+    u32 s0, ns;
+    shard_segments(w, G, r, s0, ns);
+    first = std::min(w, s0 * 8);
+    count = std::min(w, (s0 + ns) * 8) - first;
+}
+
+// rows [m.rows, m.rows + b) of every segment of `m` (allocated with b rows more than m.rows) <- the first b rows of every
+// segment of rank (r + 1) mod G: the next-state rows of the last rows of a row shard
+static int exchange_halo(ShardCtx& sc, const SegMatrix& m, size_t b) {
+    wf_ctx* ctx = sc.ctx;
+    DevScratch tmp(ctx);
+    void *pk, *pk2;
+    const size_t hb = b * m.W * 8;
+    const u32 nsg = m.nseg();
+    CKI(tmp.alloc(hb * nsg, &pk));
+    CKI(tmp.alloc(hb * nsg, &pk2));
+    CK(cudaMemcpy2DAsync(pk, hb, m.base, m.seg_stride * 8, hb, nsg, cudaMemcpyDeviceToDevice, ctx->st));
+    CKI(sc.exchange({(sc.r + sc.G - 1) % sc.G}, {pk}, {(sc.r + 1) % sc.G}, {pk2}, hb * nsg));
+    CK(cudaMemcpy2DAsync(m.base + m.rows * m.W, m.seg_stride * 8, pk2, hb, hb, nsg, cudaMemcpyDeviceToDevice, ctx->st));
+    return WF_OK;
+}
+
+// This rank's LDE rows [r N/G, (r+1) N/G) of polynomials every rank holds, too few columns to shard by column (the composition
+// polynomial, the aux segment). With blowup % G == 0 the LDE is sharded by COSET: rank r extends cosets [r b/G, (r+1) b/G)
+// (coset-major), one exchange hands every rank the rows of its range from every coset's owner, one kernel interleaves them into
+// natural order (row = b j + k). Otherwise every rank extends the whole polynomial and keeps its range. `halo`: the result also
+// holds the first `blowup` rows of rank (r + 1) mod G's range after its own (rows stays N/G), as the trace's row shard does.
+// *out: the matrix to free; `view`: the row range (without halo it may point into a replicated whole LDE held by *out).
+static int shard_lde_rows(ShardCtx& sc, const wf_mat* polys, u32 log_b, bool halo, wf_mat** out, wf_mat& view) {
+    wf_ctx* ctx = sc.ctx;
+    const int G = sc.G, r = sc.r;
+    const size_t n = polys->m.rows, b = (size_t)1 << log_b, rows_per = (n << log_b) / (size_t)G;
+    const int W = polys->m.W;
+    const u32 cols = polys->m.cols;
+    if (b % (size_t)G != 0) {
+        wf_mat *full = nullptr, *rows = nullptr;
+        CKI(wf_mat_lde(ctx, polys, log_b, &full));
+        if (!halo) {
+            *out = full;
+            view.m = full->m;
+            view.m.base += (size_t)r * rows_per * full->m.W;
+            view.m.rows = rows_per;
+            return WF_OK;
+        }
+        int rc = wf_mat_alloc_w(ctx, rows_per + b, cols, full->m.W, &rows);
+        if (rc == WF_OK) {
+            rows->m.rows = rows_per;
+            const size_t rb = (size_t)full->m.W * 8, sp = full->m.seg_stride * 8, dp = rows->m.seg_stride * 8;
+            const u32 nsg = full->m.nseg();
+            cudaError_t e = cudaMemcpy2DAsync(rows->m.base, dp, full->m.base + (size_t)r * rows_per * full->m.W, sp, rows_per * rb, nsg,
+                                              cudaMemcpyDeviceToDevice, ctx->st);
+            if (e == cudaSuccess)
+                e = cudaMemcpy2DAsync(rows->m.base + rows_per * full->m.W, dp, full->m.base + (size_t)((r + 1) % G) * rows_per * full->m.W, sp,
+                                      b * rb, nsg, cudaMemcpyDeviceToDevice, ctx->st);
+            if (e != cudaSuccess) rc = wf_fail(ctx, WF_ERR_CUDA, "row shard copy: %s", cudaGetErrorString(e));
+        }
+        wf_mat_free(ctx, full);
+        if (rc != WF_OK) { wf_mat_free(ctx, rows); return rc; }
+        *out = rows;
+        view.m = rows->m;
+        return WF_OK;
+    }
+    const u32 kpr = (u32)(b / (size_t)G);
+    const size_t nj = n / (size_t)G;     // points of every coset that fall into one rank's row range
+    wf_mat *ccos = nullptr, *stage = nullptr, *lde = nullptr;
+    int rc = wf_mat_alloc_w(ctx, (size_t)kpr * n, cols, W, &ccos);
+    if (rc == WF_OK) rc = wf_mat_lde_cosets(ctx, polys, log_b, (u32)r * kpr, (u32)(r + 1) * kpr, ccos);
+    if (rc == WF_OK) rc = wf_mat_alloc_w(ctx, rows_per, cols, W, &stage);
+    if (rc == WF_OK) rc = wf_mat_alloc_w(ctx, rows_per + (halo ? b : 0), cols, W, &lde);
+    if (rc == WF_OK) {
+        lde->m.rows = rows_per;
+        const size_t blk = nj * W;       // words of one (coset, destination) block of one segment
+        std::vector<int> sp, rp;
+        std::vector<const void*> sv;
+        std::vector<void*> rv;
+        for (u32 sg = 0; sg < ccos->m.nseg(); sg++) {
+            const u64* cb = ccos->m.base + (size_t)sg * ccos->m.seg_stride;
+            u64* sb = stage->m.base + (size_t)sg * stage->m.seg_stride;
+            for (u32 kl = 0; kl < kpr; kl++)
+                for (int q = 0; q < G; q++) {
+                    const u64* src = cb + ((size_t)kl * n + (size_t)q * nj) * W;
+                    if (q == r) CK(cudaMemcpyAsync(sb + ((size_t)r * kpr + kl) * blk, src, blk * 8, cudaMemcpyDeviceToDevice, ctx->st));
+                    else { sp.push_back(q); sv.push_back(src); }
+                }
+            for (u32 k = 0; k < (u32)b; k++) {
+                const int owner = (int)(k / kpr);
+                if (owner != r) { rp.push_back(owner); rv.push_back(sb + (size_t)k * blk); }
+            }
+        }
+        // pairwise order: sender r -> q lists (segment, local coset) ascending; receiver q <- s lists (segment, coset) ascending
+        rc = sc.exchange(sp, sv, rp, rv, blk * 8);
+        if (rc == WF_OK) {
+            dim3 grid((unsigned)((rows_per * W + 255) / 256), lde->m.nseg());
+            coset_interleave_kernel<<<grid, 256, 0, ctx->st>>>(stage->m, lde->m, nj, (u32)b);
+            ctx->launches++;
+            if (cudaGetLastError() != cudaSuccess) rc = wf_fail(ctx, WF_ERR_CUDA, "coset_interleave_kernel launch failed");
+        }
+    }
+    wf_mat_free(ctx, ccos);
+    wf_mat_free(ctx, stage);
+    if (rc == WF_OK && halo) rc = exchange_halo(sc, lde->m, b);
+    if (rc != WF_OK) { wf_mat_free(ctx, lde); return rc; }
+    *out = lde;
+    view.m = lde->m;
+    return WF_OK;
+}
+
+// One proof of `air_in` sharded over the ranks of `cm` (wf_prove_air_sharded, wf_prove_fib_sharded). Rank r owns the main-trace
+// columns shard_columns() gives it: local_cols / d_local hold exactly those (none: both may be NULL). aux_build: the described
+// build of a two-segment AIR's aux segment (replicated on every rank from the all-gathered main trace).
 template <int D>
-int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* local_cols, const uint64_t* d_local, int mont, u32 k,
-                      u32 log_n, const u64* results, const Options& o, std::vector<u8>& proof_out, double* stats) {
+int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const AuxBuildHost* aux_build, wf_aux_assertions_fn aux_assertions,
+                  void* aux_user, const uint64_t* const* local_cols, const uint64_t* d_local, int mont, u32 log_n, const Options& o,
+                  std::vector<u8>& proof_out, double* stats) {
+    AirHost air_dyn;                       // copy whose aux assertion values are rewritten from the random elements (as prove_air)
+    if (aux_assertions) air_dyn = air_in;
+    const AirHost& air = aux_assertions ? air_dyn : air_in;
     ShardCtx sc{ctx, cm, cm->world, cm->rank};
     const int G = sc.G, r = sc.r;
     const int h = o.hash_id;
     const size_t n = (size_t)1 << log_n;
     const u32 log_b = log2_ceil(o.blowup);
     const size_t N = n << log_b, b = o.blowup;
-    const u32 c = 2 * k, cl = c / (u32)G, nsl = cl / 8, nsg = c / 8;
+    const u32 c = air.w, aw = air.aw, nsg = (c + 7) / 8;
     const size_t rows_per = N / (size_t)G;
     if (G < 2 || (G & (G - 1)) || r < 0 || r >= G) return wf_fail(ctx, WF_ERR_INVALID, "world size must be a power of two >= 2");
-    if (c % (u32)G || cl % 8) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "each rank must own whole 8-column segments (2k / world a multiple of 8)");
-    const AirHost air = fib_air_host(k, n, results);
+    if (aw && !aux_build) return wf_fail(ctx, WF_ERR_INVALID, "multi-segment AIR needs an aux build description");
+    std::vector<u32> seg0(G), segs(G), col0(G), ncol(G);   // every rank's block: first segment, segments, first column, columns
+    for (int q = 0; q < G; q++) {
+        shard_segments(c, (u32)G, (u32)q, seg0[q], segs[q]);
+        shard_columns(c, (u32)G, (u32)q, col0[q], ncol[q]);
+    }
+    const u32 cl = ncol[r], fs = seg0[r], nsl = segs[r];
+    const u32 maxcl = *std::max_element(ncol.begin(), ncol.end());
     const u32 kc = air.num_comp_cols(n), log_ceb = air.log_ce_blowup();
     const size_t ce = n << log_ceb, ce_per = ce / (size_t)G;
     if (rows_per < 64 * b || ce_per < 64) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "trace too short to shard over %d ranks", G);
     Channel ch(h, context_seed(air, n, o));  // every rank replays the whole transcript
 
-    wf_mat *trace = nullptr, *polys = nullptr, *lde = nullptr, *shard = nullptr, *comp_l = nullptr, *comp = nullptr, *cpolys = nullptr,
-           *clde = nullptr, *deep = nullptr, *fri_in = nullptr, *tstage = nullptr;
-    ShardTree ttree, ctree;
+    wf_mat *polys = nullptr, *lde = nullptr, *shard = nullptr, *mtrace = nullptr, *atrace = nullptr, *apolys = nullptr, *arows = nullptr,
+           *comp_l = nullptr, *comp = nullptr, *cpolys = nullptr, *clde = nullptr, *deep = nullptr, *fri_in = nullptr, *tstage = nullptr;
+    ShardTree ttree, atree, ctree;
     wf_fri* fri = nullptr;
     ProofScope scope(ctx);   // holds the ADDRESSES of these pointers: every owned pointer lives as long as the scope
-    scope.own({&trace, &polys, &lde, &shard, &comp_l, &comp, &cpolys, &clde, &deep, &fri_in, &tstage});
-    scope.own({&ttree.local, &ctree.local});
+    scope.own({&polys, &lde, &shard, &mtrace, &atrace, &apolys, &arows, &comp_l, &comp, &cpolys, &clde, &deep, &fri_in, &tstage});
+    scope.own({&ttree.local, &atree.local, &ctree.local});
     scope.fri = &fri;
     struct SLayer { u64* vals; size_t m_l, m_g; ShardTree tree; };
     std::vector<SLayer> slayers;   // FRI layers folded on row shards
@@ -1548,14 +1678,15 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
 
     // ---- 1. interpolate the local columns, then extend them coset by coset (no communication: columns are independent).
     //         Coset k is written coset-major, so that the rows of rank q's range (n / G points of the coset) are one contiguous
-    //         block per segment: its exchange runs on the communicator's stream while coset k + 1 is being extended ----
+    //         block per segment: its exchange runs on the communicator's stream while coset k + 1 is being extended. A rank that
+    //         owns no columns only receives ----
     wf_mark(ctx, "start");
     const size_t nj = n / (size_t)G;   // points of one coset inside one rank's row range
-    CKI(wf_mat_alloc(ctx, rows_per + b, c, &shard));
+    // the row shard and the staging matrix hold all c columns in 8-column segments, a partly filled last one included
+    CKI(wf_mat_alloc_w(ctx, rows_per + b, c, 8, &shard));
     shard->m.rows = rows_per;  // seg_stride stays (rows_per + b) * 8: rows [rows_per, rows_per + b) are the halo
-    const size_t sstride = shard->m.seg_stride;
     wf_mat*& stage = tstage;           // what arrives: [global segment][coset][nj][8]
-    CKI(wf_mat_alloc_w(ctx, N, cl, 8, &lde));          // mine, coset-major: [local segment][coset][n][8]
+    if (cl) CKI(wf_mat_alloc_w(ctx, N, cl, 8, &lde));  // mine, coset-major: [local segment][coset][n][8]
     CKI(wf_mat_alloc_w(ctx, rows_per, c, 8, &stage));
     // Preferred transport: every rank maps the others' `stage` buffers (CUDA IPC) and PUSHES its blocks there with peer copies
     // on side streams — copy engines over NVLink, no SM taken from the NTT kernels they overlap (NCCL send/recv kernels on a
@@ -1566,6 +1697,9 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
         for (int i = 0; i < 4; i++) if (!ctx->push_st[i]) CK(cudaStreamCreateWithFlags(&ctx->push_st[i], cudaStreamNonBlocking));
         for (int i = 0; i < 16; i++) if (!ctx->push_ev[i]) CK(cudaEventCreateWithFlags(&ctx->push_ev[i], cudaEventDisableTiming));
     }
+    auto lde_block = [&](u32 sg, u32 k, int q) {   // my segment sg, coset k, the points of rank q's row range
+        return lde->m.base + (size_t)sg * lde->m.seg_stride + ((size_t)k * n + (size_t)q * nj) * 8;
+    };
     const std::function<int(u32)> after_coset = [&](u32 k) -> int {   // coset k of every local column is enqueued: ship it
         if (push) {
             cudaEvent_t ev = ctx->push_ev[k % 16];
@@ -1575,35 +1709,37 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
                 cudaStream_t ps = ctx->push_st[dq % 4];
                 CK(cudaStreamWaitEvent(ps, ev, 0));
                 for (u32 sg = 0; sg < nsl; sg++) {
-                    const u64* src = lde->m.base + (size_t)sg * lde->m.seg_stride + ((size_t)k * n + (size_t)q * nj) * 8;
-                    u64* dst = (u64*)peer_stage[q] + ((size_t)r * nsl + sg) * stage->m.seg_stride + (size_t)k * nj * 8;
-                    CK(cudaMemcpyAsync(dst, src, nj * 64, cudaMemcpyDeviceToDevice, ps));
+                    u64* dst = (u64*)peer_stage[q] + (size_t)(fs + sg) * stage->m.seg_stride + (size_t)k * nj * 8;
+                    CK(cudaMemcpyAsync(dst, lde_block(sg, k, q), nj * 64, cudaMemcpyDeviceToDevice, ps));
                 }
             }
-            for (u32 sg = 0; sg < nsl; sg++) {
-                const u64* src = lde->m.base + (size_t)sg * lde->m.seg_stride + ((size_t)k * n + (size_t)r * nj) * 8;
-                CK(cudaMemcpyAsync(stage->m.base + ((size_t)r * nsl + sg) * stage->m.seg_stride + (size_t)k * nj * 8, src, nj * 64,
+            for (u32 sg = 0; sg < nsl; sg++)
+                CK(cudaMemcpyAsync(stage->m.base + (size_t)(fs + sg) * stage->m.seg_stride + (size_t)k * nj * 8, lde_block(sg, k, r), nj * 64,
                                    cudaMemcpyDeviceToDevice, ctx->st));
-            }
             sc.bytes_overlapped += (double)(G - 1) * nsl * nj * 64;
             return WF_OK;
         }
         std::vector<int> sp, rp;
         std::vector<const void*> sv;
         std::vector<void*> rv;
-        for (u32 sg = 0; sg < nsl; sg++)
+        for (u32 sg = 0; sg < nsl; sg++)    // to rank q: my segments ascending
             for (int q = 0; q < G; q++) {
-                const u64* src = lde->m.base + (size_t)sg * lde->m.seg_stride + ((size_t)k * n + (size_t)q * nj) * 8;
-                u64* dst = stage->m.base + ((size_t)q * nsl + sg) * stage->m.seg_stride + (size_t)k * nj * 8;   // q = the SOURCE rank here
-                if (q == r) CK(cudaMemcpyAsync(dst, src, nj * 64, cudaMemcpyDeviceToDevice, ctx->st));
-                else { sp.push_back(q); sv.push_back(src); rp.push_back(q); rv.push_back(dst); }
+                u64* dst = stage->m.base + (size_t)(fs + sg) * stage->m.seg_stride + (size_t)k * nj * 8;
+                if (q == r) CK(cudaMemcpyAsync(dst, lde_block(sg, k, q), nj * 64, cudaMemcpyDeviceToDevice, ctx->st));
+                else { sp.push_back(q); sv.push_back(lde_block(sg, k, q)); }
+            }
+        for (int q = 0; q < G; q++)         // from rank q: its segments ascending
+            for (u32 sg = 0; q != r && sg < segs[q]; sg++) {
+                rp.push_back(q);
+                rv.push_back(stage->m.base + (size_t)(seg0[q] + sg) * stage->m.seg_stride + (size_t)k * nj * 8);
             }
         CKI(sc.fork());
         return sc.exchange(sp, sv, rp, rv, nj * 64);
     };
     // (upload ->) layout -> interpolate -> extend, pipelined per column chunk for host columns; the cosets of the last chunk
     // are extended one by one and after_coset(k) ships coset k while coset k + 1 is computed
-    CKI(wf_trace_lde_cosetwise(ctx, local_cols, d_local, cl, n, mont, log_b, &polys, &lde, true, &after_coset));
+    if (cl) CKI(wf_trace_lde_cosetwise(ctx, local_cols, d_local, cl, n, mont, log_b, &polys, &lde, true, &after_coset));
+    else for (u32 k = 0; k < (u32)b; k++) CKI(after_coset(k));
     wf_mark(ctx, "trace_lde");
     if (push) {
         // my pushes have landed when my side streams drain; everybody's have when every rank says so
@@ -1622,122 +1758,131 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     }
     scope.drop(lde);
     scope.drop(stage);
-    {   // halo: the first `blowup` rows of every segment of rank (r + 1) mod G
-        void *pk, *pk2;
-        const size_t hb = b * 64;
-        CKI(wf_dev_alloc(ctx, hb * nsg, &pk));
-        CKI(wf_dev_alloc(ctx, hb * nsg, &pk2));
-        CK(cudaMemcpy2DAsync(pk, hb, shard->m.base, sstride * 8, hb, nsg, cudaMemcpyDeviceToDevice, ctx->st));
-        CKI(sc.exchange({(r + G - 1) % G}, {pk}, {(r + 1) % G}, {pk2}, hb * nsg));
-        CK(cudaMemcpy2DAsync(shard->m.base + rows_per * 8, sstride * 8, pk2, hb, hb, nsg, cudaMemcpyDeviceToDevice, ctx->st));
-        wf_dev_free(ctx, pk);
-        wf_dev_free(ctx, pk2);
-    }
+    CKI(exchange_halo(sc, shard->m, b));   // the first `blowup` rows of every segment of rank (r + 1) mod G
     wf_mark(ctx, "trace_exchange");
-    // ---- 3. leaves + subtree over my rows, all-gather of the subtree roots ----
+    // ---- 2. leaves + subtree over my rows, all-gather of the subtree roots ----
     Digest root;
     CKI(wf_commit_rows_partitioned(ctx, h, shard, o.part_words(c, 1), &ttree.local));
     ttree.n_global = N;
     CKI(shard_tree_finish(sc, h, ttree, &root));
     wf_mark(ctx, "trace_commit");
     ch.commit(root.b);
-    // ---- 4. constraint evaluation over my CE rows ----
-    std::vector<GlExt<D>> cc = draw_coeffs<D>(ch.coin, o.batch_c, air.num_constraints());
-    CKI(eval_constraints<D>(ctx, air, shard, nullptr, cc, {}, log_n, log_b, &comp_l, (size_t)r * ce_per, ce_per));
-    wf_mark(ctx, "constraint_eval");
-    // ---- 5. composition polynomial: all-gather the CE evaluations (a few hundred MiB at most), interpolate + extend on
-    //         every rank (the transform is over the row index), commit my row range ----
-    CKI(wf_mat_alloc(ctx, ce, D, &comp));
-    CKI(sc.all_gather_dev(comp_l->m.base, comp->m.base, ce_per * comp->m.W * 8));
-    scope.drop(comp_l);
-    wf_mat cview;  // my rows of the composition LDE
-    if (b % (size_t)G == 0) {
-        // the composition polynomial has too few columns to shard by column: shard its LDE by COSET instead. Rank r extends
-        // cosets [r b/G, (r+1) b/G) (coset-major), one exchange hands every rank the rows of its row range from every coset's
-        // owner, one kernel interleaves them into natural order (row = b j + k).
-        CKI(composition_polys(ctx, comp, log_n, D, kc, &cpolys));
-        scope.drop(comp);
-        const u32 kpr = (u32)(b / (size_t)G);
-        const size_t nj = n / (size_t)G;     // points of every coset that fall into one rank's row range
-        wf_mat *ccos = nullptr, *stage = nullptr;
-        CKI(wf_mat_alloc_w(ctx, (size_t)kpr * n, cpolys->m.cols, cpolys->m.W, &ccos));
-        int rc = wf_mat_lde_cosets(ctx, cpolys, log_b, (u32)r * kpr, (u32)(r + 1) * kpr, ccos);
-        if (rc == WF_OK) rc = wf_mat_alloc_w(ctx, rows_per, cpolys->m.cols, cpolys->m.W, &stage);
-        if (rc == WF_OK) rc = wf_mat_alloc_w(ctx, rows_per, cpolys->m.cols, cpolys->m.W, &clde);
-        if (rc != WF_OK) { wf_mat_free(ctx, ccos); wf_mat_free(ctx, stage); return rc; }
-        wf_mark(ctx, "composition_lde");
+
+    // ---- 2b. auxiliary segment (as prove_air). The build reads main rows i and i + 1 of every column: every rank evaluates its
+    //          columns on the trace domain, one all-gather by segment gives every rank the whole n x c main trace, and every
+    //          rank builds and interpolates the aux segment (replicated, deterministic); its LDE is sharded as the composition
+    //          polynomial's, with the halo the constraint evaluation reads ----
+    std::vector<u64> rnd_flat;  // [nr][D], canonical
+    wf_mat aview;               // my aux rows
+    if (aw) {
+        for (u32 i = 0; i < air.nr; i++) { GlExt<D> e = draw_ext<D>(ch.coin); for (int q = 0; q < D; q++) rnd_flat.push_back(e.v[q]); }
+        CKI(wf_mat_alloc_w(ctx, n, c, 8, &mtrace));
+        if (cl) {
+            wf_mat* ev;
+            CKI(wf_mat_evaluate(ctx, polys, &ev));
+            SegMatrix dv = mtrace->m;
+            dv.base += (size_t)fs * dv.seg_stride;
+            dv.cols = cl;
+            const cudaError_t e = layout_select_cols(ev->m, 0, dv, ctx->st);
+            ctx->launches++;
+            wf_mat_free(ctx, ev);
+            CK(e);
+        }
         {
-            const int W = cpolys->m.W;
-            const size_t blk = nj * W;       // words of one (coset, destination) block of one segment
             std::vector<int> sp, rp;
             std::vector<const void*> sv;
             std::vector<void*> rv;
-            for (u32 sg = 0; sg < ccos->m.nseg(); sg++) {
-                const u64* cb = ccos->m.base + (size_t)sg * ccos->m.seg_stride;
-                u64* sb = stage->m.base + (size_t)sg * stage->m.seg_stride;
-                for (u32 kl = 0; kl < kpr; kl++)
-                    for (int q = 0; q < G; q++) {
-                        const u64* src = cb + ((size_t)kl * n + (size_t)q * nj) * W;
-                        if (q == r) CK(cudaMemcpyAsync(sb + ((size_t)r * kpr + kl) * blk, src, blk * 8, cudaMemcpyDeviceToDevice, ctx->st));
-                        else { sp.push_back(q); sv.push_back(src); }
-                    }
-                for (u32 k = 0; k < (u32)b; k++) {
-                    const int owner = (int)(k / kpr);
-                    if (owner != r) { rp.push_back(owner); rv.push_back(sb + (size_t)k * blk); }
-                }
+            for (int q = 0; q < G; q++) {
+                if (q == r) continue;
+                for (u32 sg = 0; sg < nsl; sg++) { sp.push_back(q); sv.push_back(mtrace->m.base + (size_t)(fs + sg) * mtrace->m.seg_stride); }
+                for (u32 sg = 0; sg < segs[q]; sg++) { rp.push_back(q); rv.push_back(mtrace->m.base + (size_t)(seg0[q] + sg) * mtrace->m.seg_stride); }
             }
-            // pairwise order: sender r -> q lists (segment, local coset) ascending; receiver q <- s lists (segment, coset) ascending
-            rc = sc.exchange(sp, sv, rp, rv, blk * 8);
-            if (rc == WF_OK) {
-                dim3 grid((unsigned)((rows_per * W + 255) / 256), clde->m.nseg());
-                coset_interleave_kernel<<<grid, 256, 0, ctx->st>>>(stage->m, clde->m, nj, (u32)b);
-                ctx->launches++;
-                if (cudaGetLastError() != cudaSuccess) rc = wf_fail(ctx, WF_ERR_CUDA, "coset_interleave_kernel launch failed");
-            }
+            CKI(sc.exchange(sp, sv, rp, rv, n * 64));
         }
-        wf_mat_free(ctx, ccos);
-        wf_mat_free(ctx, stage);
-        if (rc != WF_OK) return rc;
-        cview.m = clde->m;               // clde IS my row shard
-    } else {
-        CKI(composition_commit(ctx, h, comp, log_n, log_b, D, kc, &cpolys, &clde, nullptr));
-        scope.drop(comp);
-        cview.m = clde->m;
-        cview.m.base += (size_t)r * rows_per * clde->m.W;
-        cview.m.rows = rows_per;
+        wf_mark(ctx, "main_trace_gather");
+        CKI(wf_aux_build_run(ctx, *aux_build, mtrace, c, air.periodic, rnd_flat.data(), air.nr, D, &atrace));
+        scope.drop(mtrace);
+        wf_mark(ctx, "aux_build");
+        if (aux_assertions) {
+            std::vector<u64> rnd_user = rnd_flat;
+            if (mont) for (u64& v : rnd_user) v = gl_mul(v, 0xFFFFFFFFULL);  // x * R, R = 2^64 mod p
+            std::vector<u64> vals = get_aux_assertion_words(air_dyn, D, mont);
+            if (aux_assertions(aux_user, rnd_user.data(), vals.data()) != 0) return wf_fail(ctx, WF_ERR_INVALID, "aux assertion callback failed");
+            if (!set_aux_assertion_words(air_dyn, vals.data(), D, mont))
+                return wf_fail(ctx, WF_ERR_INVALID, "aux assertion value is not a canonical field element");
+        }
+        CKI(wf_mat_interpolate(ctx, atrace, &apolys));
+        scope.drop(atrace);
+        CKI(shard_lde_rows(sc, apolys, log_b, true, &arows, aview));
+        wf_mark(ctx, "aux_lde");
+        CKI(wf_commit_rows_partitioned(ctx, h, &aview, o.part_words(aw, D), &atree.local));
+        atree.n_global = N;
+        CKI(shard_tree_finish(sc, h, atree, &root));
+        wf_mark(ctx, "aux_commit");
+        ch.commit(root.b);
     }
-    const bool comp_sharded = b % (size_t)G == 0;
+    // ---- 3. constraint evaluation over my CE rows ----
+    std::vector<GlExt<D>> cc = draw_coeffs<D>(ch.coin, o.batch_c, air.num_constraints());
+    CKI(eval_constraints<D>(ctx, air, shard, aw ? arows : nullptr, cc, rnd_flat, log_n, log_b, &comp_l, (size_t)r * ce_per, ce_per));
+    wf_mark(ctx, "constraint_eval");
+    // ---- 4. composition polynomial: all-gather the CE evaluations (a few hundred MiB at most), interpolate on every rank (the
+    //         transform is over the row index), extend and commit my row range ----
+    CKI(wf_mat_alloc(ctx, ce, D, &comp));
+    CKI(sc.all_gather_dev(comp_l->m.base, comp->m.base, ce_per * comp->m.W * 8));
+    scope.drop(comp_l);
+    CKI(composition_polys(ctx, comp, log_n, D, kc, &cpolys));
+    scope.drop(comp);
+    wf_mat cview;  // my rows of the composition LDE
+    CKI(shard_lde_rows(sc, cpolys, log_b, false, &clde, cview));
+    wf_mark(ctx, "composition_lde");
     CKI(wf_commit_rows_partitioned(ctx, h, &cview, o.part_words(kc, D), &ctree.local));
     ctree.n_global = N;
     CKI(shard_tree_finish(sc, h, ctree, &root));
     wf_mark(ctx, "composition_commit");
     ch.commit(root.b);
-    // ---- 6. out-of-domain frames: my columns' polynomials, all-gathered; composition columns are replicated ----
+    // ---- 5. out-of-domain frames: my columns' polynomials, all-gathered (blocks padded to the largest); composition and aux
+    //         columns are replicated ----
     GlExt<D> z = draw_ext<D>(ch.coin);
     GlExt<D> zg = ext_mul_base(z, gl_root_of_unity(log_n));
     std::vector<std::vector<GlExt<D>>> ood;
-    CKI(ood_eval<D>(ctx, {polys, cpolys}, z, zg, ood));
+    {
+        std::vector<const wf_mat*> mats = {cpolys};
+        if (aw) mats.push_back(apolys);
+        if (cl) mats.push_back(polys);
+        CKI(ood_eval<D>(ctx, mats, z, zg, ood));
+    }
+    const u32 ct = c + aw;
     std::vector<GlExt<D>> t_cur(c), t_nxt(c);
     {
-        std::vector<u64> mine((size_t)cl * 2 * D), all((size_t)c * 2 * D);
+        std::vector<u64> mine((size_t)maxcl * 2 * D, 0), all((size_t)G * maxcl * 2 * D);
+        const size_t mi = aw ? 4 : 2;   // my columns' values in `ood`
         for (u32 j = 0; j < cl; j++)
-            for (int q = 0; q < D; q++) { mine[((size_t)j * 2) * D + q] = ood[0][j].v[q]; mine[((size_t)j * 2 + 1) * D + q] = ood[1][j].v[q]; }
+            for (int q = 0; q < D; q++) { mine[((size_t)j * 2) * D + q] = ood[mi][j].v[q]; mine[((size_t)j * 2 + 1) * D + q] = ood[mi + 1][j].v[q]; }
         CKI(sc.gather_host(mine.data(), all.data(), mine.size() * 8));
-        for (u32 j = 0; j < c; j++)
-            for (int q = 0; q < D; q++) { t_cur[j].v[q] = all[((size_t)j * 2) * D + q]; t_nxt[j].v[q] = all[((size_t)j * 2 + 1) * D + q]; }
+        for (int s = 0; s < G; s++)
+            for (u32 jl = 0; jl < ncol[s]; jl++) {
+                const u32 j = col0[s] + jl;
+                const u64* v = &all[((size_t)s * maxcl + jl) * 2 * D];
+                for (int q = 0; q < D; q++) { t_cur[j].v[q] = v[q]; t_nxt[j].v[q] = v[D + q]; }
+            }
     }
-    std::vector<GlExt<D>> q_cur = ext_from_components<D>(ood[2]), q_nxt = ext_from_components<D>(ood[3]);
+    if (aw) {  // trace frame rows = main columns then aux columns (ood_frame.rs:40-72)
+        auto a_cur = ext_from_components<D>(ood[2]), a_nxt = ext_from_components<D>(ood[3]);
+        t_cur.insert(t_cur.end(), a_cur.begin(), a_cur.end());
+        t_nxt.insert(t_nxt.end(), a_nxt.begin(), a_nxt.end());
+    }
+    std::vector<GlExt<D>> q_cur = ext_from_components<D>(ood[0]), q_nxt = ext_from_components<D>(ood[1]);
     ByteVec ood_t, ood_q;
     ch.coin.reseed(ood_frames<D>(h, t_cur, t_nxt, q_cur, q_nxt, &ood_t, &ood_q));
     wf_mark(ctx, "ood_frames");
-    // ---- 7. DEEP composition over my LDE rows (evaluation form is row-local) ----
-    std::vector<GlExt<D>> dc = draw_coeffs<D>(ch.coin, o.batch_d, c + kc);
+    // ---- 6. DEEP composition over my LDE rows (evaluation form is row-local) ----
+    std::vector<GlExt<D>> dc = draw_coeffs<D>(ch.coin, o.batch_d, ct + kc);
     GlExt<D> Sz = ext_zero<D>(), Szg = ext_zero<D>();
-    for (u32 j = 0; j < c; j++) { Sz = ext_add(Sz, ext_mul(dc[j], t_cur[j])); Szg = ext_add(Szg, ext_mul(dc[j], t_nxt[j])); }
-    for (u32 j = 0; j < kc; j++) { Sz = ext_add(Sz, ext_mul(dc[c + j], q_cur[j])); Szg = ext_add(Szg, ext_mul(dc[c + j], q_nxt[j])); }
-    CKI(deep_compose<D>(ctx, shard, nullptr, &cview, kc, log_n + log_b, dc, z, zg, Sz, Szg, &deep, (size_t)r * rows_per, rows_per));
+    for (u32 j = 0; j < ct; j++) { Sz = ext_add(Sz, ext_mul(dc[j], t_cur[j])); Szg = ext_add(Szg, ext_mul(dc[j], t_nxt[j])); }
+    for (u32 j = 0; j < kc; j++) { Sz = ext_add(Sz, ext_mul(dc[ct + j], q_cur[j])); Szg = ext_add(Szg, ext_mul(dc[ct + j], q_nxt[j])); }
+    CKI(deep_compose<D>(ctx, shard, aw ? &aview : nullptr, &cview, kc, log_n + log_b, dc, z, zg, Sz, Szg, &deep, (size_t)r * rows_per, rows_per));
     wf_mark(ctx, "deep_composition");
-    // ---- 8. FRI: layers folded on shards while they are large. A layer of L points is held as contiguous position
+    // ---- 7. FRI: layers folded on shards while they are large. A layer of L points is held as contiguous position
     //         ranges; leaf i joins positions i, i + L/nf, ...: one exchange gives the owner of leaf range o (L/nf/G leaves)
     //         its nf pieces, which then look like a complete layer of nf * L/nf/G points to the hash and fold kernels ----
     const u32 nf = o.folding;
@@ -1805,14 +1950,14 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     }
     scope.drop(fri_in);
     wf_mark(ctx, "fri_layers");
-    // ---- 9. grinding + query positions (every rank; deterministic) ----
+    // ---- 8. grinding + query positions (every rank; deterministic) ----
     u64 nonce;
     CKI(grind_on_device(ctx, h, ch.coin.seed, o.grinding, &nonce));
     if (ch.coin.check_leading_zeros(nonce) < o.grinding) return wf_fail(ctx, WF_ERR_STATE, "grinding self-check failed");
     std::vector<u64> pos;
     if (!query_positions(ch.coin, o.num_queries, N, nonce, pos)) return wf_fail(ctx, WF_ERR_STATE, "failed to draw query positions");
     wf_mark(ctx, "grinding");
-    // ---- 10. proof object: every rank queues the same gathers, contributes what it holds, the words are summed ----
+    // ---- 9. proof object: every rank queues the same gathers, contributes what it holds, the words are summed ----
     ByteVec w;
     write_context(w, air, log_n, o);
     w.u8_((u8)pos.size());
@@ -1826,13 +1971,13 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
         for (size_t i = 0; i < p.size(); i++) if ((int)(p[i] / per) == r) l[i] = p[i] % per;
         return l;
     };
-    std::vector<std::pair<size_t, u64>> top_t, top_c;
-    size_t tr_rows = gb.add_rows(shard->m, owned_rows(pos, rows_per));
-    size_t cr_rows = comp_sharded ? gb.add_rows(cview.m, owned_rows(pos, rows_per))
-                                  : gb.add_rows(clde->m, r == 0 ? pos : std::vector<u64>(pos.size(), NONE));  // replicated: rank 0 contributes
-    size_t tr_dig, cr_dig;
+    std::vector<std::pair<size_t, u64>> top_t, top_a, top_c;
+    const std::vector<u64> mine = owned_rows(pos, rows_per);
+    size_t tr_rows = gb.add_rows(shard->m, mine), cr_rows = gb.add_rows(cview.m, mine), ar_rows = aw ? gb.add_rows(aview.m, mine) : 0;
+    size_t tr_dig, cr_dig, ar_dig = 0;
     CKI(gb.add_opening_sharded(ctx, ttree.local, N, G, r, pos, &tr_dig, &top_t));
     CKI(gb.add_opening_sharded(ctx, ctree.local, N, G, r, pos, &cr_dig, &top_c));
+    if (aw) CKI(gb.add_opening_sharded(ctx, atree.local, N, G, r, pos, &ar_dig, &top_a));
     FriProofPlan splan;   // the sharded layers' gathers, and per layer the slots of the nodes above the subtree roots
     std::vector<std::vector<std::pair<size_t, u64>>> top_f(slayers.size());
     std::vector<u64> fpos = pos;
@@ -1866,8 +2011,10 @@ int prove_fib_sharded(wf_ctx* ctx, const wf_comm* cm, const uint64_t* const* loc
     };
     patch(tr_dig, top_t, ttree);
     patch(cr_dig, top_c, ctree);
+    if (aw) patch(ar_dig, top_a, atree);
     for (size_t l = 0; l < slayers.size(); l++) patch(splan.dig_ids[l], top_f[l], slayers[l].tree);
     write_queries(gb, tr_rows, tr_dig, pos.size() * c, w);
+    if (aw) write_queries(gb, ar_rows, ar_dig, pos.size() * aw * D, w);  // trace_lde/default/mod.rs:199-218
     write_queries(gb, cr_rows, cr_dig, pos.size() * kc * D, w);
     w.u16_((uint16_t)ood_t.v.size()); w.bytes(ood_t.v.data(), ood_t.v.size());
     w.u16_((uint16_t)ood_q.v.size()); w.bytes(ood_q.v.data(), ood_q.v.size());
@@ -2307,6 +2454,13 @@ extern "C" int wf_deep_compose_polys(wf_ctx* ctx, uint32_t ext, const wf_mat* ma
     }
 }
 
+static int sharded_output(wf_ctx* ctx, int r, const std::vector<u8>& out, uint8_t* proof, size_t* proof_len) {
+    if (r != WF_OK) return r;
+    if (out.size() > *proof_len) return wf_fail(ctx, WF_ERR_INVALID, "proof buffer too small (%zu needed)", out.size());
+    memcpy(proof, out.data(), out.size());
+    *proof_len = out.size();
+    return WF_OK;
+}
 extern "C" int wf_prove_fib_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* const* local_cols, const uint64_t* d_local, int mont,
                                     uint32_t k, uint32_t log_n, const uint64_t* results, const uint32_t* opts, uint8_t* proof,
                                     size_t* proof_len, double* stats) {
@@ -2315,18 +2469,71 @@ extern "C" int wf_prove_fib_sharded(wf_ctx* ctx, const wf_comm* comm, const uint
         return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     Options o;
     CKI(parse_options(ctx, opts, o));
+    const AirHost air = fib_air_host(k, (size_t)1 << log_n, results);
     std::vector<u8> out;
     int r;
     switch (o.ext) {
-        case 1: r = prove_fib_sharded<1>(ctx, comm, local_cols, d_local, mont, k, log_n, results, o, out, stats); break;
-        case 2: r = prove_fib_sharded<2>(ctx, comm, local_cols, d_local, mont, k, log_n, results, o, out, stats); break;
-        default: r = prove_fib_sharded<3>(ctx, comm, local_cols, d_local, mont, k, log_n, results, o, out, stats); break;
+        case 1: r = prove_sharded<1>(ctx, comm, air, nullptr, nullptr, nullptr, local_cols, d_local, mont, log_n, o, out, stats); break;
+        case 2: r = prove_sharded<2>(ctx, comm, air, nullptr, nullptr, nullptr, local_cols, d_local, mont, log_n, o, out, stats); break;
+        default: r = prove_sharded<3>(ctx, comm, air, nullptr, nullptr, nullptr, local_cols, d_local, mont, log_n, o, out, stats); break;
     }
-    if (r != WF_OK) return r;
-    if (out.size() > *proof_len) return wf_fail(ctx, WF_ERR_INVALID, "proof buffer too small (%zu needed)", out.size());
-    memcpy(proof, out.data(), out.size());
-    *proof_len = out.size();
+    return sharded_output(ctx, r, out, proof, proof_len);
+}
+extern "C" int wf_shard_columns(uint32_t width, uint32_t world, uint32_t rank, uint32_t* first, uint32_t* count) {
+    if (!first || !count || width == 0 || width > 255 || world == 0 || (world & (world - 1)) || rank >= world) return WF_ERR_INVALID;
+    shard_columns(width, world, rank, *first, *count);
     return WF_OK;
+}
+extern "C" int wf_prove_air_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build,
+                                    size_t aux_build_len, wf_aux_assertions_fn aux_assertions, void* aux_user, const uint64_t* const* local_cols,
+                                    const uint64_t* d_local, uint32_t local_count, int mont, uint32_t log_n, const uint32_t* opts,
+                                    uint8_t* proof, size_t* proof_len, double* stats) {
+    if (!ctx) return WF_ERR_INVALID;
+    if (!comm || !comm->exchange || !comm->all_gather_host || !comm->all_reduce_sum) return wf_fail(ctx, WF_ERR_INVALID, "bad communicator");
+    // Checks on what every rank shares (description, options, log_n, world size): the same verdict everywhere, before any
+    // collective, so a refusal leaves no rank waiting.
+    const int G = comm->world;
+    if (G < 2 || (G & (G - 1)) || comm->rank < 0 || comm->rank >= G) return wf_fail(ctx, WF_ERR_INVALID, "world size must be a power of two >= 2");
+    if (!air_desc || !opts || log_n < 3 || log_n > 32) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    Options o;
+    CKI(parse_options(ctx, opts, o));
+    AirHost air;
+    if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
+    CKI(air_check_host(ctx, air, log_n, o.blowup));
+    AuxBuildHost b;
+    if (air.aw) {
+        if (!aux_build) return wf_fail(ctx, WF_ERR_INVALID, "two-segment AIR: the sharded prover builds its aux segment from aux_build");
+        CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
+        for (auto& col : b.cols)
+            for (u32 q = o.ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
+    } else if (aux_build || aux_assertions) {
+        return wf_fail(ctx, WF_ERR_INVALID, "single-segment AIR: it has no aux segment");
+    }
+    const size_t rows_per = ((size_t)1 << (log_n + log2_ceil(o.blowup))) / (size_t)G, ce_per = ((size_t)1 << (log_n + air.log_ce_blowup())) / (size_t)G;
+    if (log_n + log2_ceil(o.blowup) > 32 || rows_per < 64 * (size_t)o.blowup || ce_per < 64)
+        return wf_fail(ctx, WF_ERR_UNSUPPORTED, "trace too short to shard over %d ranks", G);
+    // this rank's own arguments (its column block, its output buffer): every rank learns every rank's verdict in the first
+    // collective, and all of them return when one refuses
+    u32 first, count;
+    shard_columns(air.w, (u32)G, (u32)comm->rank, first, count);
+    int mine = WF_OK;
+    if (local_count != count)
+        mine = wf_fail(ctx, WF_ERR_INVALID, "rank %d owns %u columns of %u (wf_shard_columns), not %u", comm->rank, count, air.w, local_count);
+    else if ((count && !local_cols == !d_local) || !proof || !proof_len)
+        mine = wf_fail(ctx, WF_ERR_INVALID, "bad arguments: pass exactly one of local_cols and d_local, and an output buffer");
+    std::vector<int> verdicts(G);
+    if (comm->all_gather_host(comm->user, &mine, verdicts.data(), sizeof(int)) != 0) return wf_fail(ctx, WF_ERR_STATE, "all_gather_host callback failed");
+    if (mine != WF_OK) return mine;
+    for (int q = 0; q < G; q++)
+        if (verdicts[q] != WF_OK) return wf_fail(ctx, WF_ERR_INVALID, "rank %d refused its column block or output buffer", q);
+    std::vector<u8> out;
+    int r;
+    switch (o.ext) {
+        case 1: r = prove_sharded<1>(ctx, comm, air, air.aw ? &b : nullptr, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats); break;
+        case 2: r = prove_sharded<2>(ctx, comm, air, air.aw ? &b : nullptr, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats); break;
+        default: r = prove_sharded<3>(ctx, comm, air, air.aw ? &b : nullptr, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats); break;
+    }
+    return sharded_output(ctx, r, out, proof, proof_len);
 }
 extern "C" int wf_prove_fib(wf_ctx* ctx, const uint64_t* const* trace_cols, int mont, uint32_t k, uint32_t log_n,
                             const uint64_t* results, const uint32_t* opts, uint8_t* proof, size_t* proof_len) {

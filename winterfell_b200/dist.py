@@ -286,6 +286,67 @@ def prove_fib_sharded(ctx, comm, local_trace, k, log_n, results, opts, out_buf=N
     return buf[: ln.value].tobytes()
 
 
+def shard_columns(width, world, rank):
+    """wf_shard_columns: the main-trace columns [first, first + count) that `rank` of `world` owns in a sharded proof of an AIR
+    of `width` columns. Needs no device."""
+    first, count = C.c_uint32(), C.c_uint32()
+    r = wf.lib().wf_shard_columns(width, world, rank, C.byref(first), C.byref(count))
+    if r != 0:
+        raise ValueError(f"wf_shard_columns({width}, {world}, {rank}) refused ({r})")
+    return first.value, count.value
+
+
+def prove_air_sharded(ctx, comm, desc, local_trace, log_n, opts, aux_build=None, values_fn=None, num_rands=0, num_values=0, mont=False,
+                      device_ptr=None, local_count=None, out_buf=None, stats=None):
+    """One proof of the AIR `desc` over comm.world GPUs (wf_prove_air_sharded). local_trace: this rank's columns
+    [count, n] uint64 (host; count from shard_columns), or device_ptr = raw pointer to the same block column-major in HBM
+    (then local_count is required). aux_build: the aux build description of a two-segment AIR. values_fn(rand, values) ->
+    values: optional Air::get_aux_assertions, as Context.prove_air_aux_built. Returns the proof bytes (identical on every
+    rank, and equal to the one-GPU proof of the whole trace)."""
+    L = wf.lib()
+    d_ = np.ascontiguousarray(desc, dtype=np.uint64)
+    b_ = np.ascontiguousarray(aux_build, dtype=np.uint64) if aux_build is not None else None
+    o_ = np.ascontiguousarray(opts, dtype=np.uint32)
+    d = int(o_[3])
+    buf = out_buf if out_buf is not None else np.zeros(1 << 23, dtype=np.uint8)
+    ln = C.c_size_t(buf.size)
+    st = (C.c_double * 8)()
+    ptrs, dptr = None, None
+    if device_ptr is None:
+        a = np.ascontiguousarray(local_trace, dtype=np.uint64).reshape(-1, 1 << log_n)
+        count = a.shape[0]
+        if count:
+            ptrs = (wf.u64p * count)(*[a[j].ctypes.data_as(wf.u64p) for j in range(count)])
+    else:
+        if local_count is None:
+            raise ValueError("local_count is required with a device trace pointer")
+        count, dptr = local_count, C.c_void_p(device_ptr)
+    cv = wf.AUX_BUILDER()  # NULL: no aux assertion callback
+    if values_fn is not None:
+        def cb_values(_user, rand_p, val_p):
+            try:
+                rand = np.ctypeslib.as_array(rand_p, shape=(num_rands, d)).copy()
+                vals = np.ctypeslib.as_array(val_p, shape=(num_values, d))
+                vals[:] = np.ascontiguousarray(values_fn(rand, vals.copy()), dtype=np.uint64).reshape(num_values, d)
+                return 0
+            except Exception:  # must not unwind through the C caller
+                import traceback
+                traceback.print_exc()
+                return 1
+        cv = wf.AUX_BUILDER(cb_values)
+    rc = L.wf_prove_air_sharded(ctx.h, C.byref(comm.struct), d_.ctypes.data_as(wf.u64p), d_.size,
+                                b_.ctypes.data_as(wf.u64p) if b_ is not None else None, b_.size if b_ is not None else 0, cv, None,
+                                ptrs, dptr, count, int(mont), log_n, o_.ctypes.data_as(C.POINTER(C.c_uint32)), buf.ctypes.data_as(wf.u8p),
+                                C.byref(ln), st)
+    if comm.error is not None:
+        raise comm.error
+    ctx.check(rc)
+    if stats is not None:
+        stats.update({"bytes_sent": st[0], "exchange_ms": st[1], "collectives": st[2], "small_collective_ms": st[3], "sharded_fri_layers": st[4],
+                      "bytes_overlapped": st[5], "peer_push": st[6]})
+    return buf[: ln.value].tobytes()
+
+
 def bench_sharded(ctx, stream, cfg, steps, warmup, configs, proof_opts, flush, clock_sampler_cls, local_rank):
     """bench.py's N > 1 arm: ONE proof of `cfg` sharded over the ranks (strong scaling). Returns bench.py's record:
     ms per proof with this rank's column block resident in HBM, e2e ms from pinned host columns, stage times, the
