@@ -521,6 +521,19 @@ int wf_ext_ops_dev(wf_ctx* ctx, uint32_t ext, const uint64_t* d_a, const uint64_
  * gl64.cuh) on n rows of k terms (1 <= k < 2^31): d_x, d_y = [n][k] ANY 64-bit words (device). d_out = [n][6] words: the raw
  * 160-bit accumulator sum_j x_j y_j as w0..w4 (32-bit words, w0 lowest, one per output word), then its reduction mod p. */
 int wf_acc_ops_dev(wf_ctx* ctx, const uint64_t* d_x, const uint64_t* d_y, uint32_t k, size_t n, uint64_t* d_out);
+/* the constraint evaluation of wf_eval_constraints over CE rows [row0, row0 + ce_rows) only (ce_rows >= 64, inside the domain),
+ * as the row-sharded prover runs it: main_lde / aux_lde hold the window's LDE rows (ce_rows << log2(blowup / ce_blowup) of them,
+ * from row row0 << log2(blowup / ce_blowup)) followed by `blowup` halo rows (the LDE rows after the window, wrapping to row 0).
+ * *out = ce_rows x ext, row j = CE row row0 + j of wf_eval_constraints. */
+int wf_eval_constraints_window(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup,
+                               uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs,
+                               const uint64_t* aux_rand, size_t row0, size_t ce_rows, wf_mat** out);
+/* the specialised FibSmall x k constraint kernel of wf_prove_fib with caller-chosen coefficients: the same values as
+ * wf_eval_constraints on the description of FibSmall x k (pair j starting at (j+1, j+1), results[j] the last value of column
+ * 2j+1), with the same coefficient layout. ce_rows = 0 (and row0 = 0): the whole CE domain, lde = the (n * blowup) x 2k trace
+ * LDE; otherwise the window of wf_eval_constraints_window. */
+int wf_eval_constraints_fib(wf_ctx* ctx, uint32_t k, const uint64_t* results, uint32_t log_n, uint32_t blowup, uint32_t ext,
+                            const wf_mat* lde, const uint64_t* coeffs, size_t row0, size_t ce_rows, wf_mat** out);
 
 /* ---- host-side helpers of the product (transcript arithmetic; no GPU needed) ------------------- */
 /* H::hash_elements / merge / merge_with_int on the host (crypto/src/hash/mod.rs:31-64) */

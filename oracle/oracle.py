@@ -481,6 +481,31 @@ def perm_rap_aux(trace, rand):
     return out
 
 
+def eval_constraint_rows(desc, n, blowup, ext, coeffs, rand, rows, cur, nxt, acur=None, anxt=None):
+    """The prover's combined constraint evaluations on CE rows `rows` (wfo_eval_constraint_rows) from their frames:
+    cur / nxt [k, w] main LDE rows, acur / anxt [k, aw * ext] aux LDE rows (None without an aux segment);
+    coeffs [constraints + assertions, ext] in wf_eval_constraints' layout, rand [nr, ext]. Returns [k, ext]."""
+    d_, dp = _u64(desc)
+    c_, cp = _u64(coeffs)
+    r_, rp = _u64(rand if rand is not None else np.zeros(1, dtype=np.uint64))
+    w_, wp = _u64(rows)
+    k = w_.size
+    cu, cup = _u64(cur)
+    nx, nxp = _u64(nxt)
+    acp = anp = None
+    if acur is not None:
+        ac_, acp = _u64(acur)
+        an_, anp = _u64(anxt)
+    out = np.zeros((k, ext), dtype=np.uint64)
+    L = lib()
+    L.wfo_eval_constraint_rows.restype = C.c_long
+    r = L.wfo_eval_constraint_rows(dp, C.c_size_t(d_.size), C.c_size_t(n), C.c_size_t(blowup), C.c_int(ext), cp, rp, wp, C.c_size_t(k),
+                                   cup, nxp, acp, anp, out.ctypes.data_as(u64p))
+    if r != 0:
+        raise ValueError(f"wfo_eval_constraint_rows: {r}")
+    return out
+
+
 def verify_air(desc, proof: bytes, hash_id=BLAKE3):
     d_, dp = _u64(desc)
     p_, pp = _u8(np.frombuffer(proof, dtype=np.uint8))

@@ -427,6 +427,108 @@ static std::vector<std::vector<u64>> periodic_value_table(const Air& air) {
     return ptab;
 }
 
+// ---- constraint evaluation over the CE domain ----------------------------------------------------------
+// DefaultConstraintEvaluator::evaluate (evaluator/default.rs:60-118) fused with ConstraintEvaluationTable::combine
+// (evaluation_table.rs:163-407), one CE row at a time from that row's frames, in plain per-row formulas: x^a by f_exp,
+// one f_inv per divisor, table rows by % size. The prover runs it over the whole domain; wfo_eval_constraint_rows over
+// the rows a test names. ccoef: [main transition, aux transition | main assertions, aux assertions (sorted order)].
+struct CeEvaluator {
+    const Air& air;
+    Field F;
+    size_t n, ce, c, aw;
+    u64 g_ce;
+    std::vector<EE> tcoef, tcoef_aux;
+    std::vector<BoundaryGroup> groups, aux_groups;
+    std::vector<std::vector<std::vector<u64>>> gtab, agtab;
+    std::vector<u64> exempt;
+    std::vector<std::vector<u64>> ptab;
+    const EE* rnd;
+    struct Scratch {
+        std::vector<u64> tev, per;
+        std::vector<EE> mc, mn, ac, an, pe, aev;
+    };
+    CeEvaluator(const Air& a, int d, const std::vector<EE>& ccoef, const EE* rand_elems)
+        : air(a), F{d}, n(a.n), ce(a.n * a.ce_blowup()), c(a.width()), aw(a.aw), rnd(rand_elems) {
+        const size_t nTm = air.num_main_transition(), nT = air.num_transition();
+        tcoef.assign(ccoef.begin(), ccoef.begin() + nTm);          // transition/mod.rs:63-72 split
+        tcoef_aux.assign(ccoef.begin() + nTm, ccoef.begin() + nT);
+        std::vector<EE> bcoef(ccoef.begin() + nT, ccoef.begin() + nT + air.asserts.size());  // boundary/mod.rs:108-110
+        groups = boundary_groups(air, bcoef);
+        aux_groups = aux_boundary_groups(air, ccoef.data() + nT + air.asserts.size());
+        g_ce = root_of_unity((u32)__builtin_ctzll(ce));
+        exempt = exemption_points(air);
+        // periodic value table (evaluator/periodic_table.rs:24-76): column j evaluated over the coset
+        // offset^(n/L) <w_(L*ceb)>, row i of the CE domain reads entry i mod (L*ceb)
+        ptab = periodic_value_table(air);
+        gtab.resize(groups.size());
+        agtab.resize(aux_groups.size());
+        for (size_t gi = 0; gi < groups.size(); gi++) for (auto& e : groups[gi].e) gtab[gi].push_back(sequence_table(e, 1, ce));
+        for (size_t gi = 0; gi < aux_groups.size(); gi++) for (auto& e : aux_groups[gi].e) agtab[gi].push_back(sequence_table(e, d, ce));
+    }
+    Scratch scratch() const {
+        Scratch s;
+        s.tev.resize(tcoef.size()); s.per.resize(ptab.size());
+        s.mc.resize(c); s.mn.resize(c); s.ac.resize(aw); s.an.resize(aw); s.pe.resize(ptab.size()); s.aev.resize(tcoef_aux.size());
+        return s;
+    }
+    // CE row i from its frames: main rows cur / nxt [c], aux rows ar / arn [aw][d] (ignored without an aux segment)
+    EE row(size_t i, const u64* cur, const u64* nxt, const u64* ar, const u64* arn, Scratch& s) const {
+        const int d = F.d;
+        auto e_sub = [&](const EE& x, const EE& y) { return F.sub(x, y); };
+        auto e_add = [&](const EE& x, const EE& y) { return F.add(x, y); };
+        auto e_mul = [&](const EE& x, const EE& y) { return F.mul(x, y); };
+        auto e_fb = [&](u64 v) { return F.from_base(v); };
+        for (size_t j = 0; j < ptab.size(); j++) s.per[j] = ptab[j][i % ptab[j].size()];
+        std::fill(s.tev.begin(), s.tev.end(), 0);
+        air.eval_transition(cur, nxt, s.per.data(), s.tev.data(), f_sub, f_add, f_mul, [](u64 v) { return v; });
+        EE t = F.zero();
+        for (size_t j = 0; j < s.tev.size(); j++) t = F.add(t, F.mul_base(tcoef[j], s.tev[j]));
+        if (aw) {  // evaluator/default.rs:306-341 evaluate_aux_transition
+            for (size_t j = 0; j < c; j++) { s.mc[j] = F.from_base(cur[j]); s.mn[j] = F.from_base(nxt[j]); }
+            for (size_t j = 0; j < aw; j++) {
+                s.ac[j] = F.zero(); s.an[j] = F.zero();
+                for (int k = 0; k < d; k++) { s.ac[j].v[k] = ar[j * d + k]; s.an[j].v[k] = arn[j * d + k]; }
+            }
+            for (size_t j = 0; j < s.per.size(); j++) s.pe[j] = F.from_base(s.per[j]);
+            std::fill(s.aev.begin(), s.aev.end(), F.zero());
+            air.eval_aux_transition(s.mc.data(), s.mn.data(), s.ac.data(), s.an.data(), s.pe.data(), rnd, s.aev.data(), e_sub, e_add,
+                                    e_mul, e_fb);
+            for (size_t j = 0; j < s.aev.size(); j++) t = F.add(t, F.mul(s.aev[j], tcoef_aux[j]));
+        }
+        u64 x = f_mul(f_exp(g_ce, i), GENERATOR);                  // domain.rs get_ce_x_at
+        u64 zt = f_inv(f_sub(f_exp(x, n), 1));                     // 1 / (x^n - 1)
+        u64 ex = 1;
+        for (u64 e : exempt) ex = f_mul(ex, f_sub(x, e));          // divisor.rs evaluate_exemptions_at
+        EE acc = F.mul_base(t, f_mul(zt, ex));                     // evaluation_table.rs:343-366
+        for (size_t gi = 0; gi < groups.size(); gi++) {
+            auto& G = groups[gi];
+            EE bsum = F.zero();
+            for (size_t q = 0; q < G.e.size(); q++) {              // evaluator/boundary.rs Single / Small / LargePoly
+                const BoundaryEntry& e = G.e[q];
+                u64 val = e.poly.size() == 1 ? e.poly[0].v[0] : gtab[gi][q][(i + ce - (e.first_step * air.ce_blowup()) % ce) % ce];
+                bsum = F.add(bsum, F.mul_base(e.cc, f_sub(cur[e.col], val)));
+            }
+            acc = F.add(acc, F.mul_base(bsum, f_inv(f_sub(f_exp(x, G.a), G.b))));  // :329-340
+        }
+        for (size_t gi = 0; gi < aux_groups.size(); gi++) {  // evaluator/boundary.rs:228-260 aux constraints
+            auto& G = aux_groups[gi];
+            EE bsum = F.zero();
+            for (size_t q = 0; q < G.e.size(); q++) {
+                const BoundaryEntry& e = G.e[q];
+                EE val = e.poly[0];
+                if (e.poly.size() > 1) {
+                    size_t idx = (i + ce - (e.first_step * air.ce_blowup()) % ce) % ce;
+                    val = F.zero();
+                    for (int k = 0; k < d; k++) val.v[k] = agtab[gi][q][idx * d + k];
+                }
+                bsum = F.add(bsum, F.mul(F.sub(s.ac[e.col], val), e.cc));
+            }
+            acc = F.add(acc, F.mul_base(bsum, f_inv(f_sub(f_exp(x, G.a), G.b))));
+        }
+        return acc;
+    }
+};
+
 // ---- the proof -----------------------------------------------------------------------------------
 struct ProofParts {
     std::vector<u8> bytes;
@@ -609,87 +711,18 @@ static std::vector<u8> prove_fib(const FibAir& air_in, const u64* trace /*[w][n]
     tm.mark("trace_commit");
     // 2. constraint evaluation (evaluator/default.rs:60-118, evaluation_table.rs:163-407)
     std::vector<EE> ccoef = coin.draw_coeffs(F, (int)o.batch_c, air.num_transition() + air.num_assertions());
-    const size_t nTm = air.num_main_transition(), nT = air.num_transition();
-    std::vector<EE> tcoef(ccoef.begin(), ccoef.begin() + nTm);          // transition/mod.rs:63-72 split
-    std::vector<EE> tcoef_aux(ccoef.begin() + nTm, ccoef.begin() + nT);
-    std::vector<EE> bcoef(ccoef.begin() + nT, ccoef.begin() + nT + air.asserts.size());  // boundary/mod.rs:108-110
-    auto groups = boundary_groups(air, bcoef);
-    auto aux_groups = aux_boundary_groups(air, ccoef.data() + nT + air.asserts.size());
-    auto e_sub = [&](const EE& x, const EE& y) { return F.sub(x, y); };
-    auto e_add = [&](const EE& x, const EE& y) { return F.add(x, y); };
-    auto e_mul = [&](const EE& x, const EE& y) { return F.mul(x, y); };
-    auto e_fb = [&](u64 v) { return F.from_base(v); };
+    const CeEvaluator ev(air, d, ccoef, rnd.data());
     const size_t ce = n * air.ce_blowup();
     const size_t lde_shift = (size_t)__builtin_ctzll(b / air.ce_blowup());
-    const u64 g_ce = root_of_unity((u32)__builtin_ctzll(ce));
     const u64 g_tr = root_of_unity((u32)__builtin_ctzll(n));
-    const std::vector<u64> exempt = exemption_points(air);
-    // periodic value table (evaluator/periodic_table.rs:24-76): column j evaluated over the coset
-    // offset^(n/L) <w_(L*ceb)>, row i of the CE domain reads entry i mod (L*ceb)
-    std::vector<std::vector<u64>> ptab = periodic_value_table(air);
-    std::vector<std::vector<std::vector<u64>>> gtab(groups.size()), agtab(aux_groups.size());
-    for (size_t gi = 0; gi < groups.size(); gi++) for (auto& e : groups[gi].e) gtab[gi].push_back(sequence_table(e, 1, ce));
-    for (size_t gi = 0; gi < aux_groups.size(); gi++) for (auto& e : aux_groups[gi].e) agtab[gi].push_back(sequence_table(e, d, ce));
     std::vector<EE> comp(ce);
 #pragma omp parallel
     {
-        std::vector<u64> tev(nTm), per(ptab.size());
-        std::vector<EE> mc(c), mn(c), ac(aw), an(aw), pe(ptab.size()), aev(tcoef_aux.size());
+        CeEvaluator::Scratch s = ev.scratch();
 #pragma omp for schedule(static)
         for (size_t i = 0; i < ce; i++) {
-            size_t ls = i << lde_shift;
-            const u64* cur = &lde[ls * c];
-            const u64* nxt = &lde[((ls + b) % N) * c];  // trace_lde/default/mod.rs:169-180
-            for (size_t j = 0; j < ptab.size(); j++) per[j] = ptab[j][i % ptab[j].size()];
-            std::fill(tev.begin(), tev.end(), 0);
-            air.eval_transition(cur, nxt, per.data(), tev.data(), f_sub, f_add, f_mul, [](u64 v) { return v; });
-            EE t = F.zero();
-            for (size_t j = 0; j < tev.size(); j++) t = F.add(t, F.mul_base(tcoef[j], tev[j]));
-            if (aw) {  // evaluator/default.rs:306-341 evaluate_aux_transition
-                const u64* ar = &alde[ls * aw * d];
-                const u64* arn = &alde[((ls + b) % N) * aw * d];
-                for (size_t j = 0; j < c; j++) { mc[j] = F.from_base(cur[j]); mn[j] = F.from_base(nxt[j]); }
-                for (size_t j = 0; j < aw; j++) {
-                    ac[j] = F.zero(); an[j] = F.zero();
-                    for (int k = 0; k < d; k++) { ac[j].v[k] = ar[j * d + k]; an[j].v[k] = arn[j * d + k]; }
-                }
-                for (size_t j = 0; j < per.size(); j++) pe[j] = F.from_base(per[j]);
-                std::fill(aev.begin(), aev.end(), F.zero());
-                air.eval_aux_transition(mc.data(), mn.data(), ac.data(), an.data(), pe.data(), rnd.data(), aev.data(), e_sub, e_add,
-                                        e_mul, e_fb);
-                for (size_t j = 0; j < aev.size(); j++) t = F.add(t, F.mul(aev[j], tcoef_aux[j]));
-            }
-            u64 x = f_mul(f_exp(g_ce, i), GENERATOR);                  // domain.rs get_ce_x_at
-            u64 zt = f_inv(f_sub(f_exp(x, n), 1));                     // 1 / (x^n - 1)
-            u64 ex = 1;
-            for (u64 e : exempt) ex = f_mul(ex, f_sub(x, e));          // divisor.rs evaluate_exemptions_at
-            EE acc = F.mul_base(t, f_mul(zt, ex));                     // evaluation_table.rs:343-366
-            for (size_t gi = 0; gi < groups.size(); gi++) {
-                auto& G = groups[gi];
-                EE bsum = F.zero();
-                for (size_t q = 0; q < G.e.size(); q++) {              // evaluator/boundary.rs Single / Small / LargePoly
-                    const BoundaryEntry& e = G.e[q];
-                    u64 val = e.poly.size() == 1 ? e.poly[0].v[0] : gtab[gi][q][(i + ce - (e.first_step * air.ce_blowup()) % ce) % ce];
-                    bsum = F.add(bsum, F.mul_base(e.cc, f_sub(cur[e.col], val)));
-                }
-                acc = F.add(acc, F.mul_base(bsum, f_inv(f_sub(f_exp(x, G.a), G.b))));  // :329-340
-            }
-            for (size_t gi = 0; gi < aux_groups.size(); gi++) {  // evaluator/boundary.rs:228-260 aux constraints
-                auto& G = aux_groups[gi];
-                EE bsum = F.zero();
-                for (size_t q = 0; q < G.e.size(); q++) {
-                    const BoundaryEntry& e = G.e[q];
-                    EE val = e.poly[0];
-                    if (e.poly.size() > 1) {
-                        size_t idx = (i + ce - (e.first_step * air.ce_blowup()) % ce) % ce;
-                        val = F.zero();
-                        for (int k = 0; k < d; k++) val.v[k] = agtab[gi][q][idx * d + k];
-                    }
-                    bsum = F.add(bsum, F.mul(F.sub(ac[e.col], val), e.cc));
-                }
-                acc = F.add(acc, F.mul_base(bsum, f_inv(f_sub(f_exp(x, G.a), G.b))));
-            }
-            comp[i] = acc;
+            size_t ls = i << lde_shift, lx = (ls + b) % N;  // trace_lde/default/mod.rs:169-180
+            comp[i] = ev.row(i, &lde[ls * c], &lde[lx * c], aw ? &alde[ls * aw * d] : nullptr, aw ? &alde[lx * aw * d] : nullptr, s);
         }
     }
     // 3. composition polynomial + commitment (composition_poly.rs:58-78, commitment/default.rs:109-150)
@@ -1447,6 +1480,38 @@ long wfo_boundary_groups(const uint64_t* desc, size_t desc_len, size_t n, const 
     if (w.size() > cap) return -1;
     memcpy(out, w.data(), w.size() * 8);
     return (long)w.size();
+}
+// The combined, divisor-normalised constraint evaluations the prover computes on CE rows rows[0..k) (step 2 of prove_fib),
+// from the frames the caller passes: cur / nxt = [k][w] main LDE rows (i << log2(blowup / ce_blowup) and the row `blowup`
+// after it), acur / anxt = [k][aw][ext] aux LDE rows (null without an aux segment). coeffs = [transition main, aux |
+// boundary main, aux][ext] as wf_eval_constraints takes them (boundary coefficients in sorted-assertion order), rand =
+// [nr][ext]. The periodic and sequence tables are built as the prover builds them. out = [k][ext]. Returns 0, -2 for a
+// malformed description, -3 for bad shapes.
+long wfo_eval_constraint_rows(const uint64_t* desc, size_t desc_len, size_t n, size_t blowup, int ext, const uint64_t* coeffs,
+                              const uint64_t* rand, const uint64_t* rows, size_t k, const uint64_t* cur, const uint64_t* nxt,
+                              const uint64_t* acur, const uint64_t* anxt, uint64_t* out) {
+    Air air;
+    if (!parse_air(desc, desc_len, air)) return -2;
+    air.n = n;
+    memset(&air.o, 0, sizeof(air.o));
+    air.o.ext = (u32)ext; air.o.blowup = (u32)blowup;
+    if (ext < 1 || ext > 3 || n < 2 || (n & (n - 1)) || blowup < air.ce_blowup() || (blowup & (blowup - 1)) ||
+        (air.aw && (!acur || !anxt)))
+        return -3;
+    const size_t ce = n * air.ce_blowup();
+    for (size_t r = 0; r < k; r++) if (rows[r] >= ce) return -3;
+    const size_t ncc = air.num_transition() + air.num_assertions();
+    std::vector<EE> cc(ncc), rnd(air.nr);
+    for (size_t j = 0; j < ncc; j++) for (int q = 0; q < ext; q++) cc[j].v[q] = coeffs[j * ext + q];
+    for (size_t j = 0; j < air.nr; j++) for (int q = 0; q < ext; q++) rnd[j].v[q] = rand[j * ext + q];
+    const CeEvaluator ev(air, ext, cc, rnd.data());
+    const size_t w = air.width(), aw = air.aw * ext;
+    CeEvaluator::Scratch s = ev.scratch();
+    for (size_t r = 0; r < k; r++) {
+        EE v = ev.row(rows[r], cur + r * w, nxt + r * w, aw ? acur + r * aw : nullptr, aw ? anxt + r * aw : nullptr, s);
+        for (int q = 0; q < ext; q++) out[r * ext + q] = v.v[q];
+    }
+    return 0;
 }
 // MerkleTree::verify_batch (crypto/src/merkle/mod.rs:300-330) = BatchMerkleProof::get_root + comparison:
 // serialized batch proof, the opened leaves (k x 32 bytes, in the order of `indexes`). 0 = accepted.

@@ -418,3 +418,40 @@ def fold_inputs(L, nf, d, rng_np):
             for k in range(nf):
                 ev[i + k * m, c] = x[k]
     return ev
+
+
+# ---- the FibSmall constraint kernel (fib_constraints_kernel) ----
+def fib_mult(m):
+    """the coefficients of one FibSmall accumulator in an aimed call: p - 1 on its first m - 1 terms, 1 on the last"""
+    return [P - 1] * (m - 1) + [1]
+
+
+def fib_k0(k):
+    """K0 of an aimed B0 call, sum_j (b0a_j + b0b_j) (j + 1) mod p, for the coefficients fib_mult(2k)"""
+    mult = fib_mult(2 * k)
+    return sum((mult[2 * j] + mult[2 * j + 1]) * (j + 1) for j in range(k)) % P
+
+
+def _row_for(m, A):
+    q, R = divmod(A, (P - 1) ** 2)       # q (p-1)^2 + x (p-1) + r0 with q <= m - 2
+    x, r0 = divmod(R, P - 1)
+    return [P - 1] * q + [0] * (m - 2 - q) + [x, r0]
+
+
+def fib_aims(k, rng):
+    """(accumulator, class, term values) for the three accumulators of one FibSmall x k row: T over the 2k values t0_j, t1_j
+    (interleaved), B0 over cur.x_j, cur.y_j (interleaved), B1 over the k values cur.y_j, each against fib_mult of its length.
+    B0 also aims acc_reduce(a0) = K0 (B0 = 0) and acc_reduce(a0) < K0 (a borrow in gl_sub(., K0))."""
+    out = []
+    for acc, m in (("T", 2 * k), ("B0", 2 * k), ("B1", k)):
+        if m < 2:
+            continue
+        out += [(acc, cls, row) for cls, row in deep_rows(m, rng)]
+    if k >= 2:
+        amax, K0 = (2 * k - 1) * (P - 1) ** 2 - 1, fib_k0(k)
+        A = K0 + P * rng.randrange(max(1, (amax - K0) // P))
+        out.append(("B0", "reduce(a0) = K0", _row_for(2 * k, A)))
+        if K0:
+            A = P * rng.randrange(max(1, amax // P - 1)) + rng.randrange(K0)
+            out.append(("B0", "reduce(a0) < K0", _row_for(2 * k, A)))
+    return out

@@ -127,9 +127,9 @@ UNREACHED = {
         "the aimed multipliers are p - 1 and 1, whose low halves are 0 and 1: x0 y1 + x1 y0 < 2^64 "
         "(wf_acc_ops_dev covers it)",
 }
-for _cls in M.CLASSES:
-    UNREACHED[("fib_constraints", _cls)] = ("its combination coefficients are drawn from the public coin, so the "
-                                           "accumulators cannot be aimed; the same device functions run in wf_acc_ops_dev")
+UNREACHED[("fib_constraints", "odd carry ripples through all-ones w1..w3")] = UNREACHED[("deep_sum", "odd carry ripples through all-ones w1..w3")]
+UNREACHED[("fib_constraints", "m2 = 1")] = UNREACHED[("deep_sum", "m2 = 1")]
+FIB_K = (2, 3, 32)   # the widths test_gpu_constraint_rows.py aims the FibSmall kernel at
 
 
 def kernel_log():
@@ -148,7 +148,26 @@ def kernel_log():
         mult = [P - 1] * (c - 1) + [1]
         for _, row in M.deep_rows(c, rng):
             M.acc_reduce(M.dot(mult, row, log, "deep_sum"), M.deep_max(c) >> 128, log, "deep_sum")
+    for k in FIB_K:
+        for acc, _, row in M.fib_aims(k, random.Random(k)):
+            mult = M.fib_mult(len(row))
+            M.acc_reduce(M.dot(mult, row, log, "fib_constraints"), M.deep_max(len(row)) >> 128, log, "fib_constraints")
     return log
+
+
+@pytest.mark.parametrize("k", FIB_K)
+def test_fib_aims_reach_their_class(k):
+    K0 = M.fib_k0(k)
+    for acc, cls, row in M.fib_aims(k, random.Random(k)):
+        log = M.Log()
+        r = M.acc_reduce(M.dot(M.fib_mult(len(row)), row, log), M.deep_max(len(row)) >> 128, log)
+        assert all(0 <= v < P for v in row) and len(row) == (k if acc == "B1" else 2 * k)
+        if cls in M.REDUCE_CLASSES:
+            assert ("dot", cls) in log.hits, (k, acc, cls)
+        elif cls == "reduce(a0) = K0":
+            assert r == K0
+        elif cls == "reduce(a0) < K0":
+            assert r < K0
 
 
 def test_coverage_matrix(capsys):

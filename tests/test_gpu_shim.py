@@ -114,14 +114,17 @@ def test_stepwise_python_matches_one_call(ctx, oracle):
     fr = lde.read_rows(np.array([5, 13], dtype=np.uint64))
     want = oracle.lde_rows(oracle.interpolate_columns(trace), 8)
     assert (fr[0] == want[5]).all() and (fr[1] == want[13]).all()
-    # constraint evaluation with fixed coefficients vs the oracle prover's composition values is covered by the
-    # proof-level tests; here: shape + determinism of the seam
+    # constraint evaluation with fixed coefficients: every CE row equals the oracle prover's value from the same frames
     ntr, nas = 3, 5
     coeffs = oracle.rand_elems((ntr + nas, ext), 11)
     comp = ctx.eval_constraints(desc, log_n, 8, ext, lde, None, coeffs)
     assert comp.rows == n * 4 and comp.cols == ext
+    rows = np.arange(n * 4, dtype=np.uint64)
+    ls = rows.astype(np.int64) << 1                     # ce_blowup 4, blowup 8
+    got = comp.to_rows()
+    assert (got == oracle.eval_constraint_rows(desc, n, 8, ext, coeffs, None, rows, want[ls], want[(ls + 8) % (8 * n)])).all()
     comp2 = ctx.eval_constraints(desc, log_n, 8, ext, lde, None, coeffs)
-    assert (comp.to_rows() == comp2.to_rows()).all()
+    assert (got == comp2.to_rows()).all()
     cpolys, clde, ctree = ctx.composition_commit(h, comp, log_n, 8, ext, 3)
     assert cpolys.rows == n and cpolys.cols == 3 * ext and clde.rows == 8 * n
     # the composition columns, evaluated at z, recombine to the CE-domain polynomial: H(z) = sum_i z^(i n) H_i(z)

@@ -117,6 +117,10 @@ _SIGS = [
     ("wf_rescue_permute_dev", C.c_int, [vp, C.c_int, vp, vp, C.c_size_t, vp]),
     ("wf_ext_ops_dev", C.c_int, [vp, C.c_uint32, vp, vp, C.c_size_t, vp]),
     ("wf_acc_ops_dev", C.c_int, [vp, vp, vp, C.c_uint32, C.c_size_t, vp]),
+    ("wf_eval_constraints_window", C.c_int, [vp, u64p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, u64p, u64p, C.c_size_t,
+                                             C.c_size_t, C.POINTER(vp)]),
+    ("wf_eval_constraints_fib", C.c_int, [vp, C.c_uint32, u64p, C.c_uint32, C.c_uint32, C.c_uint32, vp, u64p, C.c_size_t, C.c_size_t,
+                                          C.POINTER(vp)]),
     ("wf_ctx_set_jit", C.c_int, [vp, C.c_int]),
     ("wf_ctx_jit_stats", C.c_int, [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     ("wf_jit_compile_air", C.c_int, [u64p, C.c_size_t, C.c_uint32, C.POINTER(C.c_size_t), C.c_char_p, C.c_size_t]),
@@ -286,6 +290,26 @@ class Context:
         h = vp()
         self.check(self.L.wf_eval_constraints(self.h, dp, d_.size, log_n, blowup, ext, main_lde.h, aux_lde.h if aux_lde else None,
                                               cp, rp, C.byref(h)))
+        return Mat(self, h)
+
+    def eval_constraints_window(self, desc, log_n, blowup, ext, main_lde, aux_lde, coeffs, aux_rand, row0, ce_rows):
+        """eval_constraints over CE rows [row0, row0 + ce_rows) from the window's LDE rows followed by `blowup` halo rows"""
+        d_, dp = _u64(desc)
+        c_, cp = _u64(coeffs)
+        rp = None
+        if aux_rand is not None:
+            r_, rp = _u64(aux_rand)
+        h = vp()
+        self.check(self.L.wf_eval_constraints_window(self.h, dp, d_.size, log_n, blowup, ext, main_lde.h, aux_lde.h if aux_lde else None,
+                                                     cp, rp, row0, ce_rows, C.byref(h)))
+        return Mat(self, h)
+
+    def eval_constraints_fib(self, k, results, log_n, blowup, ext, lde, coeffs, row0=0, ce_rows=0):
+        """the FibSmall x k constraint kernel with caller-chosen coefficients (layout of eval_constraints on airs.fib_small_x)"""
+        r_, rp = _u64(results)
+        c_, cp = _u64(coeffs)
+        h = vp()
+        self.check(self.L.wf_eval_constraints_fib(self.h, k, rp, log_n, blowup, ext, lde.h, cp, row0, ce_rows, C.byref(h)))
         return Mat(self, h)
 
     def composition_commit(self, hash_id, comp_trace, log_n, blowup, ext, num_cols):

@@ -833,6 +833,24 @@ static int sequence_table(wf_ctx* ctx, const u64* values, size_t L, u32 words_pe
     return r;
 }
 
+// OUT j, v sets constraint j's value (result[dst] = r[a], include/winterfell_b200.h), as the verifiers evaluate it: of several
+// OUTs of one constraint only the last one counts. The combining kernels add every OUT they run into the combination, so they
+// get the program without the earlier ones (an OUT writes no register; dropping it changes nothing else).
+static std::vector<u32> last_outs_only(const std::vector<u32>& prog) {
+    std::vector<u32> out;
+    std::vector<bool> seen;
+    for (size_t k = prog.size() / 4; k-- > 0;) {
+        const u32* in = &prog[4 * k];
+        if (in[0] == 4) {
+            if (in[1] >= seen.size()) seen.resize(in[1] + 1, false);
+            if (seen[in[1]]) continue;
+            seen[in[1]] = true;
+        }
+        out.insert(out.begin(), in, in + 4);
+    }
+    return out;
+}
+
 // DefaultConstraintEvaluator::evaluate (prover/src/constraints/evaluator/default.rs:60-118) fused with
 // ConstraintEvaluationTable::combine (evaluation_table.rs:163-407): the combined, divisor-normalised
 // constraint evaluations over the CE domain = CompositionPolyTrace, as a (n * ce_blowup) x D matrix.
@@ -914,9 +932,10 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
         GenEvalParams p;
         memset(&p, 0, sizeof(p));
         p.lde = lde->m; p.out = comp->m; p.w = c; p.log_n = log_n; p.log_blowup = log_b; p.log_ce_blowup = log_ceb;
-        p.prog_len = (u32)(air.prog.size() / 4); p.num_regs = air.num_regs; p.num_periodic = (u32)air.periodic.size(); p.num_tc = n_mtr;
+        const std::vector<u32> prog = last_outs_only(air.prog), aprog = last_outs_only(air.aux_prog);
+        p.prog_len = (u32)(prog.size() / 4); p.num_regs = air.num_regs; p.num_periodic = (u32)air.periodic.size(); p.num_tc = n_mtr;
         void* dp = nullptr;
-        CKI(upload(air.prog.data(), air.prog.size() * 4, &dp)); p.prog = (u32*)dp;
+        CKI(upload(prog.data(), prog.size() * 4, &dp)); p.prog = (u32*)dp;
         CKI(upload(air.consts.data(), air.consts.size() * 8, &dp)); p.consts = (u64*)dp;
         // periodic value tables (evaluator/periodic_table.rs:24-76): poly_j over offset^(n/L) <w_(L*ceb)>
         std::vector<u64> ptab;
@@ -974,8 +993,8 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
         std::vector<u64> aga, agb, agoa, aeval, aecc, fa;
         std::vector<const u64*> aetab;
         if (aw) {
-            p.alde = alde->m; p.aw = aw; p.nr = air.nr; p.aprog_len = (u32)(air.aux_prog.size() / 4);
-            CKI(upload(air.aux_prog.data(), air.aux_prog.size() * 4, &dp)); p.aprog = (u32*)dp;
+            p.alde = alde->m; p.aw = aw; p.nr = air.nr; p.aprog_len = (u32)(aprog.size() / 4);
+            CKI(upload(aprog.data(), aprog.size() * 4, &dp)); p.aprog = (u32*)dp;
             CKI(upload(rnd_flat.data(), rnd_flat.size() * 8, &dp)); p.rnd = (u64*)dp;
             fa = flat(n_mtr, n_atr);
             CKI(upload(fa.data(), fa.size() * 8, &dp)); p.atcoef = (u64*)dp;
@@ -1015,8 +1034,8 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
         // the kernel compiled for this AIR (NVRTC, jit.cu) when there is one, else the interpreter
         cudaKernel_t jk = nullptr;
         const bool jit = ctx->jit_enabled &&
-                         wf_jit_get_kernel(ctx, wf_jit_source(D, air.w, (u32)air.periodic.size(), air.num_regs, air.prog, air.consts, aw, air.nr,
-                                                              air.aux_num_regs, air.aux_prog), &jk) == WF_OK;
+                         wf_jit_get_kernel(ctx, wf_jit_source(D, air.w, (u32)air.periodic.size(), air.num_regs, prog, air.consts, aw, air.nr,
+                                                              air.aux_num_regs, aprog), &jk) == WF_OK;
         const unsigned blocks = (unsigned)(((ce_rows ? ce_rows : ce) + 127) / 128);
         if (jit) {
             void* args[] = {&p};
@@ -2317,30 +2336,45 @@ extern "C" int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t a
 //      and the concrete steps between them, for a host that keeps the transcript itself ----------------
 template <int D>
 static int eval_constraints_entry(wf_ctx* ctx, const AirHost& air, u32 log_n, u32 log_b, const wf_mat* lde, const wf_mat* alde,
-                                  const uint64_t* coeffs, const uint64_t* aux_rand, wf_mat** out) {
+                                  const uint64_t* coeffs, const uint64_t* aux_rand, wf_mat** out, size_t row0 = 0, size_t ce_rows = 0) {
     const size_t ncc = air.degrees.size() + air.aux_degrees.size() + air.asserts.size() + air.aux_asserts.size();
     std::vector<GlExt<D>> cc(ncc);
     for (size_t i = 0; i < ncc; i++) for (int q = 0; q < D; q++) cc[i].v[q] = coeffs[i * D + q];
     std::vector<u64> rnd;
     if (air.aw) rnd.assign(aux_rand, aux_rand + (size_t)air.nr * D);
-    CKI(eval_constraints<D>(ctx, air, lde, alde, cc, rnd, log_n, log_b, out));
-    if (ctx->validate) {   // validate_transition_degrees, as evaluator/default.rs:114 runs it after the evaluation
+    CKI(eval_constraints<D>(ctx, air, lde, alde, cc, rnd, log_n, log_b, out, row0, ce_rows));
+    if (ctx->validate && !ce_rows) {   // validate_transition_degrees, as evaluator/default.rs:114 runs it after the evaluation
         TraceReport rep;
         const int r = validation_result(ctx, wf_check_degrees(ctx, air, lde, alde, rnd.data(), log_n, log_b, D, rep), rep);
         if (r != WF_OK) { wf_mat_free(ctx, *out); *out = nullptr; return r; }
     }
     return WF_OK;
 }
-extern "C" int wf_eval_constraints(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup,
-                                   uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs,
-                                   const uint64_t* aux_rand, wf_mat** out) {
+// The LDE rows a call over CE rows [row0, row0 + ce_rows) reads (ce_rows = 0: the whole domain, row0 = 0): the whole LDE, or the
+// window's rows followed by `blowup` halo rows (the layout shard_lde_rows gives the row-sharded prover). Refuses a window outside
+// the domain or of fewer than 64 rows.
+static int check_window(wf_ctx* ctx, u32 log_n, u32 log_b, u32 log_ceb, size_t row0, size_t ce_rows, size_t* lde_rows) {
+    const size_t ce = (size_t)1 << (log_n + log_ceb);
+    if (!ce_rows) {
+        if (row0) return wf_fail(ctx, WF_ERR_INVALID, "row0 without a window");
+        *lde_rows = (size_t)1 << (log_n + log_b);
+        return WF_OK;
+    }
+    if (ce_rows < 64 || row0 >= ce || ce_rows > ce - row0) return wf_fail(ctx, WF_ERR_INVALID, "CE row window outside the domain or under 64 rows");
+    *lde_rows = (ce_rows << (log_b - log_ceb)) + ((size_t)1 << log_b);
+    return WF_OK;
+}
+static int eval_constraints_desc(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup, uint32_t ext,
+                                 const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs, const uint64_t* aux_rand,
+                                 size_t row0, size_t ce_rows, wf_mat** out) {
     if (!ctx || !air_desc || !main_lde || !coeffs || !out || log_n < 3 || blowup < 2 || (blowup & (blowup - 1)))
         return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     AirHost air;
     if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
     const u32 log_b = log2_ceil(blowup);
-    const size_t N = (size_t)1 << (log_n + log_b);
     if (air.log_ce_blowup() > log_b) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
+    size_t N = 0;
+    CKI(check_window(ctx, log_n, log_b, air.log_ce_blowup(), row0, ce_rows, &N));
     if (main_lde->m.rows != N || main_lde->m.cols != air.w) return wf_fail(ctx, WF_ERR_INVALID, "main LDE shape does not match the AIR");
     if (air.aw && (!aux_lde || !aux_rand || aux_lde->m.rows != N || aux_lde->m.cols != air.aw * ext))
         return wf_fail(ctx, WF_ERR_INVALID, "aux LDE / random elements missing or of the wrong shape");
@@ -2350,11 +2384,39 @@ extern "C" int wf_eval_constraints(wf_ctx* ctx, const uint64_t* air_desc, size_t
     CKI(validate_assertions(ctx, air.asserts, (size_t)1 << log_n, 1, "assertion"));
     const wf_mat* al = air.aw ? aux_lde : nullptr;
     switch (ext) {
-        case 1: return eval_constraints_entry<1>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out);
-        case 2: return eval_constraints_entry<2>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out);
-        case 3: return eval_constraints_entry<3>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out);
+        case 1: return eval_constraints_entry<1>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out, row0, ce_rows);
+        case 2: return eval_constraints_entry<2>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out, row0, ce_rows);
+        case 3: return eval_constraints_entry<3>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out, row0, ce_rows);
     }
     return wf_fail(ctx, WF_ERR_UNSUPPORTED, "field extension %u", ext);
+}
+extern "C" int wf_eval_constraints(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup,
+                                   uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs,
+                                   const uint64_t* aux_rand, wf_mat** out) {
+    return eval_constraints_desc(ctx, air_desc, air_desc_len, log_n, blowup, ext, main_lde, aux_lde, coeffs, aux_rand, 0, 0, out);
+}
+extern "C" int wf_eval_constraints_window(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup,
+                                          uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs,
+                                          const uint64_t* aux_rand, size_t row0, size_t ce_rows, wf_mat** out) {
+    if (!ce_rows) return wf_fail(ctx, WF_ERR_INVALID, "empty CE row window");
+    return eval_constraints_desc(ctx, air_desc, air_desc_len, log_n, blowup, ext, main_lde, aux_lde, coeffs, aux_rand, row0, ce_rows, out);
+}
+extern "C" int wf_eval_constraints_fib(wf_ctx* ctx, uint32_t k, const uint64_t* results, uint32_t log_n, uint32_t blowup, uint32_t ext,
+                                       const wf_mat* lde, const uint64_t* coeffs, size_t row0, size_t ce_rows, wf_mat** out) {
+    if (!ctx || !results || !lde || !coeffs || !out || k == 0 || 2 * k > 255 || log_n < 3 || blowup < 2 ||
+        (blowup & (blowup - 1)) || blowup > 128)
+        return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    const u32 log_b = log2_ceil(blowup);
+    const AirHost air = fib_air_host(k, (size_t)1 << log_n, results);
+    size_t N = 0;
+    CKI(check_window(ctx, log_n, log_b, air.log_ce_blowup(), row0, ce_rows, &N));
+    if (lde->m.rows != N || lde->m.cols != 2 * k) return wf_fail(ctx, WF_ERR_INVALID, "LDE shape does not match FibSmall x %u", k);
+    switch (ext) {
+        case 1: return eval_constraints_entry<1>(ctx, air, log_n, log_b, lde, nullptr, coeffs, nullptr, out, row0, ce_rows);
+        case 2: return eval_constraints_entry<2>(ctx, air, log_n, log_b, lde, nullptr, coeffs, nullptr, out, row0, ce_rows);
+        case 3: return eval_constraints_entry<3>(ctx, air, log_n, log_b, lde, nullptr, coeffs, nullptr, out, row0, ce_rows);
+    }
+    return wf_fail(ctx, WF_ERR_INVALID, "field extension %u", ext);
 }
 
 extern "C" int wf_composition_commit(wf_ctx* ctx, int hash_id, const wf_mat* comp_trace, uint32_t log_n, uint32_t blowup, uint32_t ext,
