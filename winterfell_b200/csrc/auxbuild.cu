@@ -4,10 +4,15 @@
 //   aux_term_kernel    interprets the column's program for a run of AUX_TERM_ROWS consecutive rows per thread, registers in a
 //                      local array as in the interpreted generic_constraints_kernel; the run's denominators share one extension
 //                      field inversion (Montgomery's trick). POINTWISE columns are written straight into the aux matrix, the
-//                      running kinds into a term buffer [n][D].
+//                      running kinds into a term buffer [n][D], LINEAR_RECURRENCE columns the pair (m_i, t_i) into [n][2D].
 //   aux_scan_reduce    per tile of AUX_SCAN_TILE rows: the product / sum of its terms;
 //   aux_scan_carry     one block: exclusive scan of the tile aggregates, seeded with the column's init;
 //   aux_scan_apply     per tile: block-wide exclusive scan with the tile's carry-in, written into the aux matrix.
+//   aux_affine_reduce / _carry / _apply   the same three steps for LINEAR_RECURRENCE columns, over the affine maps
+//                      x -> m_i x + t_i: a tile's aggregate is the composition of its rows' maps, the carry is the column's value
+//                      at each tile start (the composed prefix applied to init). Composition does not commute, so every step
+//                      keeps the rows in order: a thread combines consecutive rows, and the warp and block steps keep the
+//                      earlier operand on the left.
 // Field arithmetic is exact, so the association order of the scan does not change a bit of the result.
 #include "internal.hpp"
 #include "constraints_generic.cuh"  // ld_ext, seg_at, AUX_MAX_REGS
@@ -29,7 +34,7 @@ struct AuxTermParams {
     const u32* ptab_off;
     const u32* ptab_len;   // powers of two
     const u64* rnd;        // [nr][D]
-    u64* terms;            // [n][D] running kinds; nullptr: POINTWISE, written into aux column `col`
+    u64* terms;            // [n][D] running kinds, [n][2D] (m_i, t_i) LINEAR_RECURRENCE; nullptr: POINTWISE, written into aux column `col`
 };
 
 template <int D>
@@ -41,12 +46,13 @@ __device__ __forceinline__ void st_aux(const SegMatrix& m, size_t row, u32 col, 
     }
 }
 
-template <int D>
+// AFFINE: a LINEAR_RECURRENCE column, whose program also gives the multiplier m_i (OUT 2)
+template <int D, bool AFFINE>
 __global__ void __launch_bounds__(AUX_TERM_THREADS) aux_term_kernel(AuxTermParams p) {
     const size_t n = (size_t)1 << p.log_n;
     const size_t row0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * AUX_TERM_ROWS;
     if (row0 >= n) return;
-    GlExt<D> num[AUX_TERM_ROWS], den[AUX_TERM_ROWS], pre[AUX_TERM_ROWS];
+    GlExt<D> num[AUX_TERM_ROWS], den[AUX_TERM_ROWS], pre[AUX_TERM_ROWS], mlt[AUX_TERM_ROWS];
     bool zero[AUX_TERM_ROWS];
     GlExt<D> run = ext_from_base<D>(1);
     GlExt<D> ra[AUX_MAX_REGS];
@@ -74,7 +80,11 @@ __global__ void __launch_bounds__(AUX_TERM_THREADS) aux_term_kernel(AuxTermParam
                 case 1: ra[dst] = ext_sub(ra[a], ra[b]); break;
                 case 2: ra[dst] = ext_mul(ra[a], ra[b]); break;
                 case 3: ra[dst] = ext_from_base<D>(p.consts[a]); break;
-                default: if (dst == 0) num[r] = ra[a]; else den[r] = ra[a]; break;  // OUT 0 numerator, OUT 1 denominator
+                default:  // OUT 0 numerator, OUT 1 denominator, OUT 2 multiplier
+                    if (dst == 0) num[r] = ra[a];
+                    else if (AFFINE && dst == 2) mlt[r] = ra[a];
+                    else den[r] = ra[a];
+                    break;
             }
         }
         // Montgomery's trick; a zero denominator becomes 1 inside the batch and its term 0 (inv(0) = 0)
@@ -92,7 +102,10 @@ __global__ void __launch_bounds__(AUX_TERM_THREADS) aux_term_kernel(AuxTermParam
         run = ext_mul(run, den[r]);
         const GlExt<D> t = zero[r] ? ext_zero<D>() : ext_mul(num[r], inv);
         const size_t i = row0 + r;
-        if (p.terms) {
+        if (AFFINE) {
+#pragma unroll
+            for (int q = 0; q < D; q++) { p.terms[i * 2 * D + q] = mlt[r].v[q]; p.terms[i * 2 * D + D + q] = t.v[q]; }
+        } else if (p.terms) {
 #pragma unroll
             for (int q = 0; q < D; q++) p.terms[i * D + q] = t.v[q];
         } else {
@@ -112,42 +125,71 @@ __device__ __forceinline__ GlExt<D> shfl_up_ext(const GlExt<D>& v, u32 off) {
     for (int q = 0; q < D; q++) r.v[q] = __shfl_up_sync(0xffffffffu, v.v[q], off);
     return r;
 }
-// exclusive scan of one value per thread over the block (AUX_SCAN_THREADS threads); `total` = the whole block's result
+// The combine of a block scan as a type: T its state, W its u64 words, id() the identity, op(a, b) = a then b (the earlier
+// operand on the left), and T's warp shuffle and memory forms.
 template <int D, bool MUL>
-__device__ __forceinline__ GlExt<D> block_exclusive_scan(const GlExt<D>& v, GlExt<D>& total) {
-    __shared__ u64 wsum[AUX_SCAN_THREADS / 32][D];
+struct RunOp {   // RUNNING_PRODUCT / RUNNING_SUM: one extension element
+    using T = GlExt<D>;
+    static constexpr int W = D;
+    static __device__ __forceinline__ T id() { return scan_id<D, MUL>(); }
+    static __device__ __forceinline__ T op(const T& a, const T& b) { return scan_op<D, MUL>(a, b); }
+    static __device__ __forceinline__ T shfl_up(const T& v, u32 off) { return shfl_up_ext(v, off); }
+    static __device__ __forceinline__ T ld(const u64* p) { return ld_ext<D>(p); }
+    static __device__ __forceinline__ void st(u64* p, const T& v) {
+#pragma unroll
+        for (int q = 0; q < D; q++) p[q] = v.v[q];
+    }
+};
+template <int D>
+struct Affine { GlExt<D> m, t; };   // the map x -> m x + t; in memory m then t, 2D words
+template <int D>
+__device__ __forceinline__ GlExt<D> aff_apply(const Affine<D>& a, const GlExt<D>& x) { return ext_add(ext_mul(a.m, x), a.t); }
+template <int D>
+struct AffOp {   // LINEAR_RECURRENCE: composition of affine maps; a then b = (a.m b.m, b.m a.t + b.t)
+    using T = Affine<D>;
+    static constexpr int W = 2 * D;
+    static __device__ __forceinline__ T id() { return {ext_from_base<D>(1), ext_zero<D>()}; }
+    static __device__ __forceinline__ T op(const T& a, const T& b) { return {ext_mul(a.m, b.m), aff_apply(b, a.t)}; }
+    static __device__ __forceinline__ T shfl_up(const T& v, u32 off) { return {shfl_up_ext(v.m, off), shfl_up_ext(v.t, off)}; }
+    static __device__ __forceinline__ T ld(const u64* p) { return {ld_ext<D>(p), ld_ext<D>(p + D)}; }
+    static __device__ __forceinline__ void st(u64* p, const T& v) {
+#pragma unroll
+        for (int q = 0; q < D; q++) { p[q] = v.m.v[q]; p[D + q] = v.t.v[q]; }
+    }
+};
+
+// exclusive scan of one value per thread over the block (AUX_SCAN_THREADS threads), in thread order; `total` = the whole
+// block's result
+template <class Op>
+__device__ __forceinline__ typename Op::T block_exclusive_scan(const typename Op::T& v, typename Op::T& total) {
+    using T = typename Op::T;
+    __shared__ u64 wsum[AUX_SCAN_THREADS / 32][Op::W];
     const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     constexpr u32 NW = AUX_SCAN_THREADS / 32;
-    GlExt<D> x = v;
+    T x = v;
 #pragma unroll
     for (u32 off = 1; off < 32; off <<= 1) {
-        const GlExt<D> y = shfl_up_ext(x, off);
-        if (lane >= off) x = scan_op<D, MUL>(y, x);
+        const T y = Op::shfl_up(x, off);
+        if (lane >= off) x = Op::op(y, x);
     }
-    if (lane == 31) {
-#pragma unroll
-        for (int q = 0; q < D; q++) wsum[wid][q] = x.v[q];
-    }
+    if (lane == 31) Op::st(&wsum[wid][0], x);
     __syncthreads();
     if (wid == 0) {
-        GlExt<D> s = lane < NW ? ld_ext<D>(&wsum[lane][0]) : scan_id<D, MUL>();
+        T s = lane < NW ? Op::ld(&wsum[lane][0]) : Op::id();
 #pragma unroll
         for (u32 off = 1; off < NW; off <<= 1) {
-            const GlExt<D> y = shfl_up_ext(s, off);
-            if (lane >= off) s = scan_op<D, MUL>(y, s);
+            const T y = Op::shfl_up(s, off);
+            if (lane >= off) s = Op::op(y, s);
         }
-        if (lane < NW) {
-#pragma unroll
-            for (int q = 0; q < D; q++) wsum[lane][q] = s.v[q];
-        }
+        if (lane < NW) Op::st(&wsum[lane][0], s);
     }
     __syncthreads();
-    total = ld_ext<D>(&wsum[NW - 1][0]);
-    const GlExt<D> wpre = wid ? ld_ext<D>(&wsum[wid - 1][0]) : scan_id<D, MUL>();
-    GlExt<D> ex = shfl_up_ext(x, 1);
-    if (lane == 0) ex = scan_id<D, MUL>();
+    total = Op::ld(&wsum[NW - 1][0]);
+    const T wpre = wid ? Op::ld(&wsum[wid - 1][0]) : Op::id();
+    T ex = Op::shfl_up(x, 1);
+    if (lane == 0) ex = Op::id();
     __syncthreads();  // wsum is free for the next call
-    return scan_op<D, MUL>(wpre, ex);
+    return Op::op(wpre, ex);
 }
 
 template <int D, bool MUL>
@@ -160,7 +202,7 @@ __global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_scan_reduce(const u64* t
         if (i < n) v = scan_op<D, MUL>(v, ld_ext<D>(terms + i * D));
     }
     GlExt<D> total;
-    block_exclusive_scan<D, MUL>(v, total);
+    block_exclusive_scan<RunOp<D, MUL>>(v, total);
     if (threadIdx.x == 0) {
 #pragma unroll
         for (int q = 0; q < D; q++) agg[(size_t)blockIdx.x * D + q] = total.v[q];
@@ -175,7 +217,7 @@ __global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_scan_carry(u64* agg, siz
     GlExt<D> v = scan_id<D, MUL>();
     for (size_t i = b; i < e; i++) v = scan_op<D, MUL>(v, ld_ext<D>(agg + i * D));
     GlExt<D> total;
-    GlExt<D> run = scan_op<D, MUL>(init, block_exclusive_scan<D, MUL>(v, total));
+    GlExt<D> run = scan_op<D, MUL>(init, block_exclusive_scan<RunOp<D, MUL>>(v, total));
     for (size_t i = b; i < e; i++) {
         const GlExt<D> a = ld_ext<D>(agg + i * D);
 #pragma unroll
@@ -194,13 +236,68 @@ __global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_scan_apply(const u64* te
     for (int k = 0; k < AUX_SCAN_ITEMS; k++)
         if (r0 + k < n) v = scan_op<D, MUL>(v, ld_ext<D>(terms + (r0 + k) * D));
     GlExt<D> total;
-    GlExt<D> run = scan_op<D, MUL>(ld_ext<D>(carry + (size_t)blockIdx.x * D), block_exclusive_scan<D, MUL>(v, total));
+    GlExt<D> run = scan_op<D, MUL>(ld_ext<D>(carry + (size_t)blockIdx.x * D), block_exclusive_scan<RunOp<D, MUL>>(v, total));
 #pragma unroll
     for (int k = 0; k < AUX_SCAN_ITEMS; k++) {
         const size_t i = r0 + k;
         if (i < n) {
             st_aux<D>(out, i, col, run);
             run = scan_op<D, MUL>(run, ld_ext<D>(terms + i * D));
+        }
+    }
+}
+
+// The composition of the maps of rows r0 .. r0 + AUX_SCAN_ITEMS - 1 (those < n), in row order; the identity when r0 >= n.
+template <int D>
+__device__ __forceinline__ Affine<D> affine_run(const u64* terms, size_t n, size_t r0) {
+    Affine<D> v = r0 < n ? AffOp<D>::ld(terms + r0 * 2 * D) : AffOp<D>::id();
+#pragma unroll
+    for (int k = 1; k < AUX_SCAN_ITEMS; k++)
+        if (r0 + k < n) v = AffOp<D>::op(v, AffOp<D>::ld(terms + (r0 + k) * 2 * D));
+    return v;
+}
+
+// per tile: the composition of its rows' maps into agg [ntiles][2D]; thread t owns AUX_SCAN_ITEMS consecutive rows
+template <int D>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_affine_reduce(const u64* terms, size_t n, u64* agg) {
+    const Affine<D> v = affine_run<D>(terms, n, (size_t)blockIdx.x * AUX_SCAN_TILE + (size_t)threadIdx.x * AUX_SCAN_ITEMS);
+    Affine<D> total;
+    block_exclusive_scan<AffOp<D>>(v, total);
+    if (threadIdx.x == 0) AffOp<D>::st(agg + (size_t)blockIdx.x * 2 * D, total);
+}
+
+// one block; tile maps -> the column's value at each tile start (the maps of the tiles before it applied to init), written
+// over the first D words of the tile's slot. Thread t owns a run of consecutive tiles.
+template <int D>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_affine_carry(u64* agg, size_t ntiles, GlExt<D> init) {
+    const size_t per = (ntiles + AUX_SCAN_THREADS - 1) / AUX_SCAN_THREADS;
+    const size_t b = threadIdx.x * per, e = b + per < ntiles ? b + per : ntiles;
+    Affine<D> v = AffOp<D>::id();
+    for (size_t i = b; i < e; i++) v = AffOp<D>::op(v, AffOp<D>::ld(agg + i * 2 * D));
+    Affine<D> total;
+    GlExt<D> x = aff_apply(block_exclusive_scan<AffOp<D>>(v, total), init);
+    for (size_t i = b; i < e; i++) {
+        const Affine<D> a = AffOp<D>::ld(agg + i * 2 * D);
+#pragma unroll
+        for (int q = 0; q < D; q++) agg[i * 2 * D + q] = x.v[q];
+        x = aff_apply(a, x);
+    }
+}
+
+// a[i] = the maps of the tile's rows before i applied to the tile's carry-in, written as aux column `col`; thread t owns
+// AUX_SCAN_ITEMS consecutive rows (the second pass re-reads them from L1)
+template <int D>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_affine_apply(const u64* terms, size_t n, const u64* carry, SegMatrix out, u32 col) {
+    const size_t r0 = (size_t)blockIdx.x * AUX_SCAN_TILE + (size_t)threadIdx.x * AUX_SCAN_ITEMS;
+    const Affine<D> v = affine_run<D>(terms, n, r0);
+    Affine<D> total;
+    GlExt<D> x = aff_apply(block_exclusive_scan<AffOp<D>>(v, total), ld_ext<D>(carry + (size_t)blockIdx.x * 2 * D));
+#pragma unroll 1   // unrolled, the D = 3 kernel spills to local memory
+    for (int k = 0; k < AUX_SCAN_ITEMS; k++) {
+        const size_t i = r0 + k;
+        if (i < n) {
+            st_aux<D>(out, i, col, x);
+            x = aff_apply(AffOp<D>::ld(terms + i * 2 * D), x);
         }
     }
 }
@@ -225,7 +322,7 @@ const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, 
     for (u32 j = 0; j < aw; j++) {
         AuxBuildCol c;
         if (!rd(v)) return "malformed aux build description";
-        if (v > 2) return "unknown aux column kind";
+        if (v > 2 && v != 4) return "unknown aux column kind";
         c.kind = (u32)v;
         for (int q = 0; q < 3; q++) {
             if (!rd(c.init[q])) return "malformed aux build description";
@@ -237,14 +334,16 @@ const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, 
         if (!rd(cnt) || cnt > (1u << 20)) return "malformed aux build description";
         std::vector<bool> written(c.num_regs, false);
         for (u32 r = 0; r < first_tmp; r++) written[r] = !(r >= ab && r < pb) || ((r - ab) % aw) < j;
-        u32 outs[2] = {0, 0};
+        const bool affine = c.kind == 4;
+        u32 outs[3] = {0, 0, 0};
         for (u64 k = 0; k < cnt; k++) {
             u64 op, ds, x, y;
             if (!rd(op) || !rd(ds) || !rd(x) || !rd(y)) return "malformed aux build description";
             if (op > 4) return "unknown aux build opcode";
             auto readable = [&](u64 r) { return r < c.num_regs && written[r]; };
             if (op == 4) {
-                if (ds > 1) return "aux build OUT selects neither numerator (0) nor denominator (1)";
+                if (affine && ds > 2) return "aux build OUT selects neither numerator (0), denominator (1) nor multiplier (2)";
+                if (!affine && ds > 1) return "aux build OUT selects neither numerator (0) nor denominator (1)";
                 if (!readable(x)) return "aux build program reads a register out of range, an aux column >= its own, or an unwritten temporary";
                 outs[ds]++;
             } else {
@@ -258,6 +357,8 @@ const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, 
         }
         if (outs[0] != 1) return "aux build column needs exactly one numerator (OUT 0)";
         if (outs[1] > 1) return "aux build column has more than one denominator (OUT 1)";
+        if (affine && outs[2] == 0) return "aux build LINEAR_RECURRENCE column has no multiplier (OUT 2)";
+        if (affine && outs[2] > 1) return "aux build LINEAR_RECURRENCE column has more than one multiplier (OUT 2)";
         b.cols.push_back(c);
     }
     if (p != len) return "malformed aux build description";
@@ -272,6 +373,20 @@ static int aux_scan(wf_ctx* ctx, const u64* terms, size_t n, u64* agg, const u64
     aux_scan_reduce<D, MUL><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(terms, n, agg);
     aux_scan_carry<D, MUL><<<1, AUX_SCAN_THREADS, 0, ctx->st>>>(agg, ntiles, in);
     aux_scan_apply<D, MUL><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(terms, n, agg, out, col);
+    ctx->launches += 3;
+    CK(cudaGetLastError());
+    return WF_OK;
+}
+
+// terms: [n][2D] (m_i, t_i); agg: [ntiles][2D]
+template <int D>
+static int aux_affine(wf_ctx* ctx, const u64* terms, size_t n, u64* agg, const u64* init, SegMatrix out, u32 col) {
+    const size_t ntiles = (n + AUX_SCAN_TILE - 1) / AUX_SCAN_TILE;
+    GlExt<D> in;
+    for (int q = 0; q < D; q++) in.v[q] = init[q];
+    aux_affine_reduce<D><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(terms, n, agg);
+    aux_affine_carry<D><<<1, AUX_SCAN_THREADS, 0, ctx->st>>>(agg, ntiles, in);
+    aux_affine_apply<D><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(terms, n, agg, out, col);
     ctx->launches += 3;
     CK(cudaGetLastError());
     return WF_OK;
@@ -297,14 +412,15 @@ static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u
     if (u32s.size() & 1) u32s.push_back(0);
     const size_t o_u32 = up.size();
     for (size_t i = 0; i < u32s.size(); i += 2) up.push_back((u64)u32s[i] | ((u64)u32s[i + 1] << 32));
-    bool running = false;
-    for (auto& c : b.cols) running = running || c.kind != 0;
+    bool running = false, affine = false;
+    for (auto& c : b.cols) { running = running || c.kind != 0; affine = affine || c.kind == 4; }
+    const size_t tw = affine ? 2 * D : D;   // words per row of the term buffer: (m_i, t_i) when a column needs them
     DevScratch tmp(ctx);
     void *d_up, *d_terms = nullptr, *d_agg = nullptr;
     CKI(tmp.alloc(std::max(up.size(), (size_t)1) * 8, &d_up));
     if (running) {
-        CKI(tmp.alloc(n * D * 8, &d_terms));
-        CKI(tmp.alloc((n + AUX_SCAN_TILE - 1) / AUX_SCAN_TILE * D * 8, &d_agg));
+        CKI(tmp.alloc(n * tw * 8, &d_terms));
+        CKI(tmp.alloc((n + AUX_SCAN_TILE - 1) / AUX_SCAN_TILE * tw * 8, &d_agg));
     }
     CK(cudaMemcpyAsync(d_up, up.data(), up.size() * 8, cudaMemcpyHostToDevice, ctx->st));
     wf_mat* a;
@@ -323,11 +439,13 @@ static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u
         p.prog = dev32 + prog_off[j];
         p.prog_len = (u32)(c.prog.size() / 4);
         p.terms = c.kind ? (u64*)d_terms : nullptr;
-        aux_term_kernel<D><<<grid, AUX_TERM_THREADS, 0, ctx->st>>>(p);
+        if (c.kind == 4) aux_term_kernel<D, true><<<grid, AUX_TERM_THREADS, 0, ctx->st>>>(p);
+        else aux_term_kernel<D, false><<<grid, AUX_TERM_THREADS, 0, ctx->st>>>(p);
         ctx->launches++;
         if (cudaGetLastError() != cudaSuccess) { r = wf_fail(ctx, WF_ERR_CUDA, "aux_term_kernel launch failed"); break; }
         if (c.kind == 1) r = aux_scan<D, true>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
         else if (c.kind == 2) r = aux_scan<D, false>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
+        else if (c.kind == 4) r = aux_affine<D>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
     }
     if (r != WF_OK) { wf_mat_free(ctx, a); return r; }
     *out = a;
