@@ -539,6 +539,14 @@ int wf_eval_constraints_window(wf_ctx* ctx, const uint64_t* air_desc, size_t air
  * LDE; otherwise the window of wf_eval_constraints_window. */
 int wf_eval_constraints_fib(wf_ctx* ctx, uint32_t k, const uint64_t* results, uint32_t log_n, uint32_t blowup, uint32_t ext,
                             const wf_mat* lde, const uint64_t* coeffs, size_t row0, size_t ce_rows, wf_mat** out);
+/* the constraint evaluation of wf_eval_constraints (resp. wf_eval_constraints_fib) on the sub-coset of `rows` points of the CE
+ * domain only (rows a power of two, at most n * ce_blowup), as wf_prove_air / wf_prove_fib run it: the composition polynomial is
+ * interpolated from those rows. Takes the whole LDEs; *out = rows x ext, row j = CE row j * (n * ce_blowup / rows). */
+int wf_eval_constraints_subcoset(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup,
+                                 uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs,
+                                 const uint64_t* aux_rand, size_t rows, wf_mat** out);
+int wf_eval_constraints_fib_subcoset(wf_ctx* ctx, uint32_t k, const uint64_t* results, uint32_t log_n, uint32_t blowup, uint32_t ext,
+                                     const wf_mat* lde, const uint64_t* coeffs, size_t rows, wf_mat** out);
 
 /* ---- host-side helpers of the product (transcript arithmetic; no GPU needed) ------------------- */
 /* H::hash_elements / merge / merge_with_int on the host (crypto/src/hash/mod.rs:31-64) */

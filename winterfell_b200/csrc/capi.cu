@@ -731,6 +731,20 @@ int wf_mat_lde_cosets(wf_ctx* ctx, const wf_mat* polys, uint32_t log_blowup, uin
     return run_lde(ctx, polys->m, lde->m, log_n, log_blowup, 0, k0, k1, 1, (u32)polys->m.rows);
 }
 
+// Cosets k0 <= k < blowup of the LDE in natural order (row b*j + k of `lde`, as wf_mat_lde_into writes it); the rows of cosets
+// below k0 are left as they are. For a caller that holds the first cosets' values already (the composition polynomial, prover.cu).
+int wf_mat_lde_from_coset(wf_ctx* ctx, const wf_mat* polys, uint32_t log_blowup, uint32_t k0, wf_mat* lde) {
+    if (!ctx || !polys || !lde) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    u32 log_n;
+    if (log2_exact(polys->m.rows, &log_n) || log_n < 1) return wf_fail(ctx, WF_ERR_INVALID, "rows must be a power of two >= 2");
+    if (log_blowup > 7 || k0 >= (1u << log_blowup) || lde->m.rows != (polys->m.rows << log_blowup) || lde->m.cols != polys->m.cols ||
+        lde->m.W != polys->m.W)
+        return wf_fail(ctx, WF_ERR_INVALID, "coset / output matrix do not match the LDE shape");
+    SegMatrix view = lde->m;   // run_lde places its first coset at the view's origin: row k0 of the natural order
+    view.base += (size_t)k0 * view.W;
+    return run_lde(ctx, polys->m, view, log_n, log_blowup, 0, k0, 1u << log_blowup);
+}
+
 // DefaultTraceLde::new up to the commitment (trace_lde/default/mod.rs:63-100, build_trace_commitment
 // :245-282) from HOST columns, with the upload pipelined against the transforms: the columns are cut
 // into chunks (whole 8-column segments when there are several, else the two halves of the one segment);

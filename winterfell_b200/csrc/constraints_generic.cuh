@@ -73,6 +73,9 @@ struct GenEvalParams {
     // LDE rows of that range followed by `blowup` halo rows (the first rows of the next shard), so the next-state row is local
     // row + blowup without wrap-around, and `out` holds the launch's rows only. ce_rows = 0: the whole domain.
     size_t row0, ce_rows;
+    // sub-coset evaluation (ce_rows = 0 only): launch row il is CE row il << log_step, ce >> log_step rows in all. Everything that
+    // depends on the row (LDE rows, x, periodic and sequence values, exemptions) is keyed on the CE row.
+    u32 log_step;
 };
 
 #ifdef WF_JIT
@@ -119,10 +122,11 @@ template <int D, bool AUX>
 __device__ __forceinline__ void generic_constraints_row(const GenEvalParams& p) {
     const size_t ce = (size_t)1 << (p.log_n + p.log_ce_blowup);
     const size_t il = (size_t)blockIdx.x * blockDim.x + threadIdx.x;   // row of this launch
-    if (il >= (p.ce_rows ? p.ce_rows : ce)) return;
-    const size_t i = il + p.row0;                                       // row of the CE domain
+    if (il >= (p.ce_rows ? p.ce_rows : ce >> p.log_step)) return;
+    const size_t ic = il << p.log_step;                                 // its CE row, local to the shard
+    const size_t i = ic + p.row0;                                       // row of the CE domain
     const size_t N = (size_t)1 << (p.log_n + p.log_blowup);
-    const size_t ls = il << (p.log_blowup - p.log_ce_blowup);
+    const size_t ls = ic << (p.log_blowup - p.log_ce_blowup);
     const size_t nx = p.ce_rows ? ls + ((size_t)1 << p.log_blowup) : ((ls + ((size_t)1 << p.log_blowup)) & (N - 1));
     GlExt<D> T = ext_zero<D>();
 #ifdef WF_JIT

@@ -158,6 +158,7 @@ extern "C" int wf_trace_lde_cosetwise(wf_ctx* ctx, const uint64_t* const* cols, 
                            uint32_t log_blowup, wf_mat** polys_out, wf_mat** lde_out, bool coset_major,
                            const std::function<int(u32)>* after_coset);
 extern "C" int wf_mat_lde_cosets(wf_ctx* ctx, const wf_mat* polys, uint32_t log_blowup, uint32_t k0, uint32_t k1, wf_mat* lde);  // internal (not in the public header)
+extern "C" int wf_mat_lde_from_coset(wf_ctx* ctx, const wf_mat* polys, uint32_t log_blowup, uint32_t k0, wf_mat* lde);  // internal
 struct PublicCoin;
 struct Digest;
 struct wf_fri;

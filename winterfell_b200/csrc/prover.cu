@@ -54,6 +54,8 @@ struct FibEvalParams {
     // rows of that range followed by `blowup` halo rows (the first rows of the next shard), so the next-state row is
     // local row + blowup without wrap-around. ce_rows = 0: the whole domain.
     size_t row0, ce_rows;
+    // sub-coset evaluation (ce_rows = 0 only): launch row il is CE row il << log_step, ce >> log_step rows in all
+    u32 log_step;
 };
 
 // CE-domain rows, FIB_ROWS per thread sharing one field inversion (evaluator/default.rs:165-214
@@ -68,7 +70,7 @@ __global__ void __launch_bounds__(256) fib_constraints_kernel(FibEvalParams p) {
     for (u32 i = threadIdx.x; i < p.k * 5 * D; i += blockDim.x) fsm[i] = p.coef[i];
     __syncthreads();
     const size_t ce_all = (size_t)1 << (p.log_n + p.log_ce_blowup);
-    const size_t ce = p.ce_rows ? p.ce_rows : ce_all;   // rows of this launch
+    const size_t ce = p.ce_rows ? p.ce_rows : ce_all >> p.log_step;   // rows of this launch
     const size_t N = (size_t)1 << (p.log_n + p.log_blowup);
     const u32 lde_shift = p.log_blowup - p.log_ce_blowup;
     const size_t stride = (size_t)gridDim.x * blockDim.x;
@@ -80,11 +82,12 @@ __global__ void __launch_bounds__(256) fib_constraints_kernel(FibEvalParams p) {
 #pragma unroll
     for (int r = 0; r < ROWS; r++) {
         const size_t il = tid + r * stride;   // row of this launch
-        const size_t i = il + p.row0;         // row of the CE domain
+        const size_t ic = il << p.log_step;   // its CE row, local to the shard
+        const size_t i = ic + p.row0;         // row of the CE domain
         T[r] = ext_zero<D>(); B0[r] = ext_zero<D>(); B1[r] = ext_zero<D>();
         d0[r] = 1; d1[r] = 1;
         if (il >= ce) continue;
-        const size_t ls = il << lde_shift;
+        const size_t ls = ic << lde_shift;
         const size_t nx = p.ce_rows ? ls + ((size_t)1 << p.log_blowup)
                                     : ((ls + ((size_t)1 << p.log_blowup)) & (N - 1));  // trace_lde/default/mod.rs:169-180
         GlAcc aT[D], a0[D], a1[D];
@@ -129,7 +132,7 @@ __global__ void __launch_bounds__(256) fib_constraints_kernel(FibEvalParams p) {
     for (int r = ROWS - 1; r >= 0; r--) { u64 inv = gl_mul(run, pre[r]); run = gl_mul(run, prod[r]); prod[r] = inv; }
 #pragma unroll
     for (int r = 0; r < ROWS; r++) {
-        const size_t il = tid + r * stride, i = il + p.row0;
+        const size_t il = tid + r * stride, i = (il << p.log_step) + p.row0;
         if (il >= ce) continue;
         u64 z0 = gl_mul(prod[r], d1[r]), z1 = gl_mul(prod[r], d0[r]);                   // 1/(x - 1), 1/(x - g^(n-1))
         u64 zt = gl_mul(p.zt[i & (((size_t)1 << p.log_ce_blowup) - 1)], d1[r]);         // e(x) / (x^n - 1)
@@ -151,6 +154,14 @@ __global__ void comp_split_kernel(SegMatrix coefs, size_t n, u32 kc, int D, SegM
     u32 j = col / D, comp = col % D;
     u64 v = coefs.base[(j * n + i) * coefs.W + comp];
     out.base[(size_t)(col / out.W) * out.seg_stride + i * out.W + (col % out.W)] = v;
+}
+
+// row i of the n x W segment `src` -> row i * b of `dst` (coset 0 of an LDE in natural order), pad lanes included
+__global__ void coset0_rows_kernel(const u64* src, size_t n, int W, u32 b, u64* dst) {
+    const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= n * W) return;
+    const size_t row = idx / W;
+    dst[(row * b) * W + idx % W] = src[idx];
 }
 
 // Evaluation of every base-coefficient column at TWO extension points (z and z*g), as per-block partial sums
@@ -857,16 +868,21 @@ static std::vector<u32> last_outs_only(const std::vector<u32>& prog) {
 // cc: main transition, aux transition, main assertions, aux assertions (sorted order).
 template <int D>
 int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const wf_mat* alde, const std::vector<GlExt<D>>& cc,
-                     const std::vector<u64>& rnd_flat, u32 log_n, u32 log_b, wf_mat** out, size_t row0 = 0, size_t ce_rows = 0) {
+                     const std::vector<u64>& rnd_flat, u32 log_n, u32 log_b, wf_mat** out, size_t row0 = 0, size_t ce_rows = 0,
+                     u32 log_step = 0) {
     // ce_rows != 0: row-sharded call — CE rows [row0, row0 + ce_rows) only; `lde` (and `alde`) then hold the LDE rows of that
     // range followed by `blowup` halo rows (FibEvalParams::row0, GenEvalParams::row0)
+    // log_step != 0: the sub-coset 7 <w_ce^(2^log_step)> only, row j of *out = CE row j << log_step (the rows the composition
+    // polynomial is interpolated from, composition_polys)
     const size_t n = (size_t)1 << log_n;
     const u32 c = air.w, aw = air.aw, log_ceb = air.log_ce_blowup();
     const u32 n_atr = (u32)air.aux_degrees.size(), n_mtr = (u32)air.degrees.size(), n_mas = (u32)air.asserts.size();
     const u32 n_tr = n_mtr + n_atr;
     const size_t ce = n << log_ceb;
+    if (log_step && (ce_rows || log_step > log_n + log_ceb)) return wf_fail(ctx, WF_ERR_INVALID, "CE row step with a row window, or past the domain");
+    const size_t rows = ce_rows ? ce_rows : ce >> log_step;   // rows of *out
     wf_mat* comp;
-    CKI(wf_mat_alloc(ctx, ce_rows ? ce_rows : ce, D, &comp));
+    CKI(wf_mat_alloc(ctx, rows, D, &comp));
     if (comp->m.W > D) CK(cudaMemsetAsync(comp->m.base, 0, comp->m.words() * 8, ctx->st));
     const u64 g_tr = gl_root_of_unity(log_n);
     std::vector<u64> zt((size_t)1 << log_ceb);  // ce_blowup <= blowup <= 128 entries
@@ -922,9 +938,9 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
         p.last = gl_pow(g_tr, n - 1);
         if (log_ceb > 3) return wf_fail(ctx, WF_ERR_STATE, "FibSmall has degree-1 constraints");  // FibEvalParams::zt[8]
         for (u32 i = 0; i < (1u << log_ceb); i++) p.zt[i] = zt[i];
-        p.row0 = row0; p.ce_rows = ce_rows;
+        p.row0 = row0; p.ce_rows = ce_rows; p.log_step = log_step;
         const size_t rows_per_thread = D == 3 ? FIB_ROWS_D3 : 4;
-        size_t threads = ((ce_rows ? ce_rows : ce) + rows_per_thread - 1) / rows_per_thread;
+        size_t threads = (rows + rows_per_thread - 1) / rows_per_thread;
         fib_constraints_kernel<D><<<(unsigned)((threads + 255) / 256), 256, cf.size() * 8, ctx->st>>>(p);
         ctx->launches++;
         CK(cudaGetLastError());
@@ -986,7 +1002,7 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
         CKI(upload(eshift.data(), eshift.size() * 4, &dp)); p.e_shift = (u32*)dp;
         CKI(wf_get_twiddles(ctx, log_n + log_ceb, &p.tw_ce));
         CKI(upload(zt.data(), zt.size() * 8, &dp)); p.zt = (const u64*)dp;
-        p.row0 = row0; p.ce_rows = ce_rows;
+        p.row0 = row0; p.ce_rows = ce_rows; p.log_step = log_step;
         p.num_exempt = air.exemptions;
         for (u32 e = 0; e < air.exemptions; e++) p.exempt[e] = gl_pow(g_tr, n - air.exemptions + e);  // divisor.rs:31-41
         std::vector<u32> agoff = {0}, aecol, aetstride, aeshift;
@@ -1036,7 +1052,7 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
         const bool jit = ctx->jit_enabled &&
                          wf_jit_get_kernel(ctx, wf_jit_source(D, air.w, (u32)air.periodic.size(), air.num_regs, prog, air.consts, aw, air.nr,
                                                               air.aux_num_regs, aprog), &jk) == WF_OK;
-        const unsigned blocks = (unsigned)(((ce_rows ? ce_rows : ce) + 127) / 128);
+        const unsigned blocks = (unsigned)((rows + 127) / 128);
         if (jit) {
             void* args[] = {&p};
             CK(cudaLaunchKernel((const void*)jk, dim3(blocks), dim3(128), args, 0, ctx->st));
@@ -1057,17 +1073,22 @@ int eval_constraints(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const w
 // DefaultConstraintCommitment::new (prover/src/constraints/commitment/default.rs:44-150): composition
 // trace (CE-domain evaluations, ce x D) -> CompositionPoly columns (n x kc*D coefficient matrix,
 // composition_poly.rs:58-78,128-140), their LDE (N x kc*D) and the row commitment.
-// CompositionPoly::new (composition_poly.rs:58-78): CE-domain evaluations -> kc column polynomials of degree < n
+// The composition polynomial has degree < kc * n by the AIR's declared degrees (that is what kc is computed from), so the
+// evaluations on the sub-coset 7 <w_m>, m = the power of two >= kc * n — every (ce / m)-th row of the CE domain — already
+// determine it: the size-m inverse transform returns exactly the coefficients the reference reads out of its size-ce one
+// (whose upper ce - kc * n coefficients are zero, composition_poly.rs:64-70). For FibSmall m = n = ce / 2.
+static size_t comp_subcoset_rows(size_t n, u32 kc) {
+    size_t m = n;
+    while (m < n * kc) m <<= 1;
+    return m;
+}
+// CompositionPoly::new (composition_poly.rs:58-78): CE-domain evaluations -> kc column polynomials of degree < n. `comp` holds
+// either the whole CE domain or only the comp_subcoset_rows(n, kc) rows of the sub-coset.
 int composition_polys(wf_ctx* ctx, const wf_mat* comp, u32 log_n, int D, u32 kc, wf_mat** polys_out) {
     const size_t n = (size_t)1 << log_n;
     if (comp->m.rows < n * kc || (int)comp->m.cols != D) return wf_fail(ctx, WF_ERR_INVALID, "composition trace shape");
     wf_mat *ccoefs, *cpolys;
-    // The composition polynomial has degree < kc * n by the AIR's declared degrees (that is what kc is computed from), so the
-    // evaluations on the sub-coset 7 <w_m>, m = the power of two >= kc * n — every (ce / m)-th row of the CE domain — already
-    // determine it: the size-m inverse transform returns exactly the coefficients the reference reads out of its size-ce one
-    // (whose upper ce - kc * n coefficients are zero, composition_poly.rs:64-70). For FibSmall m = ce / 2.
-    size_t m = n;
-    while (m < n * kc) m <<= 1;
+    const size_t m = comp_subcoset_rows(n, kc);
     if (m < comp->m.rows && comp->m.nseg() == 1) {
         wf_mat* sub;
         CKI(wf_mat_alloc_w(ctx, m, comp->m.cols, comp->m.W, &sub));
@@ -1080,6 +1101,11 @@ int composition_polys(wf_ctx* ctx, const wf_mat* comp, u32 log_n, int D, u32 kc,
     } else {
         CKI(wf_mat_interpolate_with_offset(ctx, comp, GL_GENERATOR, &ccoefs));
     }
+    if (kc == 1 && ccoefs->m.rows == n) {   // one column: the coefficients as they are, in the layout of an n x D matrix
+        wf_mark(ctx, "composition_interpolate");
+        *polys_out = ccoefs;
+        return WF_OK;
+    }
     CKI(wf_mat_alloc(ctx, n, kc * D, &cpolys));
     if (cpolys->m.W > (int)(kc * D)) CK(cudaMemsetAsync(cpolys->m.base, 0, cpolys->m.words() * 8, ctx->st));
     comp_split_kernel<<<(unsigned)((n * kc * D + 255) / 256), 256, 0, ctx->st>>>(ccoefs->m, n, kc, D, cpolys->m);
@@ -1090,11 +1116,32 @@ int composition_polys(wf_ctx* ctx, const wf_mat* comp, u32 log_n, int D, u32 kc,
     *polys_out = cpolys;
     return WF_OK;
 }
+// The LDE of the composition columns. With one column interpolated from n rows, those rows are the column's values at 7 w_n^j:
+// coset 0 of the LDE (rows b*j), which the interpolant reproduces exactly. They are copied there, and only cosets 1..b-1 are
+// transformed.
+static int composition_lde(wf_ctx* ctx, const wf_mat* comp, const wf_mat* cpolys, u32 log_n, u32 log_b, u32 kc, wf_mat** lde_out) {
+    const size_t n = (size_t)1 << log_n;
+    if (kc != 1 || comp->m.rows != n || comp->m.nseg() != 1 || comp->m.W != cpolys->m.W || cpolys->m.nseg() != 1)
+        return wf_mat_lde(ctx, cpolys, log_b, lde_out);
+    if (log_b > 7 || log_n + log_b > 32) return wf_fail(ctx, WF_ERR_INVALID, "bad blowup");
+    const u32 b = 1u << log_b;
+    wf_mat* clde;
+    CKI(wf_mat_alloc(ctx, n << log_b, cpolys->m.cols, &clde));
+    // a kernel rather than cudaMemcpy2DAsync, which is slow on rows this narrow (32 bytes for the cubic extension)
+    coset0_rows_kernel<<<(unsigned)((n * comp->m.W + 255) / 256), 256, 0, ctx->st>>>(comp->m.base, n, comp->m.W, b, clde->m.base);
+    ctx->launches++;
+    const cudaError_t e = cudaGetLastError();
+    int r = e == cudaSuccess ? wf_mat_lde_from_coset(ctx, cpolys, log_b, 1, clde)
+                             : wf_fail(ctx, WF_ERR_CUDA, "composition coset 0 copy: %s", cudaGetErrorString(e));
+    if (r != WF_OK) { wf_mat_free(ctx, clde); return r; }
+    *lde_out = clde;
+    return WF_OK;
+}
 int composition_commit(wf_ctx* ctx, int h, const wf_mat* comp, u32 log_n, u32 log_b, int D, u32 kc, wf_mat** polys_out,
                        wf_mat** lde_out, wf_tree** tree_out, u32 partition_words = 0) {
     wf_mat *cpolys = nullptr, *clde = nullptr;
     CKI(composition_polys(ctx, comp, log_n, D, kc, &cpolys));
-    int r = wf_mat_lde(ctx, cpolys, log_b, &clde);
+    int r = composition_lde(ctx, comp, cpolys, log_n, log_b, kc, &clde);
     if (r == WF_OK) {
         wf_mark(ctx, "composition_lde");
         if (tree_out) r = wf_commit_rows_partitioned(ctx, h, clde, partition_words, tree_out);  // sharded proofs commit their own row range
@@ -1310,7 +1357,10 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     // coefficient order: main transition, aux transition (transition/mod.rs:63-72), main assertions,
     // aux assertions (boundary/mod.rs:108-110)
     std::vector<GlExt<D>> cc = draw_coeffs<D>(ch.coin, o.batch_c, air.num_constraints());
-    CKI(eval_constraints<D>(ctx, air, lde, alde, cc, rnd_flat, log_n, log_b, &comp));
+    // only the rows of the sub-coset the composition polynomial is interpolated from (composition_polys)
+    const size_t m = comp_subcoset_rows(n, kc);
+    const u32 log_step = m < (n << log_ceb) ? log_n + log_ceb - log2_ceil(m) : 0;
+    CKI(eval_constraints<D>(ctx, air, lde, alde, cc, rnd_flat, log_n, log_b, &comp, 0, 0, log_step));
     if (validate) {   // validate_transition_degrees (evaluator/default.rs:114) on the prover's own LDEs
         TraceReport rep;
         CKI(validation_result(ctx, wf_check_degrees(ctx, air, lde, alde, rnd_flat.data(), log_n, log_b, D, rep), rep));
@@ -2336,13 +2386,13 @@ extern "C" int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t a
 //      and the concrete steps between them, for a host that keeps the transcript itself ----------------
 template <int D>
 static int eval_constraints_entry(wf_ctx* ctx, const AirHost& air, u32 log_n, u32 log_b, const wf_mat* lde, const wf_mat* alde,
-                                  const uint64_t* coeffs, const uint64_t* aux_rand, wf_mat** out, size_t row0 = 0, size_t ce_rows = 0) {
+                                  const uint64_t* coeffs, const uint64_t* aux_rand, wf_mat** out, size_t row0, size_t ce_rows, u32 log_step) {
     const size_t ncc = air.degrees.size() + air.aux_degrees.size() + air.asserts.size() + air.aux_asserts.size();
     std::vector<GlExt<D>> cc(ncc);
     for (size_t i = 0; i < ncc; i++) for (int q = 0; q < D; q++) cc[i].v[q] = coeffs[i * D + q];
     std::vector<u64> rnd;
     if (air.aw) rnd.assign(aux_rand, aux_rand + (size_t)air.nr * D);
-    CKI(eval_constraints<D>(ctx, air, lde, alde, cc, rnd, log_n, log_b, out, row0, ce_rows));
+    CKI(eval_constraints<D>(ctx, air, lde, alde, cc, rnd, log_n, log_b, out, row0, ce_rows, log_step));
     if (ctx->validate && !ce_rows) {   // validate_transition_degrees, as evaluator/default.rs:114 runs it after the evaluation
         TraceReport rep;
         const int r = validation_result(ctx, wf_check_degrees(ctx, air, lde, alde, rnd.data(), log_n, log_b, D, rep), rep);
@@ -2364,9 +2414,19 @@ static int check_window(wf_ctx* ctx, u32 log_n, u32 log_b, u32 log_ceb, size_t r
     *lde_rows = (ce_rows << (log_b - log_ceb)) + ((size_t)1 << log_b);
     return WF_OK;
 }
+// The row step of a call over `rows` rows of the CE domain's sub-coset (rows = 0: the whole domain or a window, step 1). Refuses
+// a row count that is not a power of two at most the domain's size.
+static int subcoset_step(wf_ctx* ctx, u32 log_n, u32 log_ceb, size_t rows, u32* log_step) {
+    *log_step = 0;
+    if (!rows) return WF_OK;
+    const u32 lr = log2_ceil(rows);
+    if (rows != ((size_t)1 << lr) || lr > log_n + log_ceb) return wf_fail(ctx, WF_ERR_INVALID, "sub-coset rows must be a power of two at most the CE domain's size");
+    *log_step = log_n + log_ceb - lr;
+    return WF_OK;
+}
 static int eval_constraints_desc(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup, uint32_t ext,
                                  const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs, const uint64_t* aux_rand,
-                                 size_t row0, size_t ce_rows, wf_mat** out) {
+                                 size_t row0, size_t ce_rows, size_t sub_rows, wf_mat** out) {
     if (!ctx || !air_desc || !main_lde || !coeffs || !out || log_n < 3 || blowup < 2 || (blowup & (blowup - 1)))
         return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     AirHost air;
@@ -2374,7 +2434,9 @@ static int eval_constraints_desc(wf_ctx* ctx, const uint64_t* air_desc, size_t a
     const u32 log_b = log2_ceil(blowup);
     if (air.log_ce_blowup() > log_b) return wf_fail(ctx, WF_ERR_INVALID, "blowup factor too small for the constraint degrees");
     size_t N = 0;
+    u32 log_step;
     CKI(check_window(ctx, log_n, log_b, air.log_ce_blowup(), row0, ce_rows, &N));
+    CKI(subcoset_step(ctx, log_n, air.log_ce_blowup(), sub_rows, &log_step));
     if (main_lde->m.rows != N || main_lde->m.cols != air.w) return wf_fail(ctx, WF_ERR_INVALID, "main LDE shape does not match the AIR");
     if (air.aw && (!aux_lde || !aux_rand || aux_lde->m.rows != N || aux_lde->m.cols != air.aw * ext))
         return wf_fail(ctx, WF_ERR_INVALID, "aux LDE / random elements missing or of the wrong shape");
@@ -2384,39 +2446,56 @@ static int eval_constraints_desc(wf_ctx* ctx, const uint64_t* air_desc, size_t a
     CKI(validate_assertions(ctx, air.asserts, (size_t)1 << log_n, 1, "assertion"));
     const wf_mat* al = air.aw ? aux_lde : nullptr;
     switch (ext) {
-        case 1: return eval_constraints_entry<1>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out, row0, ce_rows);
-        case 2: return eval_constraints_entry<2>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out, row0, ce_rows);
-        case 3: return eval_constraints_entry<3>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out, row0, ce_rows);
+        case 1: return eval_constraints_entry<1>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out, row0, ce_rows, log_step);
+        case 2: return eval_constraints_entry<2>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out, row0, ce_rows, log_step);
+        case 3: return eval_constraints_entry<3>(ctx, air, log_n, log_b, main_lde, al, coeffs, aux_rand, out, row0, ce_rows, log_step);
     }
     return wf_fail(ctx, WF_ERR_UNSUPPORTED, "field extension %u", ext);
 }
 extern "C" int wf_eval_constraints(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup,
                                    uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs,
                                    const uint64_t* aux_rand, wf_mat** out) {
-    return eval_constraints_desc(ctx, air_desc, air_desc_len, log_n, blowup, ext, main_lde, aux_lde, coeffs, aux_rand, 0, 0, out);
+    return eval_constraints_desc(ctx, air_desc, air_desc_len, log_n, blowup, ext, main_lde, aux_lde, coeffs, aux_rand, 0, 0, 0, out);
 }
 extern "C" int wf_eval_constraints_window(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup,
                                           uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs,
                                           const uint64_t* aux_rand, size_t row0, size_t ce_rows, wf_mat** out) {
     if (!ce_rows) return wf_fail(ctx, WF_ERR_INVALID, "empty CE row window");
-    return eval_constraints_desc(ctx, air_desc, air_desc_len, log_n, blowup, ext, main_lde, aux_lde, coeffs, aux_rand, row0, ce_rows, out);
+    return eval_constraints_desc(ctx, air_desc, air_desc_len, log_n, blowup, ext, main_lde, aux_lde, coeffs, aux_rand, row0, ce_rows, 0, out);
 }
-extern "C" int wf_eval_constraints_fib(wf_ctx* ctx, uint32_t k, const uint64_t* results, uint32_t log_n, uint32_t blowup, uint32_t ext,
-                                       const wf_mat* lde, const uint64_t* coeffs, size_t row0, size_t ce_rows, wf_mat** out) {
+extern "C" int wf_eval_constraints_subcoset(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup,
+                                            uint32_t ext, const wf_mat* main_lde, const wf_mat* aux_lde, const uint64_t* coeffs,
+                                            const uint64_t* aux_rand, size_t rows, wf_mat** out) {
+    if (!rows) return wf_fail(ctx, WF_ERR_INVALID, "empty sub-coset");
+    return eval_constraints_desc(ctx, air_desc, air_desc_len, log_n, blowup, ext, main_lde, aux_lde, coeffs, aux_rand, 0, 0, rows, out);
+}
+static int eval_constraints_fib(wf_ctx* ctx, uint32_t k, const uint64_t* results, uint32_t log_n, uint32_t blowup, uint32_t ext,
+                                const wf_mat* lde, const uint64_t* coeffs, size_t row0, size_t ce_rows, size_t sub_rows, wf_mat** out) {
     if (!ctx || !results || !lde || !coeffs || !out || k == 0 || 2 * k > 255 || log_n < 3 || blowup < 2 ||
         (blowup & (blowup - 1)) || blowup > 128)
         return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     const u32 log_b = log2_ceil(blowup);
     const AirHost air = fib_air_host(k, (size_t)1 << log_n, results);
     size_t N = 0;
+    u32 log_step;
     CKI(check_window(ctx, log_n, log_b, air.log_ce_blowup(), row0, ce_rows, &N));
+    CKI(subcoset_step(ctx, log_n, air.log_ce_blowup(), sub_rows, &log_step));
     if (lde->m.rows != N || lde->m.cols != 2 * k) return wf_fail(ctx, WF_ERR_INVALID, "LDE shape does not match FibSmall x %u", k);
     switch (ext) {
-        case 1: return eval_constraints_entry<1>(ctx, air, log_n, log_b, lde, nullptr, coeffs, nullptr, out, row0, ce_rows);
-        case 2: return eval_constraints_entry<2>(ctx, air, log_n, log_b, lde, nullptr, coeffs, nullptr, out, row0, ce_rows);
-        case 3: return eval_constraints_entry<3>(ctx, air, log_n, log_b, lde, nullptr, coeffs, nullptr, out, row0, ce_rows);
+        case 1: return eval_constraints_entry<1>(ctx, air, log_n, log_b, lde, nullptr, coeffs, nullptr, out, row0, ce_rows, log_step);
+        case 2: return eval_constraints_entry<2>(ctx, air, log_n, log_b, lde, nullptr, coeffs, nullptr, out, row0, ce_rows, log_step);
+        case 3: return eval_constraints_entry<3>(ctx, air, log_n, log_b, lde, nullptr, coeffs, nullptr, out, row0, ce_rows, log_step);
     }
     return wf_fail(ctx, WF_ERR_INVALID, "field extension %u", ext);
+}
+extern "C" int wf_eval_constraints_fib(wf_ctx* ctx, uint32_t k, const uint64_t* results, uint32_t log_n, uint32_t blowup, uint32_t ext,
+                                       const wf_mat* lde, const uint64_t* coeffs, size_t row0, size_t ce_rows, wf_mat** out) {
+    return eval_constraints_fib(ctx, k, results, log_n, blowup, ext, lde, coeffs, row0, ce_rows, 0, out);
+}
+extern "C" int wf_eval_constraints_fib_subcoset(wf_ctx* ctx, uint32_t k, const uint64_t* results, uint32_t log_n, uint32_t blowup,
+                                                uint32_t ext, const wf_mat* lde, const uint64_t* coeffs, size_t rows, wf_mat** out) {
+    if (!rows) return wf_fail(ctx, WF_ERR_INVALID, "empty sub-coset");
+    return eval_constraints_fib(ctx, k, results, log_n, blowup, ext, lde, coeffs, 0, 0, rows, out);
 }
 
 extern "C" int wf_composition_commit(wf_ctx* ctx, int hash_id, const wf_mat* comp_trace, uint32_t log_n, uint32_t blowup, uint32_t ext,
