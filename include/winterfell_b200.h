@@ -234,25 +234,33 @@ int wf_prove_fib_dev(wf_ctx* ctx, const uint64_t* d_trace, uint32_t k, uint32_t 
 
 /* ---- aux segment built on the device from a description (the described alternative to the aux_builder callback) ----
  * Prover::build_aux_trace (prover/src/lib.rs:236-247) as data: each aux column is a per-row term computed by a straight-line
- * program, then (for the running kinds and linear recurrences) an exclusive prefix scan. The verifier never sees how aux
+ * program, then (for the running kinds and the recurrences) an exclusive prefix scan. The verifier never sees how aux
  * columns were built, so the AIR description and verification are unchanged. aux_build (u64 words):
  *   [aw, nC, constants...,                                         aw = the AIR's aux width; constants canonical
  *    {kind, init0, init1, init2, num_regs, nI, {op, dst, a, b} x nI} x aw]
- *   kind: 0 POINTWISE, 1 RUNNING_PRODUCT, 2 RUNNING_SUM, 4 LINEAR_RECURRENCE (3 is not a kind). init: element of E (words
- *   >= ext must be 0).
+ *   kind: 0 POINTWISE, 1 RUNNING_PRODUCT, 2 RUNNING_SUM, 4 LINEAR_RECURRENCE, 6 RATIONAL_RECURRENCE (3 and 5 are not kinds).
+ *   init: element of E (words >= ext must be 0).
  *   Registers over E, the layout of the aux constraint program: [0,w) main row i, [w,2w) main row (i+1) mod n,
  *   [2w,2w+aw) aux row i, [2w+aw,2w+2aw) aux row (i+1) mod n, nP periodic values col[i mod len], nr random elements,
  *   temporaries; num_regs <= 96. The program of column j reads aux registers of columns < j only, and no temporary before
  *   writing it. Ops as in the constraint programs: 0 ADD, 1 SUB, 2 MUL, 3 CONST (constants of this description), 4 OUT:
  *   OUT 0, r = numerator (exactly once), OUT 1, r = denominator (at most once, default 1), and in LINEAR_RECURRENCE
- *   columns only OUT 2, r = multiplier m_i (exactly once; a polynomial in the registers, never inverted).
+ *   and RATIONAL_RECURRENCE columns only OUT 2, r = multiplier m_i (exactly once; a polynomial in the registers, never
+ *   inverted), in RATIONAL_RECURRENCE columns only OUT 3, r = denominator multiplier c_i (exactly once).
  * For each column j in order, and each row i: t_i = num_i * inv(den_i), inv(0) = 0 (E::inv);
  *   POINTWISE a[i] = t_i;  RUNNING_PRODUCT a[0] = init, a[i+1] = a[i] * t_i;  RUNNING_SUM a[0] = init, a[i+1] = a[i] + t_i;
  *   LINEAR_RECURRENCE a[0] = init, a[i+1] = m_i * a[i] + t_i (i < n - 1): a Horner fingerprint (m = gamma), an accumulator
- *   that restarts where a selector f is 1 (m = 1 - f), the numerator of a fraction sum kept as N / D (m = d_i, t = n_i D[i]).
+ *   that restarts where a selector f is 1 (m = 1 - f), the numerator of a fraction sum kept as N / D (m = d_i, t = n_i D[i]);
+ *   RATIONAL_RECURRENCE a[0] = init, a[i+1] = (m_i * a[i] + n_i) * inv(c_i * a[i] + d_i) (i < n - 1), with n_i = num_i and
+ *   d_i = den_i (not divided first): a Moebius map per row, e.g. continued-fraction convergents (r' = a_i + 1/r: m = a_i, n = 1,
+ *   c = 1, d = 0), Riccati-type recurrences, a fractional fingerprint in one column (a' = (alpha a + v_i) / (a + beta), one
+ *   constraint a' (c a + d) = m a + n). With c = 0 and d = 1 it is LINEAR_RECURRENCE with t = n_i. The device scans the
+ *   maps as 2x2 matrices on projective pairs; where a denominator c_i a[i] + d_i vanishes (a[i+1] = 0) it scans the rows after
+ *   it again, so k such rows cost k further scans of the rest of the column, O(k n): negligible for honest traces with random
+ *   challenges, where a zero is improbable, and at most one host synchronisation per such column when there is none.
  * wf_aux_build_check: the checks of the description against the AIR (structure, width, register ranges and the columns < j
- * rule, one numerator, one multiplier in a LINEAR_RECURRENCE column, kinds, canonical constants and inits), without a
- * device. WF_OK, or WF_ERR_INVALID with the reason. */
+ * rule, one numerator, one multiplier in a LINEAR_RECURRENCE or RATIONAL_RECURRENCE column, one denominator multiplier in a
+ * RATIONAL_RECURRENCE column, kinds, canonical constants and inits), without a device. WF_OK, or WF_ERR_INVALID with the reason. */
 int wf_aux_build_check(const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len, uint32_t log_n,
                        char* msg, size_t msg_cap);
 /* The build as a step: main_evals = the main trace's evaluations (n x width, as from wf_mat_from_host_columns), rand =

@@ -13,6 +13,13 @@
 //                      at each tile start (the composed prefix applied to init). Composition does not commute, so every step
 //                      keeps the rows in order: a thread combines consecutive rows, and the warp and block steps keep the
 //                      earlier operand on the left.
+//   aux_moebius_term_kernel   RATIONAL_RECURRENCE columns: the program's four outputs, the map a -> (m_i a + n_i) / (c_i a + d_i)
+//                      as the matrix (m_i, n_i, c_i, d_i), into [n][4D]; nothing is inverted there.
+//   aux_moebius_reduce / _carry / _apply   the three scan steps over those 2x2 matrices, acting on projective pairs (x, y) ~ x / y:
+//                      a tile's aggregate is the product of its rows' matrices (later rows on the left), the carry is the pair at
+//                      each tile start (the composed prefix applied to (init, 1)), and apply writes a[i] = x_i inv(y_i) with one
+//                      inversion per thread run (Montgomery's trick). Where y_z = 0 first, the serial value is a[z] = 0 (inv(0) = 0)
+//                      and the pairs after z no longer follow it, so the host scans rows z .. again from (0, 1) (aux_moebius).
 // Field arithmetic is exact, so the association order of the scan does not change a bit of the result.
 #include "internal.hpp"
 #include "constraints_generic.cuh"  // ld_ext, seg_at, AUX_MAX_REGS
@@ -34,7 +41,8 @@ struct AuxTermParams {
     const u32* ptab_off;
     const u32* ptab_len;   // powers of two
     const u64* rnd;        // [nr][D]
-    u64* terms;            // [n][D] running kinds, [n][2D] (m_i, t_i) LINEAR_RECURRENCE; nullptr: POINTWISE, written into aux column `col`
+    u64* terms;            // [n][D] running kinds, [n][2D] (m_i, t_i) LINEAR_RECURRENCE, [n][4D] (m_i, n_i, c_i, d_i)
+                           // RATIONAL_RECURRENCE; nullptr: POINTWISE, written into aux column `col`
 };
 
 template <int D>
@@ -44,6 +52,32 @@ __device__ __forceinline__ void st_aux(const SegMatrix& m, size_t row, u32 col, 
         const u32 c = col * D + q;
         m.base[(size_t)(c / m.W) * m.seg_stride + row * m.W + (c % m.W)] = v.v[q];
     }
+}
+
+// the registers a program may read at row i (wf_aux_build_check): main rows, aux columns < col, periodic values, random elements
+template <int D>
+__device__ __forceinline__ void aux_load_regs(const AuxTermParams& p, size_t i, size_t nx, u32 ab, u32 pb, GlExt<D>* ra) {
+    for (u32 c = 0; c < p.w; c++) { ra[c] = ext_from_base<D>(seg_at(p.main, i, c)); ra[p.w + c] = ext_from_base<D>(seg_at(p.main, nx, c)); }
+    for (u32 j = 0; j < p.col; j++) {
+#pragma unroll
+        for (int q = 0; q < D; q++) {
+            ra[ab + j].v[q] = seg_at(p.aux, i, j * D + q);
+            ra[ab + p.aw + j].v[q] = seg_at(p.aux, nx, j * D + q);
+        }
+    }
+    for (u32 j = 0; j < p.np; j++) ra[pb + j] = ext_from_base<D>(p.ptab[p.ptab_off[j] + (u32)(i & (p.ptab_len[j] - 1))]);
+    for (u32 j = 0; j < p.nr; j++) ra[pb + p.np + j] = ld_ext<D>(p.rnd + (size_t)j * D);
+}
+
+template <int D>
+__device__ __forceinline__ GlExt<D> ld_aux(const SegMatrix& m, size_t row, u32 col) {
+    GlExt<D> v;
+#pragma unroll
+    for (int q = 0; q < D; q++) {
+        const u32 c = col * D + q;
+        v.v[q] = m.base[(size_t)(c / m.W) * m.seg_stride + row * m.W + (c % m.W)];
+    }
+    return v;
 }
 
 // AFFINE: a LINEAR_RECURRENCE column, whose program also gives the multiplier m_i (OUT 2)
@@ -60,17 +94,7 @@ __global__ void __launch_bounds__(AUX_TERM_THREADS) aux_term_kernel(AuxTermParam
 #pragma unroll
     for (int r = 0; r < AUX_TERM_ROWS; r++) {
         const size_t i = row0 + r, nx = (i + 1) & (n - 1);
-        // the registers a program may read (wf_aux_build_check): main rows, aux columns < col, periodic values, random elements
-        for (u32 c = 0; c < p.w; c++) { ra[c] = ext_from_base<D>(seg_at(p.main, i, c)); ra[p.w + c] = ext_from_base<D>(seg_at(p.main, nx, c)); }
-        for (u32 j = 0; j < p.col; j++) {
-#pragma unroll
-            for (int q = 0; q < D; q++) {
-                ra[ab + j].v[q] = seg_at(p.aux, i, j * D + q);
-                ra[ab + p.aw + j].v[q] = seg_at(p.aux, nx, j * D + q);
-            }
-        }
-        for (u32 j = 0; j < p.np; j++) ra[pb + j] = ext_from_base<D>(p.ptab[p.ptab_off[j] + (u32)(i & (p.ptab_len[j] - 1))]);
-        for (u32 j = 0; j < p.nr; j++) ra[pb + p.np + j] = ld_ext<D>(p.rnd + (size_t)j * D);
+        aux_load_regs<D>(p, i, nx, ab, pb, ra);
         num[r] = ext_zero<D>();
         den[r] = ext_from_base<D>(1);
         for (u32 k = 0; k < p.prog_len; k++) {
@@ -157,6 +181,59 @@ struct AffOp {   // LINEAR_RECURRENCE: composition of affine maps; a then b = (a
         for (int q = 0; q < D; q++) { p[q] = v.m.v[q]; p[D + q] = v.t.v[q]; }
     }
 };
+template <int D>
+struct Moebius { GlExt<D> m, n, c, d; };   // the matrix [[m, n], [c, d]]: a -> (m a + n) / (c a + d); in memory m, n, c, d, 4D words
+template <int D>
+__device__ __forceinline__ void mob_apply(const Moebius<D>& a, GlExt<D>& x, GlExt<D>& y) {   // (x, y) <- A (x, y)
+    const GlExt<D> x2 = ext_add(ext_mul(a.m, x), ext_mul(a.n, y));
+    y = ext_add(ext_mul(a.c, x), ext_mul(a.d, y));
+    x = x2;
+}
+template <int D>
+struct MobOp {   // RATIONAL_RECURRENCE: composition of Moebius maps as 2x2 matrices up to scale; a then b = B A
+    using T = Moebius<D>;
+    static constexpr int W = 4 * D;
+    static __device__ __forceinline__ T id() { return {ext_from_base<D>(1), ext_zero<D>(), ext_zero<D>(), ext_from_base<D>(1)}; }
+    static __device__ __forceinline__ T op(const T& a, const T& b) {
+        return {ext_add(ext_mul(b.m, a.m), ext_mul(b.n, a.c)), ext_add(ext_mul(b.m, a.n), ext_mul(b.n, a.d)),
+                ext_add(ext_mul(b.c, a.m), ext_mul(b.d, a.c)), ext_add(ext_mul(b.c, a.n), ext_mul(b.d, a.d))};
+    }
+    static __device__ __forceinline__ T shfl_up(const T& v, u32 off) {
+        return {shfl_up_ext(v.m, off), shfl_up_ext(v.n, off), shfl_up_ext(v.c, off), shfl_up_ext(v.d, off)};
+    }
+    static __device__ __forceinline__ T ld(const u64* p) { return {ld_ext<D>(p), ld_ext<D>(p + D), ld_ext<D>(p + 2 * D), ld_ext<D>(p + 3 * D)}; }
+    static __device__ __forceinline__ void st(u64* p, const T& v) {
+#pragma unroll
+        for (int q = 0; q < D; q++) { p[q] = v.m.v[q]; p[D + q] = v.n.v[q]; p[2 * D + q] = v.c.v[q]; p[3 * D + q] = v.d.v[q]; }
+    }
+};
+
+// RATIONAL_RECURRENCE: row i's map (m_i, n_i, c_i, d_i) = (OUT 2, OUT 0, OUT 3, OUT 1) into terms [n][4D]; one row per thread
+template <int D>
+__global__ void __launch_bounds__(AUX_TERM_THREADS) aux_moebius_term_kernel(AuxTermParams p) {
+    const size_t n = (size_t)1 << p.log_n;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    GlExt<D> ra[AUX_MAX_REGS];
+    aux_load_regs<D>(p, i, (i + 1) & (n - 1), 2 * p.w, 2 * p.w + 2 * p.aw, ra);
+    Moebius<D> o = MobOp<D>::id();   // d_i defaults to 1; the program writes the other three exactly once
+    for (u32 k = 0; k < p.prog_len; k++) {
+        const u32 op = p.prog[4 * k], dst = p.prog[4 * k + 1], a = p.prog[4 * k + 2], b = p.prog[4 * k + 3];
+        switch (op) {
+            case 0: ra[dst] = ext_add(ra[a], ra[b]); break;
+            case 1: ra[dst] = ext_sub(ra[a], ra[b]); break;
+            case 2: ra[dst] = ext_mul(ra[a], ra[b]); break;
+            case 3: ra[dst] = ext_from_base<D>(p.consts[a]); break;
+            default:  // OUT 0 numerator n_i, OUT 1 denominator d_i, OUT 2 multiplier m_i, OUT 3 denominator multiplier c_i
+                if (dst == 0) o.n = ra[a];
+                else if (dst == 1) o.d = ra[a];
+                else if (dst == 2) o.m = ra[a];
+                else o.c = ra[a];
+                break;
+        }
+    }
+    MobOp<D>::st(p.terms + i * 4 * D, o);
+}
 
 // exclusive scan of one value per thread over the block (AUX_SCAN_THREADS threads), in thread order; `total` = the whole
 // block's result
@@ -302,6 +379,87 @@ __global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_affine_apply(const u64* 
     }
 }
 
+// The product of the matrices of rows r0 .. r0 + AUX_SCAN_ITEMS - 1 (those < n), later rows on the left; the identity when r0 >= n.
+template <int D>
+__device__ __forceinline__ Moebius<D> moebius_run(const u64* terms, size_t n, size_t r0) {
+    Moebius<D> v = r0 < n ? MobOp<D>::ld(terms + r0 * 4 * D) : MobOp<D>::id();
+#pragma unroll
+    for (int k = 1; k < AUX_SCAN_ITEMS; k++)
+        if (r0 + k < n) v = MobOp<D>::op(v, MobOp<D>::ld(terms + (r0 + k) * 4 * D));
+    return v;
+}
+
+// per tile: the product of its rows' matrices into agg [ntiles][4D]; thread t owns AUX_SCAN_ITEMS consecutive rows
+template <int D>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_moebius_reduce(const u64* terms, size_t n, u64* agg) {
+    const Moebius<D> v = moebius_run<D>(terms, n, (size_t)blockIdx.x * AUX_SCAN_TILE + (size_t)threadIdx.x * AUX_SCAN_ITEMS);
+    Moebius<D> total;
+    block_exclusive_scan<MobOp<D>>(v, total);
+    if (threadIdx.x == 0) MobOp<D>::st(agg + (size_t)blockIdx.x * 4 * D, total);
+}
+
+// one block; tile matrices -> the pair (x, y) at each tile start (the matrices of the tiles before it applied to (init, 1)),
+// written over the first 2D words of the tile's slot. Thread t owns a run of consecutive tiles.
+template <int D>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_moebius_carry(u64* agg, size_t ntiles, GlExt<D> init) {
+    const size_t per = (ntiles + AUX_SCAN_THREADS - 1) / AUX_SCAN_THREADS;
+    const size_t b = threadIdx.x * per, e = b + per < ntiles ? b + per : ntiles;
+    Moebius<D> v = MobOp<D>::id();
+    for (size_t i = b; i < e; i++) v = MobOp<D>::op(v, MobOp<D>::ld(agg + i * 4 * D));
+    Moebius<D> total;
+    GlExt<D> x = init, y = ext_from_base<D>(1);
+    mob_apply(block_exclusive_scan<MobOp<D>>(v, total), x, y);
+    for (size_t i = b; i < e; i++) {
+        const Moebius<D> a = MobOp<D>::ld(agg + i * 4 * D);
+#pragma unroll
+        for (int q = 0; q < D; q++) { agg[i * 4 * D + q] = x.v[q]; agg[i * 4 * D + D + q] = y.v[q]; }
+        mob_apply(a, x, y);
+    }
+}
+
+// rows base + r of aux column `col`, r < n: (x_r, y_r) = the matrices of the tile's rows before r applied to the tile's carry-in,
+// a = x_r inv(y_r), the run's y_r inverted together (Montgomery's trick). A row with y_r = 0 counts as 1 in that batch and lowers
+// *zmin to base + r; it and the rows after it are scanned again. Thread t owns AUX_SCAN_ITEMS consecutive rows.
+template <int D>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_moebius_apply(const u64* terms, size_t n, const u64* carry, SegMatrix out, u32 col,
+                                                                      size_t base, unsigned long long* zmin) {
+    const size_t r0 = (size_t)blockIdx.x * AUX_SCAN_TILE + (size_t)threadIdx.x * AUX_SCAN_ITEMS;
+    const Moebius<D> v = moebius_run<D>(terms, n, r0);
+    Moebius<D> total;
+    const Moebius<D> pre = block_exclusive_scan<MobOp<D>>(v, total);
+    GlExt<D> x = ld_ext<D>(carry + (size_t)blockIdx.x * 4 * D), y = ld_ext<D>(carry + (size_t)blockIdx.x * 4 * D + D);
+    mob_apply(pre, x, y);
+    // forward: w_k = x_k * (y of the run's rows before k), parked in the output; backward: a_k = w_k * (y of the rows after k) /
+    // (product of all y)
+    GlExt<D> ys[AUX_SCAN_ITEMS];
+    GlExt<D> run = ext_from_base<D>(1);
+    unsigned long long z = ~0ull;
+#pragma unroll
+    for (int k = 0; k < AUX_SCAN_ITEMS; k++) {
+        const size_t r = r0 + k;
+        if (r < n) {
+            bool zero = true;
+#pragma unroll
+            for (int q = 0; q < D; q++) zero = zero && y.v[q] == 0;
+            if (zero && z == ~0ull) z = base + r;
+            ys[k] = zero ? ext_from_base<D>(1) : y;
+            st_aux<D>(out, base + r, col, ext_mul(x, run));
+            run = ext_mul(run, ys[k]);
+            mob_apply(MobOp<D>::ld(terms + r * 4 * D), x, y);
+        }
+    }
+    run = ext_inv(run);
+#pragma unroll
+    for (int k = AUX_SCAN_ITEMS - 1; k >= 0; k--) {
+        const size_t r = r0 + k;
+        if (r < n) {
+            st_aux<D>(out, base + r, col, ext_mul(ld_aux<D>(out, base + r, col), run));
+            run = ext_mul(run, ys[k]);
+        }
+    }
+    if (z != ~0ull) atomicMin(zmin, z);
+}
+
 // ---- host ---------------------------------------------------------------------------------------------------------------
 // Parses and checks an aux build description against the AIR's shape (w main columns, aw aux columns, np periodic columns,
 // nr random elements). Returns nullptr, or the reason it is rejected.
@@ -322,7 +480,7 @@ const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, 
     for (u32 j = 0; j < aw; j++) {
         AuxBuildCol c;
         if (!rd(v)) return "malformed aux build description";
-        if (v > 2 && v != 4) return "unknown aux column kind";
+        if (v > 2 && v != 4 && v != 6) return "unknown aux column kind";
         c.kind = (u32)v;
         for (int q = 0; q < 3; q++) {
             if (!rd(c.init[q])) return "malformed aux build description";
@@ -334,16 +492,18 @@ const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, 
         if (!rd(cnt) || cnt > (1u << 20)) return "malformed aux build description";
         std::vector<bool> written(c.num_regs, false);
         for (u32 r = 0; r < first_tmp; r++) written[r] = !(r >= ab && r < pb) || ((r - ab) % aw) < j;
-        const bool affine = c.kind == 4;
-        u32 outs[3] = {0, 0, 0};
+        const bool affine = c.kind == 4, moebius = c.kind == 6;
+        u32 outs[4] = {0, 0, 0, 0};
         for (u64 k = 0; k < cnt; k++) {
             u64 op, ds, x, y;
             if (!rd(op) || !rd(ds) || !rd(x) || !rd(y)) return "malformed aux build description";
             if (op > 4) return "unknown aux build opcode";
             auto readable = [&](u64 r) { return r < c.num_regs && written[r]; };
             if (op == 4) {
+                if (moebius && ds > 3)
+                    return "aux build OUT selects neither numerator (0), denominator (1), multiplier (2) nor denominator multiplier (3)";
                 if (affine && ds > 2) return "aux build OUT selects neither numerator (0), denominator (1) nor multiplier (2)";
-                if (!affine && ds > 1) return "aux build OUT selects neither numerator (0) nor denominator (1)";
+                if (!affine && !moebius && ds > 1) return "aux build OUT selects neither numerator (0) nor denominator (1)";
                 if (!readable(x)) return "aux build program reads a register out of range, an aux column >= its own, or an unwritten temporary";
                 outs[ds]++;
             } else {
@@ -359,6 +519,10 @@ const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, 
         if (outs[1] > 1) return "aux build column has more than one denominator (OUT 1)";
         if (affine && outs[2] == 0) return "aux build LINEAR_RECURRENCE column has no multiplier (OUT 2)";
         if (affine && outs[2] > 1) return "aux build LINEAR_RECURRENCE column has more than one multiplier (OUT 2)";
+        if (moebius && outs[2] == 0) return "aux build RATIONAL_RECURRENCE column has no multiplier (OUT 2)";
+        if (moebius && outs[2] > 1) return "aux build RATIONAL_RECURRENCE column has more than one multiplier (OUT 2)";
+        if (moebius && outs[3] == 0) return "aux build RATIONAL_RECURRENCE column has no denominator multiplier (OUT 3)";
+        if (moebius && outs[3] > 1) return "aux build RATIONAL_RECURRENCE column has more than one denominator multiplier (OUT 3)";
         b.cols.push_back(c);
     }
     if (p != len) return "malformed aux build description";
@@ -392,6 +556,31 @@ static int aux_affine(wf_ctx* ctx, const u64* terms, size_t n, u64* agg, const u
     return WF_OK;
 }
 
+// terms: [n][4D] (m_i, n_i, c_i, d_i); agg: [ntiles][4D]; zmin: one device word. The projective scan equals the serial
+// definition before the first row z with y_z = 0, where the serial value is 0: rows z .. are scanned again from (0, 1) until no
+// zero is left, so k such rows cost k further scans, O(k n). One host synchronisation per scan.
+template <int D>
+static int aux_moebius(wf_ctx* ctx, const u64* terms, size_t n, u64* agg, unsigned long long* zmin, const u64* init, SegMatrix out, u32 col) {
+    GlExt<D> in;
+    for (int q = 0; q < D; q++) in.v[q] = init[q];
+    for (size_t base = 0;;) {
+        const size_t m = n - base, ntiles = (m + AUX_SCAN_TILE - 1) / AUX_SCAN_TILE;
+        const u64* t = terms + base * 4 * D;
+        CK(cudaMemsetAsync(zmin, 0xff, sizeof(*zmin), ctx->st));
+        aux_moebius_reduce<D><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(t, m, agg);
+        aux_moebius_carry<D><<<1, AUX_SCAN_THREADS, 0, ctx->st>>>(agg, ntiles, in);
+        aux_moebius_apply<D><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(t, m, agg, out, col, base, zmin);
+        ctx->launches += 3;
+        CK(cudaGetLastError());
+        unsigned long long z;
+        CK(cudaMemcpyAsync(&z, zmin, sizeof(z), cudaMemcpyDeviceToHost, ctx->st));
+        CK(cudaStreamSynchronize(ctx->st));
+        if (z >= n) return WF_OK;
+        base = (size_t)z;
+        in = ext_zero<D>();
+    }
+}
+
 template <int D>
 static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u32 w, const std::vector<std::vector<u64>>& periodic,
                        const u64* rnd, u32 nr, wf_mat** out) {
@@ -412,16 +601,18 @@ static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u
     if (u32s.size() & 1) u32s.push_back(0);
     const size_t o_u32 = up.size();
     for (size_t i = 0; i < u32s.size(); i += 2) up.push_back((u64)u32s[i] | ((u64)u32s[i + 1] << 32));
-    bool running = false, affine = false;
-    for (auto& c : b.cols) { running = running || c.kind != 0; affine = affine || c.kind == 4; }
-    const size_t tw = affine ? 2 * D : D;   // words per row of the term buffer: (m_i, t_i) when a column needs them
+    bool running = false, affine = false, moebius = false;
+    for (auto& c : b.cols) { running = running || c.kind != 0; affine = affine || c.kind == 4; moebius = moebius || c.kind == 6; }
+    // words per row of the term buffer: (m_i, n_i, c_i, d_i) or (m_i, t_i) when a column needs them
+    const size_t tw = moebius ? 4 * D : affine ? 2 * D : D;
     DevScratch tmp(ctx);
-    void *d_up, *d_terms = nullptr, *d_agg = nullptr;
+    void *d_up, *d_terms = nullptr, *d_agg = nullptr, *d_zmin = nullptr;
     CKI(tmp.alloc(std::max(up.size(), (size_t)1) * 8, &d_up));
     if (running) {
         CKI(tmp.alloc(n * tw * 8, &d_terms));
         CKI(tmp.alloc((n + AUX_SCAN_TILE - 1) / AUX_SCAN_TILE * tw * 8, &d_agg));
     }
+    if (moebius) CKI(tmp.alloc(8, &d_zmin));
     CK(cudaMemcpyAsync(d_up, up.data(), up.size() * 8, cudaMemcpyHostToDevice, ctx->st));
     wf_mat* a;
     CKI(wf_mat_alloc(ctx, n, b.aw * D, &a));
@@ -439,13 +630,15 @@ static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u
         p.prog = dev32 + prog_off[j];
         p.prog_len = (u32)(c.prog.size() / 4);
         p.terms = c.kind ? (u64*)d_terms : nullptr;
-        if (c.kind == 4) aux_term_kernel<D, true><<<grid, AUX_TERM_THREADS, 0, ctx->st>>>(p);
+        if (c.kind == 6) aux_moebius_term_kernel<D><<<(unsigned)((n + AUX_TERM_THREADS - 1) / AUX_TERM_THREADS), AUX_TERM_THREADS, 0, ctx->st>>>(p);
+        else if (c.kind == 4) aux_term_kernel<D, true><<<grid, AUX_TERM_THREADS, 0, ctx->st>>>(p);
         else aux_term_kernel<D, false><<<grid, AUX_TERM_THREADS, 0, ctx->st>>>(p);
         ctx->launches++;
         if (cudaGetLastError() != cudaSuccess) { r = wf_fail(ctx, WF_ERR_CUDA, "aux_term_kernel launch failed"); break; }
         if (c.kind == 1) r = aux_scan<D, true>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
         else if (c.kind == 2) r = aux_scan<D, false>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
         else if (c.kind == 4) r = aux_affine<D>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
+        else if (c.kind == 6) r = aux_moebius<D>(ctx, (const u64*)d_terms, n, (u64*)d_agg, (unsigned long long*)d_zmin, c.init, a->m, j);
     }
     if (r != WF_OK) { wf_mat_free(ctx, a); return r; }
     *out = a;
