@@ -365,7 +365,8 @@ int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len
  * and wf_prove_air_batch run the trace check after the aux segment is built and its assertion values are final (with the
  * transcript's random elements), and the degree check on their own LDEs right after constraint evaluation;
  * wf_eval_constraints runs the degree check. A violation returns WF_ERR_INVALID with the reference's message, writes no proof
- * and leaves no buffer live. Off: these paths are unchanged. wf_prove_fib* and the sharded prover are not checked. */
+ * and leaves no buffer live. Off: these paths are unchanged. wf_prove_air_sharded runs the same checks at the same points,
+ * each rank on its share (see there). wf_prove_fib and wf_prove_fib_sharded are not checked. */
 int wf_ctx_set_validation(wf_ctx* ctx, int on);
 
 /* ---- the same pipeline as separate steps, for a host that owns the transcript (the Rust shim of
@@ -470,8 +471,14 @@ int wf_prove_fib_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* const
  * for the whole trace. Two-segment AIR: aux_build is required (host-callback builders are not supported here); every rank
  * gathers the whole main trace (n * width * 8 bytes of device memory per rank), builds the aux segment on the device with the
  * transcript's random elements and returns the bytes wf_prove_air_aux_built gives; aux_assertions (may be NULL) is called on
- * every rank with the same random elements, as there. stats as wf_prove_fib_sharded. wf_ctx_set_validation's checks are not
- * run. Refusals (WF_ERR_INVALID / WF_ERR_UNSUPPORTED: a world that is not a power of two >= 2, a trace too short for the
+ * every rank with the same random elements, as there. stats as wf_prove_fib_sharded. With wf_ctx_set_validation on, the trace
+ * check runs once the aux segment and its assertion values are final and the degree check right after constraint
+ * evaluation, as in the one-GPU prover, each rank on its share: the main assertions on its own columns, every aux assertion,
+ * transition steps [r n/G, (r+1) n/G) (a single-segment AIR's rows come by one exchange of n * width * 8 / G bytes per rank),
+ * and the degrees of its block of the CE x (n_main + n_aux * ext) transition matrix (its CE rows from its own LDE rows, one
+ * exchange into column blocks). One all_gather_host of the raw results gives every rank the same verdict: a violation returns
+ * WF_ERR_INVALID on every rank with the message the one-GPU prover gives for the same inputs, writes no proof and leaves no
+ * buffer live. Off: this path is unchanged. Refusals (WF_ERR_INVALID / WF_ERR_UNSUPPORTED: a world that is not a power of two >= 2, a trace too short for the
  * world, a description that fails wf_air_check, a bad aux build, a local_count that is not this rank's) happen before any
  * device buffer is allocated, and every rank returns an error: the checks on shared values need no communication, and every
  * rank's verdict on its own block is all-gathered before the first exchange. */

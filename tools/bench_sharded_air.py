@@ -9,7 +9,11 @@ at world > 1 every rank passes its wf_shard_columns block from host memory. Per 
 the max over ranks of each rep), the stage split of one proof on rank 0 (wf_ctx_set_profiling), the communication counters,
 and on rank 0 whether the proof bytes equal the one-GPU proof of the whole trace. The card's name and power limit are read in
 the same run. One JSON object per workload on stdout, appended to --out by rank 0. --backend gloo runs the same sequence with
-host-staged exchanges (several ranks may then share one GPU: a functional rehearsal, not a measurement)."""
+host-staged exchanges (several ranks may then share one GPU: a functional rehearsal, not a measurement).
+--validation: the validation arm instead. Per workload, ms per proof with wf_ctx_set_validation off and on (reps alternated,
+max over ranks, median), whether the proof bytes are the same both ways, and every rank's pooled device bytes after the
+proofs with validation off, then after those with it on (the pool keeps every buffer a proof frees, so that is the rank's
+high-water mark of device memory)."""
 import argparse
 import json
 import os
@@ -62,6 +66,45 @@ def opts(ext):
     return np.array([28, 8, 16, ext, 8, 31, 0, 0, wf.HASH_BLAKE3_256], dtype=np.uint32)
 
 
+def validation_arm(ctx, prove, args, world, barrier):
+    def gather(vals):
+        t = torch.tensor(vals, dtype=torch.float64, device="cuda" if dist.get_backend() == "nccl" else "cpu")
+        out = [torch.empty_like(t) for _ in range(world)]
+        dist.all_gather(out, t)
+        return [[float(x) for x in g] for g in out]
+
+    def timed(on):
+        ctx.set_validation(on)
+        barrier()
+        t0 = time.perf_counter()
+        proof = prove()
+        torch.cuda.synchronize()
+        ctx.set_validation(0)
+        return (time.perf_counter() - t0) * 1e3, proof
+
+    pooled = []
+    for on in (0, 1):   # warm-up; the pool's high-water mark after the proofs without, then with, the checks
+        for _ in range(args.warmup):
+            _, proof = timed(on)
+        pooled.append(ctx.mem_stats()[2])
+    ms = {0: [], 1: []}
+    proofs = {}
+    for _ in range(args.reps):
+        for on in (0, 1):
+            t, proofs[on] = timed(on)
+            ms[on].append(t)
+    per_rank = gather([ms[0][i] for i in range(args.reps)] + [ms[1][i] for i in range(args.reps)] + pooled)
+    R = args.reps
+    off = [max(g[i] for g in per_rank) for i in range(R)]
+    on = [max(g[R + i] for g in per_rank) for i in range(R)]
+    gib = 1 << 30
+    return {"ms_median_off": round(statistics.median(off), 3), "ms_median_on": round(statistics.median(on), 3),
+            "ms_per_rep_off": [round(x, 3) for x in off], "ms_per_rep_on": [round(x, 3) for x in on],
+            "same_proof_bytes": proofs[0] == proofs[1],
+            "pooled_gib_per_rank_off": [round(g[2 * R] / gib, 3) for g in per_rank],
+            "pooled_gib_per_rank_on": [round(g[2 * R + 1] / gib, 3) for g in per_rank]}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--log-n", type=int, default=22)
@@ -70,6 +113,7 @@ def main():
     ap.add_argument("--workloads", default="fib16,perm_rap")
     ap.add_argument("--backend", default="nccl", choices=["nccl", "gloo"])
     ap.add_argument("--out", default=None)
+    ap.add_argument("--validation", action="store_true")
     args = ap.parse_args()
     dist.init_process_group(args.backend)
     rank, world = dist.get_rank(), dist.get_world_size()
@@ -97,6 +141,17 @@ def main():
             torch.cuda.synchronize()
             dist.barrier()
 
+        if args.validation:
+            with torch.cuda.stream(stream):
+                rec = validation_arm(ctx, prove, args, world, barrier)
+            rec.update({"tool": "bench_sharded_air", "arm": "validation", "workload": name, "log_n": args.log_n, "width": int(tr.shape[0]),
+                        "ext": 3, "world": world, "backend": args.backend if world > 1 else None, "card": the_card})
+            if rank == 0:
+                print(json.dumps(rec), flush=True)
+                if args.out:
+                    with open(args.out, "a") as f:
+                        f.write(json.dumps(rec) + "\n")
+            continue
         with torch.cuda.stream(stream):
             for _ in range(args.warmup):
                 proof = prove()

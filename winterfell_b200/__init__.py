@@ -634,7 +634,9 @@ class Context:
 
     def set_validation(self, on):
         """The analogue of a debug build (default off): the proving entry points and eval_constraints check the trace against
-        its AIR and refuse a violation with the reference's panic message."""
+        its AIR and refuse a violation with the reference's panic message. The sharded prover (dist.prove_air_sharded) runs the
+        same checks, each rank on its share, and refuses on every rank with the one-GPU message; prove_fib and
+        dist.prove_fib_sharded are not checked."""
         self.check(self.L.wf_ctx_set_validation(self.h, int(on)))
 
     def prove_fib_dev(self, d_trace, k, log_n, results, opts, out_buf=None):

@@ -393,3 +393,26 @@ int wf_check_trace(wf_ctx* ctx, const AirHost& air, const wf_mat* main, const wf
 // when it is still WF_VALID (the trace check comes first in the reference); always fills expected / actual.
 int wf_check_degrees(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const wf_mat* alde, const u64* rnd, u32 log_n, u32 log_b,
                      int D, TraceReport& rep);
+
+// The two checks split into what a device computes on its share of the work and one host verdict, so that the sharded prover
+// combines every rank's raw results (element-wise minimum for the trace check, the column blocks for the degrees) and gives
+// the one-GPU prover's report and message.
+// Trace check, raw results: [0] / [1] = the smallest (assertion << 40 | cell) over the failing main / aux assertion cells,
+// [2 + j] = the first failing step of transition constraint j (main, then aux); ~0 = none.
+struct TraceCheckPart {
+    SegMatrix amain{};          // main assertions on columns [acol0, acol0 + amain.cols) only: n trace-domain rows of those columns
+    u32 acol0 = 0;
+    const wf_mat* main = nullptr;   // transitions: main (and aux, which is also where the aux assertions are read) trace rows
+    const wf_mat* aux = nullptr;
+    size_t s0 = 0, s1 = 0;      // the steps checked: [s0, s1)
+    size_t row0 = 0, rows = 0;  // rows != 0: main / aux hold trace rows [row0, row0 + rows), then row (row0 + rows) mod n
+};
+int wf_check_trace_part(wf_ctx* ctx, const AirHost& air, const TraceCheckPart& part, const u64* rnd, u32 log_n, int D, std::vector<u64>& raw);
+void wf_trace_verdict(const AirHost& air, bool aux, int D, const std::vector<u64>& raw, TraceReport& rep);
+// Degree check: CE rows [row0, row0 + ce_rows) (ce_rows = 0: all, row0 = 0) of every transition constraint over its divisor into
+// `out` (ce_rows x n_mtr + n_atr*D, zeroed here); lde / alde hold those rows' LDE rows and the blowup halo rows when windowed
+// (GenEvalParams::row0). Then deg1[col] = 1 + the degree of column col of `cols` (interpolated, and freed: cols = nullptr).
+int wf_transition_columns(wf_ctx* ctx, const AirHost& air, const wf_mat* lde, const wf_mat* alde, const u64* rnd, u32 log_n, u32 log_b,
+                          int D, size_t row0, size_t ce_rows, const SegMatrix& out);
+int wf_column_degrees(wf_ctx* ctx, wf_mat*& cols, std::vector<u64>& deg1);
+void wf_degree_verdict(const AirHost& air, bool aux, int D, u32 log_n, const std::vector<u64>& deg1, TraceReport& rep);

@@ -1697,6 +1697,128 @@ static int shard_lde_rows(ShardCtx& sc, const wf_mat* polys, u32 log_b, bool hal
     return WF_OK;
 }
 
+// ---- wf_ctx_set_validation in the sharded prover: the one-GPU prover's two checks (validate.cu), each rank doing its share
+//      of the work. One all_gather_host hands every rank everyone's raw results and every rank reduces them with the same host
+//      code, so all ranks reach the same verdict, return at the same point and stay in step for the next collective ----
+
+// Trace::validate. Rank r checks the main assertions on its own columns, every aux assertion (the aux segment is replicated)
+// and transition steps [r n/G, (r+1) n/G) of [0, n - exemptions). Two-segment AIRs: mtrace / atrace hold the whole trace (the
+// aux build gathered it), own columns included. Single-segment AIRs: rank r evaluates its columns (`polys`) on the trace
+// domain, and one exchange gives every rank its n/G rows of every column plus the next row (n c 8 / G bytes per rank).
+// The raw results combine by their minimum: for the assertions (assertion << 40 | cell), the reference's order.
+template <int D>
+static int sharded_check_trace(ShardCtx& sc, const AirHost& air, const wf_mat* polys, const wf_mat* mtrace, const wf_mat* atrace,
+                               const std::vector<u64>& rnd, u32 log_n, const std::vector<u32>& seg0, const std::vector<u32>& segs) {
+    wf_ctx* ctx = sc.ctx;
+    const int G = sc.G, r = sc.r;
+    const size_t n = (size_t)1 << log_n, nt = n / (size_t)G;
+    const u32 fs = seg0[r], nsl = segs[r];
+    const u32 col0 = std::min(air.w, fs * 8), cl = std::min(air.w, (fs + nsl) * 8) - col0;
+    wf_mat *own = nullptr, *rows = nullptr;
+    struct Free { wf_ctx* c; wf_mat** a; wf_mat** b; ~Free() { wf_mat_free(c, *a); wf_mat_free(c, *b); } } fr{ctx, &own, &rows};
+    TraceCheckPart part;
+    part.acol0 = col0;
+    part.s0 = (size_t)r * nt;
+    part.s1 = std::min((size_t)(r + 1) * nt, n - air.exemptions);
+    if (mtrace) {
+        part.amain = mtrace->m;
+        part.amain.base += (size_t)fs * mtrace->m.seg_stride;
+        part.amain.cols = cl;
+        part.main = mtrace;
+        part.aux = atrace;
+    } else {
+        CKI(wf_mat_alloc_w(ctx, n, cl, 8, &own));
+        if (cl) {
+            wf_mat* ev;
+            CKI(wf_mat_evaluate(ctx, polys, &ev));
+            const cudaError_t e = layout_select_cols(ev->m, 0, own->m, ctx->st);
+            ctx->launches++;
+            wf_mat_free(ctx, ev);
+            CK(e);
+        }
+        part.amain = own->m;
+        CKI(wf_mat_alloc_w(ctx, nt + 1, air.w, 8, &rows));
+        rows->m.rows = nt;   // row nt: the halo row
+        std::vector<int> sp, rp;
+        std::vector<const void*> sv;
+        std::vector<void*> rv;
+        for (int q = 0; q < G; q++) {   // my segments' rows of rank q's range, ascending; from rank q its segments, ascending
+            for (u32 sg = 0; sg < nsl; sg++) {
+                const u64* src = own->m.base + (size_t)sg * own->m.seg_stride + (size_t)q * nt * 8;
+                if (q == r) CK(cudaMemcpyAsync(rows->m.base + (size_t)(fs + sg) * rows->m.seg_stride, src, nt * 64, cudaMemcpyDeviceToDevice, ctx->st));
+                else { sp.push_back(q); sv.push_back(src); }
+            }
+            for (u32 sg = 0; q != r && sg < segs[q]; sg++) { rp.push_back(q); rv.push_back(rows->m.base + (size_t)(seg0[q] + sg) * rows->m.seg_stride); }
+        }
+        CKI(sc.exchange(sp, sv, rp, rv, nt * 64));
+        CKI(exchange_halo(sc, rows->m, 1));
+        part.main = rows;
+        part.row0 = (size_t)r * nt;
+        part.rows = nt;
+    }
+    std::vector<u64> raw;
+    CKI(wf_check_trace_part(ctx, air, part, rnd.data(), log_n, D, raw));
+    std::vector<u64> all(raw.size() * (size_t)G);
+    CKI(sc.gather_host(raw.data(), all.data(), raw.size() * 8));
+    for (int q = 0; q < G; q++)
+        for (size_t j = 0; j < raw.size(); j++) raw[j] = std::min(raw[j], all[(size_t)q * raw.size() + j]);
+    TraceReport rep;
+    wf_trace_verdict(air, atrace != nullptr, D, raw, rep);
+    return validation_result(ctx, WF_OK, rep);
+}
+
+// validate_transition_degrees on the prover's own LDE row shards (`lde`, `alde`: LDE rows [r N/G, (r+1) N/G) and the blowup
+// halo rows). Rank r evaluates every transition constraint over its divisor on CE rows [r ce/G, (r+1) ce/G); one exchange
+// moves that ce/G x ncols matrix into column blocks (rank q: shard_segments(ncols, G, q)'s 8-column segments over all ce
+// rows); every rank interpolates its block and finds its columns' degrees; one all_gather_host of the blocks' degrees (padded
+// to the largest block) gives every rank all of them. An aux constraint's D columns may lie in two blocks: the verdict takes
+// the maximum over its columns either way. With ncols <= 8 rank 0 alone transforms.
+template <int D>
+static int sharded_check_degrees(ShardCtx& sc, const AirHost& air, const wf_mat* lde, const wf_mat* alde, const std::vector<u64>& rnd,
+                                 u32 log_n, u32 log_b) {
+    wf_ctx* ctx = sc.ctx;
+    const int G = sc.G, r = sc.r;
+    const u32 ncols = (u32)air.degrees.size() + (alde ? (u32)air.aux_degrees.size() * D : 0);
+    const size_t ce = (size_t)1 << (log_n + air.log_ce_blowup()), ce_per = ce / (size_t)G;
+    std::vector<u32> cs0(G), cns(G);
+    u32 blk = 0;
+    for (int q = 0; q < G; q++) { shard_segments(ncols, (u32)G, (u32)q, cs0[q], cns[q]); blk = std::max(blk, cns[q] * 8); }
+    u32 first, cnt;
+    shard_columns(ncols, (u32)G, (u32)r, first, cnt);
+    wf_mat *loc = nullptr, *mine = nullptr;
+    struct Free { wf_ctx* c; wf_mat** a; wf_mat** b; ~Free() { wf_mat_free(c, *a); wf_mat_free(c, *b); } } fr{ctx, &loc, &mine};
+    CKI(wf_mat_alloc_w(ctx, ce_per, ncols, 8, &loc));
+    CKI(wf_transition_columns(ctx, air, lde, alde, rnd.data(), log_n, log_b, D, (size_t)r * ce_per, ce_per, loc->m));
+    if (cnt) CKI(wf_mat_alloc_w(ctx, ce, cnt, 8, &mine));
+    {
+        std::vector<int> sp, rp;
+        std::vector<const void*> sv;
+        std::vector<void*> rv;
+        for (int q = 0; q < G; q++) {   // to rank q: its segments ascending; from rank q: my segments ascending
+            for (u32 sg = 0; sg < cns[q]; sg++) {
+                const u64* src = loc->m.base + (size_t)(cs0[q] + sg) * loc->m.seg_stride;
+                if (q == r) CK(cudaMemcpyAsync(mine->m.base + (size_t)sg * mine->m.seg_stride + (size_t)r * ce_per * 8, src, ce_per * 64,
+                                               cudaMemcpyDeviceToDevice, ctx->st));
+                else { sp.push_back(q); sv.push_back(src); }
+            }
+            for (u32 sg = 0; q != r && sg < cns[r]; sg++) { rp.push_back(q); rv.push_back(mine->m.base + (size_t)sg * mine->m.seg_stride + (size_t)q * ce_per * 8); }
+        }
+        CKI(sc.exchange(sp, sv, rp, rv, ce_per * 64));
+    }
+    wf_mat_free(ctx, loc);
+    loc = nullptr;
+    std::vector<u64> d1;
+    if (cnt) CKI(wf_column_degrees(ctx, mine, d1));
+    d1.resize(blk, 0);
+    std::vector<u64> all((size_t)blk * G), deg1(ncols);
+    CKI(sc.gather_host(d1.data(), all.data(), (size_t)blk * 8));
+    for (int q = 0; q < G; q++)
+        for (u32 j = cs0[q] * 8; j < std::min(ncols, (cs0[q] + cns[q]) * 8); j++) deg1[j] = all[(size_t)q * blk + j - cs0[q] * 8];
+    TraceReport rep;
+    wf_degree_verdict(air, alde != nullptr, D, log_n, deg1, rep);
+    return validation_result(ctx, WF_OK, rep);
+}
+
 // One proof of `air_in` sharded over the ranks of `cm` (wf_prove_air_sharded, wf_prove_fib_sharded). Rank r owns the main-trace
 // columns shard_columns() gives it: local_cols / d_local hold exactly those (none: both may be NULL). aux_build: the described
 // build of a two-segment AIR's aux segment (replicated on every rank from the all-gathered main trace).
@@ -1727,6 +1849,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
     const u32 kc = air.num_comp_cols(n), log_ceb = air.log_ce_blowup();
     const size_t ce = n << log_ceb, ce_per = ce / (size_t)G;
     if (rows_per < 64 * b || ce_per < 64) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "trace too short to shard over %d ranks", G);
+    const bool validate = ctx->validate && !air.is_fib;   // wf_ctx_set_validation, as prove_air; wf_prove_fib_sharded is not checked
     Channel ch(h, context_seed(air, n, o));  // every rank replays the whole transcript
 
     wf_mat *polys = nullptr, *lde = nullptr, *shard = nullptr, *mtrace = nullptr, *atrace = nullptr, *apolys = nullptr, *arows = nullptr,
@@ -1870,7 +1993,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
         }
         wf_mark(ctx, "main_trace_gather");
         CKI(wf_aux_build_run(ctx, *aux_build, mtrace, c, air.periodic, rnd_flat.data(), air.nr, D, &atrace));
-        scope.drop(mtrace);
+        if (!validate) scope.drop(mtrace);   // else: the whole main trace the trace check reads
         wf_mark(ctx, "aux_build");
         if (aux_assertions) {
             std::vector<u64> rnd_user = rnd_flat;
@@ -1881,7 +2004,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
                 return wf_fail(ctx, WF_ERR_INVALID, "aux assertion value is not a canonical field element");
         }
         CKI(wf_mat_interpolate(ctx, atrace, &apolys));
-        scope.drop(atrace);
+        if (!validate) scope.drop(atrace);
         CKI(shard_lde_rows(sc, apolys, log_b, true, &arows, aview));
         wf_mark(ctx, "aux_lde");
         CKI(wf_commit_rows_partitioned(ctx, h, &aview, o.part_words(aw, D), &atree.local));
@@ -1890,9 +2013,15 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
         wf_mark(ctx, "aux_commit");
         ch.commit(root.b);
     }
+    if (validate) {   // Trace::validate (lib.rs:355-356): the aux segment and its assertion values are final
+        CKI(sharded_check_trace<D>(sc, air, polys, mtrace, atrace, rnd_flat, log_n, seg0, segs));
+        scope.drop(mtrace);
+        scope.drop(atrace);
+    }
     // ---- 3. constraint evaluation over my CE rows ----
     std::vector<GlExt<D>> cc = draw_coeffs<D>(ch.coin, o.batch_c, air.num_constraints());
     CKI(eval_constraints<D>(ctx, air, shard, aw ? arows : nullptr, cc, rnd_flat, log_n, log_b, &comp_l, (size_t)r * ce_per, ce_per));
+    if (validate) CKI(sharded_check_degrees<D>(sc, air, shard, aw ? arows : nullptr, rnd_flat, log_n, log_b));   // evaluator/default.rs:114
     wf_mark(ctx, "constraint_eval");
     // ---- 4. composition polynomial: all-gather the CE evaluations (a few hundred MiB at most), interpolate on every rank (the
     //         transform is over the row index), extend and commit my row range ----
