@@ -238,7 +238,8 @@ int wf_prove_fib_dev(wf_ctx* ctx, const uint64_t* d_trace, uint32_t k, uint32_t 
  * columns were built, so the AIR description and verification are unchanged. aux_build (u64 words):
  *   [aw, nC, constants...,                                         aw = the AIR's aux width; constants canonical
  *    {kind, init0, init1, init2, num_regs, nI, {op, dst, a, b} x nI} x aw]
- *   kind: 0 POINTWISE, 1 RUNNING_PRODUCT, 2 RUNNING_SUM, 4 LINEAR_RECURRENCE, 6 RATIONAL_RECURRENCE (3 and 5 are not kinds).
+ *   kind: 0 POINTWISE, 1 RUNNING_PRODUCT, 2 RUNNING_SUM, 4 LINEAR_RECURRENCE, 6 RATIONAL_RECURRENCE, 8 COUPLED_RECURRENCE,
+ *   9 COUPLED_MEMBER (3, 5 and 7 are not kinds).
  *   init: element of E (words >= ext must be 0).
  *   Registers over E, the layout of the aux constraint program: [0,w) main row i, [w,2w) main row (i+1) mod n,
  *   [2w,2w+aw) aux row i, [2w+aw,2w+2aw) aux row (i+1) mod n, nP periodic values col[i mod len], nr random elements,
@@ -258,9 +259,23 @@ int wf_prove_fib_dev(wf_ctx* ctx, const uint64_t* d_trace, uint32_t k, uint32_t 
  *   maps as 2x2 matrices on projective pairs; where a denominator c_i a[i] + d_i vanishes (a[i+1] = 0) it scans the rows after
  *   it again, so k such rows cost k further scans of the rest of the column, O(k n): negligible for honest traces with random
  *   challenges, where a zero is improbable, and at most one host synchronisation per such column when there is none.
+ *   COUPLED_RECURRENCE groups: a kind-8 column j and the k - 1 kind-9 entries right after it, each {9, init0, init1, init2,
+ *   0, 0} (no registers, no program), are one group of k = 2..4 columns whose state is a vector: a[i] = (a_0[i], ..,
+ *   a_{k-1}[i]) with a_r the column j + r, a_r[0] = the init of column j + r, and a[i+1] = M_i a[i] + t_i over E (i < n - 1).
+ *   The leader's program gives the whole step: OUT r, reg = t_r (r < k) and OUT 4 + 4r + c, reg = M[r][c] (r, c < k), each
+ *   slot at most once, an unwritten slot 0 (a sparse M needs no zero constants); there is no denominator (a divided term goes
+ *   into an earlier POINTWISE column, which the program reads). The leader reads aux columns < j under the rule above; a column
+ *   after the group reads all of it. E.g. a second-order recurrence u[i+2] = p_i u[i+1] + q_i u[i] + v_i as the pair
+ *   (u[i+1], u[i]) (M = [[p, q], [1, 0]], t = (v, 0)), ordered products of 2x2 to 4x4 matrices of trace values as fingerprints,
+ *   linear state machines or filters driven by the trace and the random elements; state that passes through 0 too. A diagonal
+ *   M gives k LINEAR_RECURRENCE columns; a 2-group with t = 0 and init (a0, 1) is the projective pair (x, y) of the
+ *   RATIONAL_RECURRENCE column of the same matrix (x = y a while no denominator vanishes). The device scans the affine maps
+ *   on E^k: one term launch and three scan launches per group, no host synchronisation.
  * wf_aux_build_check: the checks of the description against the AIR (structure, width, register ranges and the columns < j
  * rule, one numerator, one multiplier in a LINEAR_RECURRENCE or RATIONAL_RECURRENCE column, one denominator multiplier in a
- * RATIONAL_RECURRENCE column, kinds, canonical constants and inits), without a device. WF_OK, or WF_ERR_INVALID with the reason. */
+ * RATIONAL_RECURRENCE column, a group's members right after its leader, 2 <= k <= 4, members without registers or
+ * instructions, a leader's OUT slots inside its group's t and M and none written twice, kinds, canonical constants and
+ * inits), without a device. WF_OK, or WF_ERR_INVALID with the reason. */
 int wf_aux_build_check(const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len, uint32_t log_n,
                        char* msg, size_t msg_cap);
 /* The build as a step: main_evals = the main trace's evaluations (n x width, as from wf_mat_from_host_columns), rand =

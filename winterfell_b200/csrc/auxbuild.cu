@@ -20,6 +20,12 @@
 //                      each tile start (the composed prefix applied to (init, 1)), and apply writes a[i] = x_i inv(y_i) with one
 //                      inversion per thread run (Montgomery's trick). Where y_z = 0 first, the serial value is a[z] = 0 (inv(0) = 0)
 //                      and the pairs after z no longer follow it, so the host scans rows z .. again from (0, 1) (aux_moebius).
+//   aux_coupled_term_kernel   COUPLED_RECURRENCE groups of k columns: the leader's program gives row i's affine map on E^k,
+//                      the augmented matrix [M_i | t_i] row by row into [n][k (k + 1) D]; nothing is inverted there.
+//   aux_coupled_reduce / _carry / _apply   the three scan steps over those maps, one map per group of k lanes (padded to 2 or
+//                      4): a tile's aggregate is the composition of its rows' maps (later rows on the left), the carry is the
+//                      state vector at each tile start (the composed prefix applied to the inits), and apply writes the k
+//                      columns. Nothing is inverted, so no row is ever scanned again.
 // Field arithmetic is exact, so the association order of the scan does not change a bit of the result.
 #include "internal.hpp"
 #include "constraints_generic.cuh"  // ld_ext, seg_at, AUX_MAX_REGS
@@ -42,7 +48,8 @@ struct AuxTermParams {
     const u32* ptab_len;   // powers of two
     const u64* rnd;        // [nr][D]
     u64* terms;            // [n][D] running kinds, [n][2D] (m_i, t_i) LINEAR_RECURRENCE, [n][4D] (m_i, n_i, c_i, d_i)
-                           // RATIONAL_RECURRENCE; nullptr: POINTWISE, written into aux column `col`
+                           // RATIONAL_RECURRENCE, [n][k (k + 1) D] [M_i | t_i] COUPLED_RECURRENCE; nullptr: POINTWISE, written
+                           // into aux column `col`
 };
 
 template <int D>
@@ -460,6 +467,223 @@ __global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_moebius_apply(const u64*
     if (z != ~0ull) atomicMin(zmin, z);
 }
 
+// ---- COUPLED_RECURRENCE groups: a[i+1] = M_i a[i] + t_i over k = 2..4 columns --------------------------------------------
+// A map (M, t) on E^k is k rows of the augmented matrix [M | t], k + 1 elements each; in the term buffer row r of row i's map is
+// at words i S + r (k + 1) D, S = k (k + 1) D. In the scan kernels a map lives on a group of K lanes (k padded to 2 or 4): lane
+// r < k holds row r, the padding lane holds zeros and is never read. Composition takes the other rows from the group by
+// shuffles; applying a map to a state vector (lane r holds a_r) takes k shuffles of one element.
+template <int k>
+__host__ __device__ constexpr int cp_lanes() { return k == 2 ? 2 : 4; }
+template <int k, int D>
+struct CRow { GlExt<D> e[k + 1]; };   // row r of [M | t]: M[r][0 .. k-1], then t_r
+
+// the rows of one scan tile that a lane group owns: AUX_SCAN_TILE rows over AUX_SCAN_THREADS / K groups
+template <int k>
+__host__ __device__ constexpr int cp_items() { return AUX_SCAN_TILE / (AUX_SCAN_THREADS / cp_lanes<k>()); }
+
+template <int D>
+__device__ __forceinline__ GlExt<D> shfl_grp(u32 mask, const GlExt<D>& v, int src, int width) {
+    GlExt<D> r;
+#pragma unroll
+    for (int q = 0; q < D; q++) r.v[q] = __shfl_sync(mask, v.v[q], src, width);
+    return r;
+}
+template <int k, int D>
+__device__ __forceinline__ CRow<k, D> crow_id(u32 r) {
+    CRow<k, D> v;
+#pragma unroll
+    for (int c = 0; c <= k; c++) v.e[c] = (u32)c == r ? ext_from_base<D>(1) : ext_zero<D>();
+    return v;
+}
+template <int k, int D>
+__device__ __forceinline__ CRow<k, D> crow_ld(const u64* p, u32 r) {   // p: one map (S words); zeros on the padding lane
+    CRow<k, D> v;
+#pragma unroll
+    for (int c = 0; c <= k; c++) v.e[c] = r < (u32)k ? ld_ext<D>(p + (r * (k + 1) + c) * D) : ext_zero<D>();
+    return v;
+}
+template <int k, int D>
+__device__ __forceinline__ void crow_st(u64* p, u32 r, const CRow<k, D>& v) {
+    if (r >= (u32)k) return;
+#pragma unroll
+    for (int c = 0; c <= k; c++)
+#pragma unroll
+        for (int q = 0; q < D; q++) p[(r * (k + 1) + c) * D + q] = v.e[c].v[q];
+}
+// "a then b" = B o A, row r: M'[r][c] = sum_s B[r][s] A[s][c], t'_r = sum_s B[r][s] A_t[s] + B_t[r]; lane r holds row r of a and
+// b, the rows of a come from its group (gmask, width K)
+template <int k, int D>
+__device__ __forceinline__ CRow<k, D> crow_op(u32 gmask, const CRow<k, D>& a, const CRow<k, D>& b) {
+    CRow<k, D> o;
+#pragma unroll
+    for (int c = 0; c < k; c++) o.e[c] = ext_zero<D>();
+    o.e[k] = b.e[k];
+#pragma unroll
+    for (int s = 0; s < k; s++)
+#pragma unroll
+        for (int c = 0; c <= k; c++) o.e[c] = ext_add(o.e[c], ext_mul(b.e[s], shfl_grp(gmask, a.e[c], s, cp_lanes<k>())));
+    return o;
+}
+// the state vector after the map: lane r gets sum_s M[r][s] x_s + t_r
+template <int k, int D>
+__device__ __forceinline__ GlExt<D> crow_apply(u32 gmask, const CRow<k, D>& m, const GlExt<D>& x) {
+    GlExt<D> y = m.e[k];
+#pragma unroll
+    for (int s = 0; s < k; s++) y = ext_add(y, ext_mul(m.e[s], shfl_grp(gmask, x, s, cp_lanes<k>())));
+    return y;
+}
+template <int k, int D>
+__device__ __forceinline__ CRow<k, D> crow_shfl_up(const CRow<k, D>& v, u32 off) {
+    CRow<k, D> r;
+#pragma unroll
+    for (int c = 0; c <= k; c++) r.e[c] = shfl_up_ext(v.e[c], off);
+    return r;
+}
+__device__ __forceinline__ u32 cp_gmask(u32 K) { return ((1u << K) - 1) << ((threadIdx.x & 31) & ~(K - 1)); }
+
+// exclusive scan of one map per lane group over the block, in group order; `total` = the whole block's composition
+template <int k, int D>
+__device__ __forceinline__ CRow<k, D> coupled_block_exclusive_scan(const CRow<k, D>& v, CRow<k, D>& total) {
+    constexpr u32 K = cp_lanes<k>(), G = 32 / K, NW = AUX_SCAN_THREADS / 32;
+    __shared__ u64 wsum[NW][K][(k + 1) * D];
+    const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5, r = lane & (K - 1), g = lane / K, gm = cp_gmask(K);
+    auto ld = [&](u32 w) { CRow<k, D> x; for (int c = 0; c <= k; c++) x.e[c] = ld_ext<D>(&wsum[w][r][c * D]); return x; };
+    auto st = [&](u32 w, const CRow<k, D>& x) {
+        for (int c = 0; c <= k; c++)
+            for (int q = 0; q < D; q++) wsum[w][r][c * D + q] = x.e[c].v[q];
+    };
+    CRow<k, D> x = v;
+#pragma unroll
+    for (u32 off = 1; off < G; off <<= 1) {
+        const CRow<k, D> y = crow_op(gm, crow_shfl_up(x, off * K), x);
+        if (g >= off) x = y;
+    }
+    if (g == G - 1) st(wid, x);
+    __syncthreads();
+    if (wid == 0) {
+        CRow<k, D> s = g < NW ? ld(g) : crow_id<k, D>(r);
+#pragma unroll
+        for (u32 off = 1; off < NW; off <<= 1) {
+            const CRow<k, D> y = crow_op(gm, crow_shfl_up(s, off * K), s);
+            if (g >= off) s = y;
+        }
+        if (g < NW) st(g, s);
+    }
+    __syncthreads();
+    total = ld(NW - 1);
+    const CRow<k, D> wpre = wid ? ld(wid - 1) : crow_id<k, D>(r);
+    CRow<k, D> ex = crow_shfl_up(x, K);
+    if (g == 0) ex = crow_id<k, D>(r);
+    __syncthreads();  // wsum is free for the next call
+    return crow_op(gm, wpre, ex);
+}
+
+// COUPLED_RECURRENCE: row i's map from the leader's program into terms [n][S]: OUT r = t_r, OUT 4 + 4r + c = M[r][c]; the slots
+// the program never writes (bit set in `unwritten`, slot r (k + 1) + c) are 0. One row per thread.
+template <int D>
+__global__ void __launch_bounds__(AUX_TERM_THREADS) aux_coupled_term_kernel(AuxTermParams p, u32 k, u32 unwritten) {
+    const size_t n = (size_t)1 << p.log_n;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    GlExt<D> ra[AUX_MAX_REGS];
+    aux_load_regs<D>(p, i, (i + 1) & (n - 1), 2 * p.w, 2 * p.w + 2 * p.aw, ra);
+    u64* t = p.terms + i * k * (k + 1) * D;
+    for (u32 s = 0; s < k * (k + 1); s++)
+        if (unwritten >> s & 1)
+#pragma unroll
+            for (int q = 0; q < D; q++) t[s * D + q] = 0;
+    for (u32 j = 0; j < p.prog_len; j++) {
+        const u32 op = p.prog[4 * j], dst = p.prog[4 * j + 1], a = p.prog[4 * j + 2], b = p.prog[4 * j + 3];
+        switch (op) {
+            case 0: ra[dst] = ext_add(ra[a], ra[b]); break;
+            case 1: ra[dst] = ext_sub(ra[a], ra[b]); break;
+            case 2: ra[dst] = ext_mul(ra[a], ra[b]); break;
+            case 3: ra[dst] = ext_from_base<D>(p.consts[a]); break;
+            default: {
+                const u32 s = dst < 4 ? dst * (k + 1) + k : (dst - 4) / 4 * (k + 1) + (dst - 4) % 4;
+#pragma unroll
+                for (int q = 0; q < D; q++) t[s * D + q] = ra[a].v[q];
+                break;
+            }
+        }
+    }
+}
+
+// The composition of the maps of rows r0 .. r0 + cp_items - 1 (those < n), in row order; the identity when r0 >= n.
+template <int k, int D>
+__device__ __forceinline__ CRow<k, D> coupled_run(const u64* terms, size_t n, size_t r0, u32 r, u32 gm) {
+    constexpr size_t S = k * (k + 1) * D;
+    CRow<k, D> v = r0 < n ? crow_ld<k, D>(terms + r0 * S, r) : crow_id<k, D>(r);
+#pragma unroll 1
+    for (int j = 1; j < cp_items<k>(); j++)
+        if (r0 + j < n) v = crow_op(gm, v, crow_ld<k, D>(terms + (r0 + j) * S, r));
+    return v;
+}
+
+// per tile: the composition of its rows' maps into agg [ntiles][S]
+template <int k, int D>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_coupled_reduce(const u64* terms, size_t n, u64* agg) {
+    constexpr u32 K = cp_lanes<k>();
+    const u32 r = threadIdx.x & (K - 1);
+    const CRow<k, D> v = coupled_run<k, D>(terms, n, (size_t)blockIdx.x * AUX_SCAN_TILE + (size_t)(threadIdx.x / K) * cp_items<k>(), r,
+                                           cp_gmask(K));
+    CRow<k, D> total;
+    coupled_block_exclusive_scan<k, D>(v, total);
+    if (threadIdx.x < K) crow_st<k, D>(agg + (size_t)blockIdx.x * k * (k + 1) * D, r, total);
+}
+
+template <int k, int D>
+struct CVec { GlExt<D> a[k]; };   // a state vector of the group: a_r = the value of column j + r
+
+// one block; tile maps -> the state vector at each tile start (the maps of the tiles before it applied to init); a_r is written
+// over the first D words of row r of the tile's slot. Each lane group owns a run of consecutive tiles.
+template <int k, int D>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_coupled_carry(u64* agg, size_t ntiles, CVec<k, D> init) {
+    constexpr u32 K = cp_lanes<k>();
+    constexpr size_t S = k * (k + 1) * D;
+    const u32 r = threadIdx.x & (K - 1), gm = cp_gmask(K);
+    const size_t per = (ntiles + AUX_SCAN_THREADS / K - 1) / (AUX_SCAN_THREADS / K);
+    const size_t b = (threadIdx.x / K) * per, e = b + per < ntiles ? b + per : ntiles;
+    CRow<k, D> v = crow_id<k, D>(r);
+#pragma unroll 1
+    for (size_t i = b; i < e; i++) v = crow_op(gm, v, crow_ld<k, D>(agg + i * S, r));
+    GlExt<D> x = ext_zero<D>();
+#pragma unroll
+    for (int s = 0; s < k; s++) if ((u32)s == r) x = init.a[s];
+    CRow<k, D> total;
+    x = crow_apply(gm, coupled_block_exclusive_scan<k, D>(v, total), x);
+#pragma unroll 1
+    for (size_t i = b; i < e; i++) {
+        const CRow<k, D> a = crow_ld<k, D>(agg + i * S, r);
+        if (r < (u32)k)
+#pragma unroll
+            for (int q = 0; q < D; q++) agg[i * S + r * (k + 1) * D + q] = x.v[q];
+        x = crow_apply(gm, a, x);
+    }
+}
+
+// a[i] = the maps of the tile's rows before i applied to the tile's carry-in; lane r writes aux column col + r
+template <int k, int D>
+__global__ void __launch_bounds__(AUX_SCAN_THREADS) aux_coupled_apply(const u64* terms, size_t n, const u64* carry, SegMatrix out, u32 col) {
+    constexpr u32 K = cp_lanes<k>();
+    constexpr size_t S = k * (k + 1) * D;
+    const u32 r = threadIdx.x & (K - 1), gm = cp_gmask(K);
+    const size_t r0 = (size_t)blockIdx.x * AUX_SCAN_TILE + (size_t)(threadIdx.x / K) * cp_items<k>();
+    const CRow<k, D> v = coupled_run<k, D>(terms, n, r0, r, gm);
+    CRow<k, D> total;
+    const CRow<k, D> pre = coupled_block_exclusive_scan<k, D>(v, total);
+    GlExt<D> x = r < (u32)k ? ld_ext<D>(carry + (size_t)blockIdx.x * S + r * (k + 1) * D) : ext_zero<D>();
+    x = crow_apply(gm, pre, x);
+#pragma unroll 1
+    for (int j = 0; j < cp_items<k>(); j++) {
+        const size_t i = r0 + j;
+        if (i < n) {
+            if (r < (u32)k) st_aux<D>(out, i, col + r, x);
+            x = crow_apply(gm, crow_ld<k, D>(terms + i * S, r), x);
+        }
+    }
+}
+
 // ---- host ---------------------------------------------------------------------------------------------------------------
 // Parses and checks an aux build description against the AIR's shape (w main columns, aw aux columns, np periodic columns,
 // nr random elements). Returns nullptr, or the reason it is rejected.
@@ -477,35 +701,63 @@ const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, 
         b.consts.push_back(v);
     }
     const u32 ab = 2 * w, pb = 2 * w + 2 * aw, first_tmp = pb + np + nr;
+    // the open COUPLED_RECURRENCE group: its leader's index and the OUT slots its program writes (bit = OUT index); the group
+    // size k, and with it the slots allowed, is known when the next column is not a member
+    u32 lead = ~0u, lead_slots = 0;
+    auto close_group = [&]() -> const char* {
+        if (lead == ~0u) return nullptr;
+        const u32 k = (u32)b.cols.size() - lead;
+        lead = ~0u;
+        if (k < 2 || k > 4) return "aux build COUPLED_RECURRENCE group has fewer than 2 or more than 4 columns";
+        for (u32 s = 0; s < 20; s++)
+            if ((lead_slots >> s & 1) && (s < 4 ? s >= k : (s - 4) / 4 >= k || (s - 4) % 4 >= k))
+                return "aux build COUPLED_RECURRENCE OUT selects a slot outside the group's t (0 .. k-1) and M (4 + 4r + c, r, c < k)";
+        return nullptr;
+    };
     for (u32 j = 0; j < aw; j++) {
         AuxBuildCol c;
         if (!rd(v)) return "malformed aux build description";
-        if (v > 2 && v != 4 && v != 6) return "unknown aux column kind";
+        if (v > 2 && v != 4 && v != 6 && v != 8 && v != 9) return "unknown aux column kind";
         c.kind = (u32)v;
+        if (c.kind != 9) {
+            if (const char* why = close_group()) return why;
+        } else if (lead == ~0u) {
+            return "aux build COUPLED_MEMBER column does not follow a COUPLED_RECURRENCE column or another member";
+        }
         for (int q = 0; q < 3; q++) {
             if (!rd(c.init[q])) return "malformed aux build description";
             if (c.init[q] >= GL_P) return "aux column init is not a canonical field element";
         }
         if (!rd(v)) return "malformed aux build description";
+        if (c.kind == 9) {   // {9, init, 0, 0}: the leader's program gives the whole group's step
+            if (!rd(cnt)) return "malformed aux build description";
+            if (v != 0 || cnt != 0) return "aux build COUPLED_MEMBER column has registers or instructions";
+            b.cols.push_back(c);
+            continue;
+        }
         if (v > AUX_MAX_REGS || v < first_tmp) return "aux build register count out of range";
         c.num_regs = (u32)v;
         if (!rd(cnt) || cnt > (1u << 20)) return "malformed aux build description";
         std::vector<bool> written(c.num_regs, false);
         for (u32 r = 0; r < first_tmp; r++) written[r] = !(r >= ab && r < pb) || ((r - ab) % aw) < j;
-        const bool affine = c.kind == 4, moebius = c.kind == 6;
-        u32 outs[4] = {0, 0, 0, 0};
+        const bool affine = c.kind == 4, moebius = c.kind == 6, coupled = c.kind == 8;
+        u32 outs[4] = {0, 0, 0, 0}, slots = 0;
         for (u64 k = 0; k < cnt; k++) {
             u64 op, ds, x, y;
             if (!rd(op) || !rd(ds) || !rd(x) || !rd(y)) return "malformed aux build description";
             if (op > 4) return "unknown aux build opcode";
             auto readable = [&](u64 r) { return r < c.num_regs && written[r]; };
             if (op == 4) {
+                if (coupled && ds > 19)
+                    return "aux build COUPLED_RECURRENCE OUT selects a slot outside the group's t (0 .. k-1) and M (4 + 4r + c, r, c < k)";
+                if (coupled && (slots >> ds & 1)) return "aux build COUPLED_RECURRENCE program writes an OUT slot more than once";
                 if (moebius && ds > 3)
                     return "aux build OUT selects neither numerator (0), denominator (1), multiplier (2) nor denominator multiplier (3)";
                 if (affine && ds > 2) return "aux build OUT selects neither numerator (0), denominator (1) nor multiplier (2)";
-                if (!affine && !moebius && ds > 1) return "aux build OUT selects neither numerator (0) nor denominator (1)";
+                if (!affine && !moebius && !coupled && ds > 1) return "aux build OUT selects neither numerator (0) nor denominator (1)";
                 if (!readable(x)) return "aux build program reads a register out of range, an aux column >= its own, or an unwritten temporary";
-                outs[ds]++;
+                if (coupled) slots |= 1u << ds;
+                else outs[ds]++;
             } else {
                 if (ds >= c.num_regs || ds < first_tmp) return "aux build program writes a register outside its temporaries";
                 if (op == 3) { if (x >= b.consts.size()) return "aux build constant index out of range"; }
@@ -515,7 +767,8 @@ const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, 
             }
             c.prog.insert(c.prog.end(), {(u32)op, (u32)ds, (u32)x, (u32)y});
         }
-        if (outs[0] != 1) return "aux build column needs exactly one numerator (OUT 0)";
+        if (coupled) { lead = j; lead_slots = slots; }
+        if (!coupled && outs[0] != 1) return "aux build column needs exactly one numerator (OUT 0)";
         if (outs[1] > 1) return "aux build column has more than one denominator (OUT 1)";
         if (affine && outs[2] == 0) return "aux build LINEAR_RECURRENCE column has no multiplier (OUT 2)";
         if (affine && outs[2] > 1) return "aux build LINEAR_RECURRENCE column has more than one multiplier (OUT 2)";
@@ -525,6 +778,7 @@ const char* wf_aux_build_parse(const u64* d, size_t len, u32 w, u32 aw, u32 np, 
         if (moebius && outs[3] > 1) return "aux build RATIONAL_RECURRENCE column has more than one denominator multiplier (OUT 3)";
         b.cols.push_back(c);
     }
+    if (const char* why = close_group()) return why;
     if (p != len) return "malformed aux build description";
     return nullptr;
 }
@@ -581,6 +835,28 @@ static int aux_moebius(wf_ctx* ctx, const u64* terms, size_t n, u64* agg, unsign
     }
 }
 
+// the group of columns col .. col + k - 1; terms: [n][S] (M_i, t_i) row by row, S = k (k + 1) D; agg: [ntiles][S]
+template <int k, int D>
+static int aux_coupled(wf_ctx* ctx, const u64* terms, size_t n, u64* agg, const AuxBuildCol* cols, SegMatrix out, u32 col) {
+    const size_t ntiles = (n + AUX_SCAN_TILE - 1) / AUX_SCAN_TILE;
+    CVec<k, D> in;
+    for (int r = 0; r < k; r++)
+        for (int q = 0; q < D; q++) in.a[r].v[q] = cols[r].init[q];
+    aux_coupled_reduce<k, D><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(terms, n, agg);
+    aux_coupled_carry<k, D><<<1, AUX_SCAN_THREADS, 0, ctx->st>>>(agg, ntiles, in);
+    aux_coupled_apply<k, D><<<(unsigned)ntiles, AUX_SCAN_THREADS, 0, ctx->st>>>(terms, n, agg, out, col);
+    ctx->launches += 3;
+    CK(cudaGetLastError());
+    return WF_OK;
+}
+
+// the size of the COUPLED_RECURRENCE group led by column j: 1 + the COUPLED_MEMBER columns after it
+static u32 coupled_size(const AuxBuildHost& b, u32 j) {
+    u32 k = 1;
+    while (j + k < b.cols.size() && b.cols[j + k].kind == 9) k++;
+    return k;
+}
+
 template <int D>
 static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u32 w, const std::vector<std::vector<u64>>& periodic,
                        const u64* rnd, u32 nr, wf_mat** out) {
@@ -602,9 +878,15 @@ static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u
     const size_t o_u32 = up.size();
     for (size_t i = 0; i < u32s.size(); i += 2) up.push_back((u64)u32s[i] | ((u64)u32s[i + 1] << 32));
     bool running = false, affine = false, moebius = false;
-    for (auto& c : b.cols) { running = running || c.kind != 0; affine = affine || c.kind == 4; moebius = moebius || c.kind == 6; }
-    // words per row of the term buffer: (m_i, n_i, c_i, d_i) or (m_i, t_i) when a column needs them
-    const size_t tw = moebius ? 4 * D : affine ? 2 * D : D;
+    u32 kmax = 0;
+    for (u32 j = 0; j < b.aw; j++) {
+        const u32 kind = b.cols[j].kind;
+        running = running || kind != 0; affine = affine || kind == 4; moebius = moebius || kind == 6;
+        if (kind == 8) kmax = std::max(kmax, coupled_size(b, j));
+    }
+    // words per row of the term buffer: (m_i, n_i, c_i, d_i) or (m_i, t_i) when a column needs them, the largest group's
+    // (M_i, t_i) when there is a group
+    const size_t tw = std::max((size_t)kmax * (kmax + 1) * D, (size_t)(moebius ? 4 * D : affine ? 2 * D : D));
     DevScratch tmp(ctx);
     void *d_up, *d_terms = nullptr, *d_agg = nullptr, *d_zmin = nullptr;
     CKI(tmp.alloc(std::max(up.size(), (size_t)1) * 8, &d_up));
@@ -626,11 +908,22 @@ static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u
     int r = WF_OK;
     for (u32 j = 0; j < b.aw && r == WF_OK; j++) {
         const AuxBuildCol& c = b.cols[j];
+        if (c.kind == 9) continue;   // built with its group's leader
         p.col = j;
         p.prog = dev32 + prog_off[j];
         p.prog_len = (u32)(c.prog.size() / 4);
         p.terms = c.kind ? (u64*)d_terms : nullptr;
-        if (c.kind == 6) aux_moebius_term_kernel<D><<<(unsigned)((n + AUX_TERM_THREADS - 1) / AUX_TERM_THREADS), AUX_TERM_THREADS, 0, ctx->st>>>(p);
+        const u32 k = c.kind == 8 ? coupled_size(b, j) : 0;
+        if (c.kind == 8) {
+            u32 written = 0;
+            for (size_t q = 0; q < c.prog.size(); q += 4)
+                if (c.prog[q] == 4) {
+                    const u32 ds = c.prog[q + 1];
+                    written |= 1u << (ds < 4 ? ds * (k + 1) + k : (ds - 4) / 4 * (k + 1) + (ds - 4) % 4);
+                }
+            aux_coupled_term_kernel<D><<<(unsigned)((n + AUX_TERM_THREADS - 1) / AUX_TERM_THREADS), AUX_TERM_THREADS, 0, ctx->st>>>(
+                p, k, ((1u << k * (k + 1)) - 1) & ~written);
+        } else if (c.kind == 6) aux_moebius_term_kernel<D><<<(unsigned)((n + AUX_TERM_THREADS - 1) / AUX_TERM_THREADS), AUX_TERM_THREADS, 0, ctx->st>>>(p);
         else if (c.kind == 4) aux_term_kernel<D, true><<<grid, AUX_TERM_THREADS, 0, ctx->st>>>(p);
         else aux_term_kernel<D, false><<<grid, AUX_TERM_THREADS, 0, ctx->st>>>(p);
         ctx->launches++;
@@ -639,6 +932,13 @@ static int aux_build_d(wf_ctx* ctx, const AuxBuildHost& b, const wf_mat* main, u
         else if (c.kind == 2) r = aux_scan<D, false>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
         else if (c.kind == 4) r = aux_affine<D>(ctx, (const u64*)d_terms, n, (u64*)d_agg, c.init, a->m, j);
         else if (c.kind == 6) r = aux_moebius<D>(ctx, (const u64*)d_terms, n, (u64*)d_agg, (unsigned long long*)d_zmin, c.init, a->m, j);
+        else if (c.kind == 8) {
+            const u64* t = (const u64*)d_terms;
+            u64* g = (u64*)d_agg;
+            r = k == 2 ? aux_coupled<2, D>(ctx, t, n, g, &c, a->m, j)
+              : k == 3 ? aux_coupled<3, D>(ctx, t, n, g, &c, a->m, j)
+                       : aux_coupled<4, D>(ctx, t, n, g, &c, a->m, j);
+        }
     }
     if (r != WF_OK) { wf_mat_free(ctx, a); return r; }
     *out = a;

@@ -120,7 +120,8 @@ int wf_dev_alloc(wf_ctx* ctx, size_t bytes, void** out);
 void wf_dev_free(wf_ctx* ctx, void* p);
 // auxbuild.cu: the aux segment built on the device from a column-program description (format at wf_aux_build in the header)
 struct AuxBuildCol {
-    u32 kind = 0;          // 0 POINTWISE, 1 RUNNING_PRODUCT, 2 RUNNING_SUM, 4 LINEAR_RECURRENCE, 6 RATIONAL_RECURRENCE
+    u32 kind = 0;          // 0 POINTWISE, 1 RUNNING_PRODUCT, 2 RUNNING_SUM, 4 LINEAR_RECURRENCE, 6 RATIONAL_RECURRENCE,
+                           // 8 COUPLED_RECURRENCE (a group's leader), 9 COUPLED_MEMBER (built with its leader)
     u64 init[3] = {0, 0, 0};
     u32 num_regs = 0;
     std::vector<u32> prog; // 4 words per instruction
