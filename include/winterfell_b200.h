@@ -501,6 +501,38 @@ int wf_prove_air_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* air_d
                          size_t aux_build_len, wf_aux_assertions_fn aux_assertions, void* aux_user, const uint64_t* const* local_cols,
                          const uint64_t* d_local, uint32_t local_count, int mont, uint32_t log_n, const uint32_t* opts, uint8_t* proof,
                          size_t* proof_len, double* stats);
+/* wf_trace_validate over comm->world GPUs, without a proof: the checks wf_prove_air_sharded runs with validation on, with the
+ * report wf_trace_validate gives. Every rank passes the same description, log_n, ext, check_degrees and random elements
+ * (rand: [nr][ext] canonical), plus its own block of main-trace columns as wf_prove_air_sharded takes it: local_count =
+ * wf_shard_columns(width, world, rank)'s count, host columns (local_cols, representation by `mont`) or device memory (d_local,
+ * column-major [local_count][2^log_n], canonical); a rank that owns no column passes local_count = 0 and may pass NULL for
+ * both. A two-segment AIR takes exactly one of aux_build (built on the device on every rank from the gathered main trace, as
+ * the sharded prover builds it) and aux_cols (the whole aux segment, [aw] host columns of [2^log_n][ext] words, representation
+ * by `mont`, the same on every rank). On every rank the return value, report, first_failing_step, expected_degrees,
+ * actual_degrees and msg are exactly what wf_trace_validate returns for the whole trace with the same arguments: WF_OK when the
+ * checks ran, a violation being a result; the degree check runs even when the trace check failed.
+ * Work per rank r: the main assertions on its own columns, every aux assertion, transition steps [r n/G, (r+1) n/G); the
+ * degree check on CE rows [r ce/G, (r+1) ce/G) from LDE row shards at the CE blowup (its columns extended locally and turned
+ * into row shards with ce_blowup halo rows; the aux segment extended on every rank and sharded as the prover's), then the
+ * degrees of its 8-column block of the CE x (n_main + n_aux * ext) transition matrix.
+ * Device memory per rank, with c main columns of which cl are its own and k = n_main + n_aux * ext:
+ *   trace check: n * cl * 8 * 2 (its columns' coefficients and evaluations) and (n/G + 1) * c * 8 (its rows: one exchange of
+ *     n * c * 8 / G bytes) -- except with aux_build, which gathers the whole main trace, n * c * 8, as the sharded prover does;
+ *     the aux segment n * aw * ext * 8 is held whole (it is replicated, not sharded);
+ *   degree check: n * ce_blowup * cl * 8 (its columns' LDE) and 2 * (ce/G + ce_blowup) * c * 8 (staging and row shard), then
+ *     (ce/G) * k * 8 (its CE rows) and, twice, ce * 8 * (8 x its share of the k/8 column segments) (its block and its
+ *     coefficients); about 1/G of wf_trace_validate's ce * k * 8, twice.
+ * Refusals (WF_ERR_INVALID / WF_ERR_UNSUPPORTED: a world that is not a power of two >= 2, a trace shorter than 64 * world rows
+ * -- the prover's row-shard condition, N/G >= 64 * blowup, with the CE blowup in place of the proof's --, what
+ * wf_trace_validate refuses, a local_count that is not this rank's) happen before any device buffer is allocated, and every
+ * rank returns an error: the checks on shared values need no communication, and every rank's verdict on its own block is
+ * all-gathered before the first exchange. No device buffer stays live after any return. */
+int wf_trace_validate_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* air_desc, size_t air_desc_len,
+                              const uint64_t* aux_build, size_t aux_build_len, const uint64_t* const* aux_cols,
+                              const uint64_t* const* local_cols, const uint64_t* d_local, uint32_t local_count, int mont,
+                              const uint64_t* rand, uint32_t log_n, uint32_t ext, int check_degrees, wf_validation* report,
+                              uint64_t* first_failing_step, uint64_t* expected_degrees, uint64_t* actual_degrees,
+                              char* msg, size_t msg_cap);
 
 /* ---- constraint kernels compiled per AIR ---------------------------------------------------------------------------
  * wf_eval_constraints / wf_prove_air[_aux] evaluate the AIR's transition programs with a kernel compiled at run time for that

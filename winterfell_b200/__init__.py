@@ -45,6 +45,16 @@ class Validation(C.Structure):
                 ("num_transition_constraints", C.c_uint32)]
 
 
+def validation_dict(rep, first, exp, act, msg, check_degrees):
+    """The dict of Context.trace_validate from a filled wf_validation, its three arrays and its message buffer."""
+    k = rep.num_transition_constraints
+    return {"kind": rep.kind, "index": rep.index, "step": rep.step, "column": rep.column,
+            "first_failing_step": [None if int(v) == 2**64 - 1 else int(v) for v in first[:k]],
+            "expected_degrees": [int(v) for v in exp[:k]] if check_degrees else None,
+            "actual_degrees": [int(v) for v in act[:k]] if check_degrees else None,
+            "msg": msg.value.decode(errors="replace")}
+
+
 _lib = None
 
 # every symbol include/winterfell_b200.h declares: (name, restype, argtypes)
@@ -153,6 +163,9 @@ _SIGS = [
     ("wf_shard_columns", C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     ("wf_prove_air_sharded", C.c_int, [vp, vp, u64p, C.c_size_t, u64p, C.c_size_t, AUX_BUILDER, vp, C.POINTER(u64p), vp, C.c_uint32,
                                        C.c_int, C.c_uint32, C.POINTER(C.c_uint32), u8p, C.POINTER(C.c_size_t), C.POINTER(C.c_double)]),
+    ("wf_trace_validate_sharded", C.c_int, [vp, vp, u64p, C.c_size_t, u64p, C.c_size_t, C.POINTER(u64p), C.POINTER(u64p), vp, C.c_uint32,
+                                            C.c_int, u64p, C.c_uint32, C.c_uint32, C.c_int, C.POINTER(Validation), u64p, u64p, u64p,
+                                            C.c_char_p, C.c_size_t]),
 ]
 
 
@@ -625,12 +638,7 @@ class Context:
         self.check(self.L.wf_trace_validate(self.h, dp, d_.size, bp, bl, aps, ptrs, dev, int(mont), rp, int(n).bit_length() - 1, ext,
                                             int(check_degrees), C.byref(rep), first.ctypes.data_as(u64p), exp.ctypes.data_as(u64p),
                                             act.ctypes.data_as(u64p), msg, 1 << 16))
-        k = rep.num_transition_constraints
-        return {"kind": rep.kind, "index": rep.index, "step": rep.step, "column": rep.column,
-                "first_failing_step": [None if int(v) == 2**64 - 1 else int(v) for v in first[:k]],
-                "expected_degrees": [int(v) for v in exp[:k]] if check_degrees else None,
-                "actual_degrees": [int(v) for v in act[:k]] if check_degrees else None,
-                "msg": msg.value.decode(errors="replace")}
+        return validation_dict(rep, first, exp, act, msg, check_degrees)
 
     def set_validation(self, on):
         """The analogue of a debug build (default off): the proving entry points and eval_constraints check the trace against

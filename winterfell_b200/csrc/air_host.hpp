@@ -404,6 +404,7 @@ struct TraceCheckPart {
     u32 acol0 = 0;
     const wf_mat* main = nullptr;   // transitions: main (and aux, which is also where the aux assertions are read) trace rows
     const wf_mat* aux = nullptr;
+    SegMatrix aasrt{};          // the aux assertions' n trace rows when `aux` holds a row window (base NULL: aux's own rows)
     size_t s0 = 0, s1 = 0;      // the steps checked: [s0, s1)
     size_t row0 = 0, rows = 0;  // rows != 0: main / aux hold trace rows [row0, row0 + rows), then row (row0 + rows) mod n
 };

@@ -1463,6 +1463,7 @@ struct ShardCtx {
     int G, r;
     double bytes_sent = 0, bytes_overlapped = 0, ncoll = 0, ms_small = 0;
     bool forked = false;
+    bool peer_push = false;   // shard_trace_lde pushed its blocks with peer copies
     // exchanges issued between fork() and join() run on the communicator's stream, behind the ctx stream's tail at fork time
     // (wf_comm::fork / join; without the callbacks they simply stay on the ctx stream)
     int fork() {
@@ -1612,6 +1613,22 @@ static int exchange_halo(ShardCtx& sc, const SegMatrix& m, size_t b) {
     return WF_OK;
 }
 
+// *out (rows + halo rows allocated, m.rows = rows) <- rows [row0, row0 + rows) of every segment of `full`, then its rows
+// [h0, h0 + halo): a row shard with its halo, cut from a matrix this rank holds whole
+static int copy_row_window(wf_ctx* ctx, const wf_mat* full, size_t row0, size_t rows, size_t h0, size_t halo, wf_mat** out) {
+    wf_mat* win = nullptr;
+    CKI(wf_mat_alloc_w(ctx, rows + halo, full->m.cols, full->m.W, &win));
+    win->m.rows = rows;
+    const size_t rb = (size_t)full->m.W * 8, sp = full->m.seg_stride * 8, dp = win->m.seg_stride * 8;
+    const u32 nsg = full->m.nseg();
+    cudaError_t e = cudaMemcpy2DAsync(win->m.base, dp, full->m.base + row0 * full->m.W, sp, rows * rb, nsg, cudaMemcpyDeviceToDevice, ctx->st);
+    if (e == cudaSuccess)
+        e = cudaMemcpy2DAsync(win->m.base + rows * full->m.W, dp, full->m.base + h0 * full->m.W, sp, halo * rb, nsg, cudaMemcpyDeviceToDevice, ctx->st);
+    if (e != cudaSuccess) { wf_mat_free(ctx, win); return wf_fail(ctx, WF_ERR_CUDA, "row shard copy: %s", cudaGetErrorString(e)); }
+    *out = win;
+    return WF_OK;
+}
+
 // This rank's LDE rows [r N/G, (r+1) N/G) of polynomials every rank holds, too few columns to shard by column (the composition
 // polynomial, the aux segment). With blowup % G == 0 the LDE is sharded by COSET: rank r extends cosets [r b/G, (r+1) b/G)
 // (coset-major), one exchange hands every rank the rows of its range from every coset's owner, one kernel interleaves them into
@@ -1634,20 +1651,9 @@ static int shard_lde_rows(ShardCtx& sc, const wf_mat* polys, u32 log_b, bool hal
             view.m.rows = rows_per;
             return WF_OK;
         }
-        int rc = wf_mat_alloc_w(ctx, rows_per + b, cols, full->m.W, &rows);
-        if (rc == WF_OK) {
-            rows->m.rows = rows_per;
-            const size_t rb = (size_t)full->m.W * 8, sp = full->m.seg_stride * 8, dp = rows->m.seg_stride * 8;
-            const u32 nsg = full->m.nseg();
-            cudaError_t e = cudaMemcpy2DAsync(rows->m.base, dp, full->m.base + (size_t)r * rows_per * full->m.W, sp, rows_per * rb, nsg,
-                                              cudaMemcpyDeviceToDevice, ctx->st);
-            if (e == cudaSuccess)
-                e = cudaMemcpy2DAsync(rows->m.base + rows_per * full->m.W, dp, full->m.base + (size_t)((r + 1) % G) * rows_per * full->m.W, sp,
-                                      b * rb, nsg, cudaMemcpyDeviceToDevice, ctx->st);
-            if (e != cudaSuccess) rc = wf_fail(ctx, WF_ERR_CUDA, "row shard copy: %s", cudaGetErrorString(e));
-        }
+        const int rc = copy_row_window(ctx, full, (size_t)r * rows_per, rows_per, (size_t)((r + 1) % G) * rows_per, b, &rows);
         wf_mat_free(ctx, full);
-        if (rc != WF_OK) { wf_mat_free(ctx, rows); return rc; }
+        if (rc != WF_OK) return rc;
         *out = rows;
         view.m = rows->m;
         return WF_OK;
@@ -1697,187 +1703,29 @@ static int shard_lde_rows(ShardCtx& sc, const wf_mat* polys, u32 log_b, bool hal
     return WF_OK;
 }
 
-// ---- wf_ctx_set_validation in the sharded prover: the one-GPU prover's two checks (validate.cu), each rank doing its share
-//      of the work. One all_gather_host hands every rank everyone's raw results and every rank reduces them with the same host
-//      code, so all ranks reach the same verdict, return at the same point and stay in step for the next collective ----
-
-// Trace::validate. Rank r checks the main assertions on its own columns, every aux assertion (the aux segment is replicated)
-// and transition steps [r n/G, (r+1) n/G) of [0, n - exemptions). Two-segment AIRs: mtrace / atrace hold the whole trace (the
-// aux build gathered it), own columns included. Single-segment AIRs: rank r evaluates its columns (`polys`) on the trace
-// domain, and one exchange gives every rank its n/G rows of every column plus the next row (n c 8 / G bytes per rank).
-// The raw results combine by their minimum: for the assertions (assertion << 40 | cell), the reference's order.
-template <int D>
-static int sharded_check_trace(ShardCtx& sc, const AirHost& air, const wf_mat* polys, const wf_mat* mtrace, const wf_mat* atrace,
-                               const std::vector<u64>& rnd, u32 log_n, const std::vector<u32>& seg0, const std::vector<u32>& segs) {
+// The column -> row turn of a c-column trace LDE at blowup 2^log_b, the first phase of a sharded proof (and of the sharded
+// degree check, at the constraint evaluation blowup). Rank r owns columns shard_columns(c, G, r) (local_cols / d_local, as
+// wf_prove_air_sharded takes them; none: both may be NULL): it interpolates them (*polys, n rows) and extends them coset by
+// coset with no communication. Coset k is written coset-major, so that the rows of rank q's range (n / G points of the
+// coset) are one contiguous block per segment: its exchange runs while coset k + 1 is being extended. A rank that owns no
+// columns only receives. *shard: LDE rows [r N/G, (r+1) N/G) of every column, in natural order, followed by the first 2^log_b
+// rows of rank (r + 1) mod G's range (the halo the constraint frames read). polys / shard are the caller's to free.
+static int shard_trace_lde(ShardCtx& sc, const uint64_t* const* local_cols, const uint64_t* d_local, int mont, u32 log_n, u32 c, u32 log_b,
+                           const std::vector<u32>& seg0, const std::vector<u32>& segs, wf_mat*& polys, wf_mat*& shard) {
     wf_ctx* ctx = sc.ctx;
     const int G = sc.G, r = sc.r;
-    const size_t n = (size_t)1 << log_n, nt = n / (size_t)G;
-    const u32 fs = seg0[r], nsl = segs[r];
-    const u32 col0 = std::min(air.w, fs * 8), cl = std::min(air.w, (fs + nsl) * 8) - col0;
-    wf_mat *own = nullptr, *rows = nullptr;
-    struct Free { wf_ctx* c; wf_mat** a; wf_mat** b; ~Free() { wf_mat_free(c, *a); wf_mat_free(c, *b); } } fr{ctx, &own, &rows};
-    TraceCheckPart part;
-    part.acol0 = col0;
-    part.s0 = (size_t)r * nt;
-    part.s1 = std::min((size_t)(r + 1) * nt, n - air.exemptions);
-    if (mtrace) {
-        part.amain = mtrace->m;
-        part.amain.base += (size_t)fs * mtrace->m.seg_stride;
-        part.amain.cols = cl;
-        part.main = mtrace;
-        part.aux = atrace;
-    } else {
-        CKI(wf_mat_alloc_w(ctx, n, cl, 8, &own));
-        if (cl) {
-            wf_mat* ev;
-            CKI(wf_mat_evaluate(ctx, polys, &ev));
-            const cudaError_t e = layout_select_cols(ev->m, 0, own->m, ctx->st);
-            ctx->launches++;
-            wf_mat_free(ctx, ev);
-            CK(e);
-        }
-        part.amain = own->m;
-        CKI(wf_mat_alloc_w(ctx, nt + 1, air.w, 8, &rows));
-        rows->m.rows = nt;   // row nt: the halo row
-        std::vector<int> sp, rp;
-        std::vector<const void*> sv;
-        std::vector<void*> rv;
-        for (int q = 0; q < G; q++) {   // my segments' rows of rank q's range, ascending; from rank q its segments, ascending
-            for (u32 sg = 0; sg < nsl; sg++) {
-                const u64* src = own->m.base + (size_t)sg * own->m.seg_stride + (size_t)q * nt * 8;
-                if (q == r) CK(cudaMemcpyAsync(rows->m.base + (size_t)(fs + sg) * rows->m.seg_stride, src, nt * 64, cudaMemcpyDeviceToDevice, ctx->st));
-                else { sp.push_back(q); sv.push_back(src); }
-            }
-            for (u32 sg = 0; q != r && sg < segs[q]; sg++) { rp.push_back(q); rv.push_back(rows->m.base + (size_t)(seg0[q] + sg) * rows->m.seg_stride); }
-        }
-        CKI(sc.exchange(sp, sv, rp, rv, nt * 64));
-        CKI(exchange_halo(sc, rows->m, 1));
-        part.main = rows;
-        part.row0 = (size_t)r * nt;
-        part.rows = nt;
-    }
-    std::vector<u64> raw;
-    CKI(wf_check_trace_part(ctx, air, part, rnd.data(), log_n, D, raw));
-    std::vector<u64> all(raw.size() * (size_t)G);
-    CKI(sc.gather_host(raw.data(), all.data(), raw.size() * 8));
-    for (int q = 0; q < G; q++)
-        for (size_t j = 0; j < raw.size(); j++) raw[j] = std::min(raw[j], all[(size_t)q * raw.size() + j]);
-    TraceReport rep;
-    wf_trace_verdict(air, atrace != nullptr, D, raw, rep);
-    return validation_result(ctx, WF_OK, rep);
-}
-
-// validate_transition_degrees on the prover's own LDE row shards (`lde`, `alde`: LDE rows [r N/G, (r+1) N/G) and the blowup
-// halo rows). Rank r evaluates every transition constraint over its divisor on CE rows [r ce/G, (r+1) ce/G); one exchange
-// moves that ce/G x ncols matrix into column blocks (rank q: shard_segments(ncols, G, q)'s 8-column segments over all ce
-// rows); every rank interpolates its block and finds its columns' degrees; one all_gather_host of the blocks' degrees (padded
-// to the largest block) gives every rank all of them. An aux constraint's D columns may lie in two blocks: the verdict takes
-// the maximum over its columns either way. With ncols <= 8 rank 0 alone transforms.
-template <int D>
-static int sharded_check_degrees(ShardCtx& sc, const AirHost& air, const wf_mat* lde, const wf_mat* alde, const std::vector<u64>& rnd,
-                                 u32 log_n, u32 log_b) {
-    wf_ctx* ctx = sc.ctx;
-    const int G = sc.G, r = sc.r;
-    const u32 ncols = (u32)air.degrees.size() + (alde ? (u32)air.aux_degrees.size() * D : 0);
-    const size_t ce = (size_t)1 << (log_n + air.log_ce_blowup()), ce_per = ce / (size_t)G;
-    std::vector<u32> cs0(G), cns(G);
-    u32 blk = 0;
-    for (int q = 0; q < G; q++) { shard_segments(ncols, (u32)G, (u32)q, cs0[q], cns[q]); blk = std::max(blk, cns[q] * 8); }
-    u32 first, cnt;
-    shard_columns(ncols, (u32)G, (u32)r, first, cnt);
-    wf_mat *loc = nullptr, *mine = nullptr;
-    struct Free { wf_ctx* c; wf_mat** a; wf_mat** b; ~Free() { wf_mat_free(c, *a); wf_mat_free(c, *b); } } fr{ctx, &loc, &mine};
-    CKI(wf_mat_alloc_w(ctx, ce_per, ncols, 8, &loc));
-    CKI(wf_transition_columns(ctx, air, lde, alde, rnd.data(), log_n, log_b, D, (size_t)r * ce_per, ce_per, loc->m));
-    if (cnt) CKI(wf_mat_alloc_w(ctx, ce, cnt, 8, &mine));
-    {
-        std::vector<int> sp, rp;
-        std::vector<const void*> sv;
-        std::vector<void*> rv;
-        for (int q = 0; q < G; q++) {   // to rank q: its segments ascending; from rank q: my segments ascending
-            for (u32 sg = 0; sg < cns[q]; sg++) {
-                const u64* src = loc->m.base + (size_t)(cs0[q] + sg) * loc->m.seg_stride;
-                if (q == r) CK(cudaMemcpyAsync(mine->m.base + (size_t)sg * mine->m.seg_stride + (size_t)r * ce_per * 8, src, ce_per * 64,
-                                               cudaMemcpyDeviceToDevice, ctx->st));
-                else { sp.push_back(q); sv.push_back(src); }
-            }
-            for (u32 sg = 0; q != r && sg < cns[r]; sg++) { rp.push_back(q); rv.push_back(mine->m.base + (size_t)sg * mine->m.seg_stride + (size_t)q * ce_per * 8); }
-        }
-        CKI(sc.exchange(sp, sv, rp, rv, ce_per * 64));
-    }
-    wf_mat_free(ctx, loc);
-    loc = nullptr;
-    std::vector<u64> d1;
-    if (cnt) CKI(wf_column_degrees(ctx, mine, d1));
-    d1.resize(blk, 0);
-    std::vector<u64> all((size_t)blk * G), deg1(ncols);
-    CKI(sc.gather_host(d1.data(), all.data(), (size_t)blk * 8));
-    for (int q = 0; q < G; q++)
-        for (u32 j = cs0[q] * 8; j < std::min(ncols, (cs0[q] + cns[q]) * 8); j++) deg1[j] = all[(size_t)q * blk + j - cs0[q] * 8];
-    TraceReport rep;
-    wf_degree_verdict(air, alde != nullptr, D, log_n, deg1, rep);
-    return validation_result(ctx, WF_OK, rep);
-}
-
-// One proof of `air_in` sharded over the ranks of `cm` (wf_prove_air_sharded, wf_prove_fib_sharded). Rank r owns the main-trace
-// columns shard_columns() gives it: local_cols / d_local hold exactly those (none: both may be NULL). aux_build: the described
-// build of a two-segment AIR's aux segment (replicated on every rank from the all-gathered main trace).
-template <int D>
-int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const AuxBuildHost* aux_build, wf_aux_assertions_fn aux_assertions,
-                  void* aux_user, const uint64_t* const* local_cols, const uint64_t* d_local, int mont, u32 log_n, const Options& o,
-                  std::vector<u8>& proof_out, double* stats) {
-    AirHost air_dyn;                       // copy whose aux assertion values are rewritten from the random elements (as prove_air)
-    if (aux_assertions) air_dyn = air_in;
-    const AirHost& air = aux_assertions ? air_dyn : air_in;
-    ShardCtx sc{ctx, cm, cm->world, cm->rank};
-    const int G = sc.G, r = sc.r;
-    const int h = o.hash_id;
-    const size_t n = (size_t)1 << log_n;
-    const u32 log_b = log2_ceil(o.blowup);
-    const size_t N = n << log_b, b = o.blowup;
-    const u32 c = air.w, aw = air.aw, nsg = (c + 7) / 8;
-    const size_t rows_per = N / (size_t)G;
-    if (G < 2 || (G & (G - 1)) || r < 0 || r >= G) return wf_fail(ctx, WF_ERR_INVALID, "world size must be a power of two >= 2");
-    if (aw && !aux_build) return wf_fail(ctx, WF_ERR_INVALID, "multi-segment AIR needs an aux build description");
-    std::vector<u32> seg0(G), segs(G), col0(G), ncol(G);   // every rank's block: first segment, segments, first column, columns
-    for (int q = 0; q < G; q++) {
-        shard_segments(c, (u32)G, (u32)q, seg0[q], segs[q]);
-        shard_columns(c, (u32)G, (u32)q, col0[q], ncol[q]);
-    }
-    const u32 cl = ncol[r], fs = seg0[r], nsl = segs[r];
-    const u32 maxcl = *std::max_element(ncol.begin(), ncol.end());
-    const u32 kc = air.num_comp_cols(n), log_ceb = air.log_ce_blowup();
-    const size_t ce = n << log_ceb, ce_per = ce / (size_t)G;
-    if (rows_per < 64 * b || ce_per < 64) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "trace too short to shard over %d ranks", G);
-    const bool validate = ctx->validate && !air.is_fib;   // wf_ctx_set_validation, as prove_air; wf_prove_fib_sharded is not checked
-    Channel ch(h, context_seed(air, n, o));  // every rank replays the whole transcript
-
-    wf_mat *polys = nullptr, *lde = nullptr, *shard = nullptr, *mtrace = nullptr, *atrace = nullptr, *apolys = nullptr, *arows = nullptr,
-           *comp_l = nullptr, *comp = nullptr, *cpolys = nullptr, *clde = nullptr, *deep = nullptr, *fri_in = nullptr, *tstage = nullptr;
-    ShardTree ttree, atree, ctree;
-    wf_fri* fri = nullptr;
-    ProofScope scope(ctx);   // holds the ADDRESSES of these pointers: every owned pointer lives as long as the scope
-    scope.own({&polys, &lde, &shard, &mtrace, &atrace, &apolys, &arows, &comp_l, &comp, &cpolys, &clde, &deep, &fri_in, &tstage});
-    scope.own({&ttree.local, &atree.local, &ctree.local});
-    scope.fri = &fri;
-    struct SLayer { u64* vals; size_t m_l, m_g; ShardTree tree; };
-    std::vector<SLayer> slayers;   // FRI layers folded on row shards
-    std::vector<void*> owned;      // device buffers of the sharded FRI phase
-    struct Cleanup {
-        wf_ctx* ctx; std::vector<SLayer>& sl; std::vector<void*>& ow;
-        ~Cleanup() { for (auto& l : sl) wf_tree_free(ctx, l.tree.local); for (void* p : ow) wf_dev_free(ctx, p); }
-    } cleanup{ctx, slayers, owned};
-
-    // ---- 1. interpolate the local columns, then extend them coset by coset (no communication: columns are independent).
-    //         Coset k is written coset-major, so that the rows of rank q's range (n / G points of the coset) are one contiguous
-    //         block per segment: its exchange runs on the communicator's stream while coset k + 1 is being extended. A rank that
-    //         owns no columns only receives ----
-    wf_mark(ctx, "start");
+    const size_t n = (size_t)1 << log_n, b = (size_t)1 << log_b, N = n << log_b, rows_per = N / (size_t)G;
+    const u32 nsg = (c + 7) / 8, fs = seg0[r], nsl = segs[r];
+    u32 first, cl;
+    shard_columns(c, (u32)G, (u32)r, first, cl);
     const size_t nj = n / (size_t)G;   // points of one coset inside one rank's row range
+    wf_mat *lde = nullptr, *stage = nullptr;
+    ProofScope scope(ctx);
+    scope.own({&lde, &stage});
     // the row shard and the staging matrix hold all c columns in 8-column segments, a partly filled last one included
     CKI(wf_mat_alloc_w(ctx, rows_per + b, c, 8, &shard));
     shard->m.rows = rows_per;  // seg_stride stays (rows_per + b) * 8: rows [rows_per, rows_per + b) are the halo
-    wf_mat*& stage = tstage;           // what arrives: [global segment][coset][nj][8]
+    // what arrives: [global segment][coset][nj][8]
     if (cl) CKI(wf_mat_alloc_w(ctx, N, cl, 8, &lde));  // mine, coset-major: [local segment][coset][n][8]
     CKI(wf_mat_alloc_w(ctx, rows_per, c, 8, &stage));
     // Preferred transport: every rank maps the others' `stage` buffers (CUDA IPC) and PUSHES its blocks there with peer copies
@@ -1885,6 +1733,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
     // side stream were measured: they slow the LDE down by as much as they hide). Fallback: the communicator's exchange.
     std::vector<void*> peer_stage;
     const bool push = sc.map_peers(stage->m.base, peer_stage) == WF_OK;
+    sc.peer_push = push;
     if (push) {
         for (int i = 0; i < 4; i++) if (!ctx->push_st[i]) CK(cudaStreamCreateWithFlags(&ctx->push_st[i], cudaStreamNonBlocking));
         for (int i = 0; i < 16; i++) if (!ctx->push_ev[i]) CK(cudaEventCreateWithFlags(&ctx->push_ev[i], cudaEventDisableTiming));
@@ -1952,6 +1801,224 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
     scope.drop(stage);
     CKI(exchange_halo(sc, shard->m, b));   // the first `blowup` rows of every segment of rank (r + 1) mod G
     wf_mark(ctx, "trace_exchange");
+    return WF_OK;
+}
+
+// *mtrace <- the whole n x c main trace on every rank (the aux build reads main rows i and i + 1 of every column): rank r
+// evaluates its columns (`polys`, none: NULL) on the trace domain and one all-gather by segment fills in everyone else's.
+static int gather_main_trace(ShardCtx& sc, const wf_mat* polys, u32 log_n, u32 c, const std::vector<u32>& seg0, const std::vector<u32>& segs,
+                             wf_mat*& mtrace) {
+    wf_ctx* ctx = sc.ctx;
+    const int G = sc.G, r = sc.r;
+    const size_t n = (size_t)1 << log_n;
+    const u32 fs = seg0[r], nsl = segs[r];
+    u32 first, cl;
+    shard_columns(c, (u32)G, (u32)r, first, cl);
+    CKI(wf_mat_alloc_w(ctx, n, c, 8, &mtrace));
+    if (cl) {
+        wf_mat* ev;
+        CKI(wf_mat_evaluate(ctx, polys, &ev));
+        SegMatrix dv = mtrace->m;
+        dv.base += (size_t)fs * dv.seg_stride;
+        dv.cols = cl;
+        const cudaError_t e = layout_select_cols(ev->m, 0, dv, ctx->st);
+        ctx->launches++;
+        wf_mat_free(ctx, ev);
+        CK(e);
+    }
+    std::vector<int> sp, rp;
+    std::vector<const void*> sv;
+    std::vector<void*> rv;
+    for (int q = 0; q < G; q++) {
+        if (q == r) continue;
+        for (u32 sg = 0; sg < nsl; sg++) { sp.push_back(q); sv.push_back(mtrace->m.base + (size_t)(fs + sg) * mtrace->m.seg_stride); }
+        for (u32 sg = 0; sg < segs[q]; sg++) { rp.push_back(q); rv.push_back(mtrace->m.base + (size_t)(seg0[q] + sg) * mtrace->m.seg_stride); }
+    }
+    return sc.exchange(sp, sv, rp, rv, n * 64);
+}
+
+// ---- wf_ctx_set_validation in the sharded prover: the one-GPU prover's two checks (validate.cu), each rank doing its share
+//      of the work. One all_gather_host hands every rank everyone's raw results and every rank reduces them with the same host
+//      code, so all ranks reach the same verdict, return at the same point and stay in step for the next collective ----
+
+// Trace::validate into `rep` (fresh; the same on every rank). Rank r checks the main assertions on its own columns, every aux
+// assertion (the aux segment is replicated) and transition steps [r n/G, (r+1) n/G) of [0, n - exemptions). With mtrace, the
+// whole main trace (the aux build gathered it), own columns included. Without: rank r evaluates its columns (`polys`) on the
+// trace domain, and one exchange gives every rank its n/G rows of every column plus the next row (n c 8 / G bytes per rank);
+// a replicated aux segment (atrace, whole) gives its rows of the same window by a device copy.
+// The raw results combine by their minimum: for the assertions (assertion << 40 | cell), the reference's order.
+template <int D>
+static int sharded_check_trace(ShardCtx& sc, const AirHost& air, const wf_mat* polys, const wf_mat* mtrace, const wf_mat* atrace,
+                               const std::vector<u64>& rnd, u32 log_n, const std::vector<u32>& seg0, const std::vector<u32>& segs,
+                               TraceReport& rep) {
+    wf_ctx* ctx = sc.ctx;
+    const int G = sc.G, r = sc.r;
+    const size_t n = (size_t)1 << log_n, nt = n / (size_t)G;
+    const u32 fs = seg0[r], nsl = segs[r];
+    const u32 col0 = std::min(air.w, fs * 8), cl = std::min(air.w, (fs + nsl) * 8) - col0;
+    wf_mat *own = nullptr, *rows = nullptr, *arows = nullptr;
+    ProofScope scope(ctx);
+    scope.own({&own, &rows, &arows});
+    TraceCheckPart part;
+    part.acol0 = col0;
+    part.s0 = (size_t)r * nt;
+    part.s1 = std::min((size_t)(r + 1) * nt, n - air.exemptions);
+    if (mtrace) {
+        part.amain = mtrace->m;
+        part.amain.base += (size_t)fs * mtrace->m.seg_stride;
+        part.amain.cols = cl;
+        part.main = mtrace;
+        part.aux = atrace;
+    } else {
+        CKI(wf_mat_alloc_w(ctx, n, cl, 8, &own));
+        if (cl) {
+            wf_mat* ev;
+            CKI(wf_mat_evaluate(ctx, polys, &ev));
+            const cudaError_t e = layout_select_cols(ev->m, 0, own->m, ctx->st);
+            ctx->launches++;
+            wf_mat_free(ctx, ev);
+            CK(e);
+        }
+        part.amain = own->m;
+        CKI(wf_mat_alloc_w(ctx, nt + 1, air.w, 8, &rows));
+        rows->m.rows = nt;   // row nt: the halo row
+        std::vector<int> sp, rp;
+        std::vector<const void*> sv;
+        std::vector<void*> rv;
+        for (int q = 0; q < G; q++) {   // my segments' rows of rank q's range, ascending; from rank q its segments, ascending
+            for (u32 sg = 0; sg < nsl; sg++) {
+                const u64* src = own->m.base + (size_t)sg * own->m.seg_stride + (size_t)q * nt * 8;
+                if (q == r) CK(cudaMemcpyAsync(rows->m.base + (size_t)(fs + sg) * rows->m.seg_stride, src, nt * 64, cudaMemcpyDeviceToDevice, ctx->st));
+                else { sp.push_back(q); sv.push_back(src); }
+            }
+            for (u32 sg = 0; q != r && sg < segs[q]; sg++) { rp.push_back(q); rv.push_back(rows->m.base + (size_t)(seg0[q] + sg) * rows->m.seg_stride); }
+        }
+        CKI(sc.exchange(sp, sv, rp, rv, nt * 64));
+        CKI(exchange_halo(sc, rows->m, 1));
+        part.main = rows;
+        part.row0 = (size_t)r * nt;
+        part.rows = nt;
+        if (atrace) {
+            CKI(copy_row_window(ctx, atrace, (size_t)r * nt, nt, (size_t)((r + 1) % G) * nt, 1, &arows));
+            part.aux = arows;
+            part.aasrt = atrace->m;
+        }
+    }
+    std::vector<u64> raw;
+    CKI(wf_check_trace_part(ctx, air, part, rnd.data(), log_n, D, raw));
+    std::vector<u64> all(raw.size() * (size_t)G);
+    CKI(sc.gather_host(raw.data(), all.data(), raw.size() * 8));
+    for (int q = 0; q < G; q++)
+        for (size_t j = 0; j < raw.size(); j++) raw[j] = std::min(raw[j], all[(size_t)q * raw.size() + j]);
+    wf_trace_verdict(air, atrace != nullptr, D, raw, rep);
+    return WF_OK;
+}
+
+// validate_transition_degrees into `rep` (its trace check's verdict, which a degree violation does not override; expected and
+// actual filled either way) on row shards of the trace LDE at blowup 2^log_b (`lde`, `alde`: LDE rows [r N/G, (r+1) N/G) and
+// the blowup halo rows; the prover's own, or the validator's at the CE blowup). Rank r evaluates every transition constraint over its divisor on CE rows [r ce/G, (r+1) ce/G); one exchange
+// moves that ce/G x ncols matrix into column blocks (rank q: shard_segments(ncols, G, q)'s 8-column segments over all ce
+// rows); every rank interpolates its block and finds its columns' degrees; one all_gather_host of the blocks' degrees (padded
+// to the largest block) gives every rank all of them. An aux constraint's D columns may lie in two blocks: the verdict takes
+// the maximum over its columns either way. With ncols <= 8 rank 0 alone transforms.
+template <int D>
+static int sharded_check_degrees(ShardCtx& sc, const AirHost& air, const wf_mat* lde, const wf_mat* alde, const std::vector<u64>& rnd,
+                                 u32 log_n, u32 log_b, TraceReport& rep) {
+    wf_ctx* ctx = sc.ctx;
+    const int G = sc.G, r = sc.r;
+    const u32 ncols = (u32)air.degrees.size() + (alde ? (u32)air.aux_degrees.size() * D : 0);
+    const size_t ce = (size_t)1 << (log_n + air.log_ce_blowup()), ce_per = ce / (size_t)G;
+    std::vector<u32> cs0(G), cns(G);
+    u32 blk = 0;
+    for (int q = 0; q < G; q++) { shard_segments(ncols, (u32)G, (u32)q, cs0[q], cns[q]); blk = std::max(blk, cns[q] * 8); }
+    u32 first, cnt;
+    shard_columns(ncols, (u32)G, (u32)r, first, cnt);
+    wf_mat *loc = nullptr, *mine = nullptr;
+    struct Free { wf_ctx* c; wf_mat** a; wf_mat** b; ~Free() { wf_mat_free(c, *a); wf_mat_free(c, *b); } } fr{ctx, &loc, &mine};
+    CKI(wf_mat_alloc_w(ctx, ce_per, ncols, 8, &loc));
+    CKI(wf_transition_columns(ctx, air, lde, alde, rnd.data(), log_n, log_b, D, (size_t)r * ce_per, ce_per, loc->m));
+    if (cnt) CKI(wf_mat_alloc_w(ctx, ce, cnt, 8, &mine));
+    {
+        std::vector<int> sp, rp;
+        std::vector<const void*> sv;
+        std::vector<void*> rv;
+        for (int q = 0; q < G; q++) {   // to rank q: its segments ascending; from rank q: my segments ascending
+            for (u32 sg = 0; sg < cns[q]; sg++) {
+                const u64* src = loc->m.base + (size_t)(cs0[q] + sg) * loc->m.seg_stride;
+                if (q == r) CK(cudaMemcpyAsync(mine->m.base + (size_t)sg * mine->m.seg_stride + (size_t)r * ce_per * 8, src, ce_per * 64,
+                                               cudaMemcpyDeviceToDevice, ctx->st));
+                else { sp.push_back(q); sv.push_back(src); }
+            }
+            for (u32 sg = 0; q != r && sg < cns[r]; sg++) { rp.push_back(q); rv.push_back(mine->m.base + (size_t)sg * mine->m.seg_stride + (size_t)q * ce_per * 8); }
+        }
+        CKI(sc.exchange(sp, sv, rp, rv, ce_per * 64));
+    }
+    wf_mat_free(ctx, loc);
+    loc = nullptr;
+    std::vector<u64> d1;
+    if (cnt) CKI(wf_column_degrees(ctx, mine, d1));
+    d1.resize(blk, 0);
+    std::vector<u64> all((size_t)blk * G), deg1(ncols);
+    CKI(sc.gather_host(d1.data(), all.data(), (size_t)blk * 8));
+    for (int q = 0; q < G; q++)
+        for (u32 j = cs0[q] * 8; j < std::min(ncols, (cs0[q] + cns[q]) * 8); j++) deg1[j] = all[(size_t)q * blk + j - cs0[q] * 8];
+    wf_degree_verdict(air, alde != nullptr, D, log_n, deg1, rep);
+    return WF_OK;
+}
+
+// One proof of `air_in` sharded over the ranks of `cm` (wf_prove_air_sharded, wf_prove_fib_sharded). Rank r owns the main-trace
+// columns shard_columns() gives it: local_cols / d_local hold exactly those (none: both may be NULL). aux_build: the described
+// build of a two-segment AIR's aux segment (replicated on every rank from the all-gathered main trace).
+template <int D>
+int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const AuxBuildHost* aux_build, wf_aux_assertions_fn aux_assertions,
+                  void* aux_user, const uint64_t* const* local_cols, const uint64_t* d_local, int mont, u32 log_n, const Options& o,
+                  std::vector<u8>& proof_out, double* stats) {
+    AirHost air_dyn;                       // copy whose aux assertion values are rewritten from the random elements (as prove_air)
+    if (aux_assertions) air_dyn = air_in;
+    const AirHost& air = aux_assertions ? air_dyn : air_in;
+    ShardCtx sc{ctx, cm, cm->world, cm->rank};
+    const int G = sc.G, r = sc.r;
+    const int h = o.hash_id;
+    const size_t n = (size_t)1 << log_n;
+    const u32 log_b = log2_ceil(o.blowup);
+    const size_t N = n << log_b, b = o.blowup;
+    const u32 c = air.w, aw = air.aw;
+    const size_t rows_per = N / (size_t)G;
+    if (G < 2 || (G & (G - 1)) || r < 0 || r >= G) return wf_fail(ctx, WF_ERR_INVALID, "world size must be a power of two >= 2");
+    if (aw && !aux_build) return wf_fail(ctx, WF_ERR_INVALID, "multi-segment AIR needs an aux build description");
+    std::vector<u32> seg0(G), segs(G), col0(G), ncol(G);   // every rank's block: first segment, segments, first column, columns
+    for (int q = 0; q < G; q++) {
+        shard_segments(c, (u32)G, (u32)q, seg0[q], segs[q]);
+        shard_columns(c, (u32)G, (u32)q, col0[q], ncol[q]);
+    }
+    const u32 cl = ncol[r];
+    const u32 maxcl = *std::max_element(ncol.begin(), ncol.end());
+    const u32 kc = air.num_comp_cols(n), log_ceb = air.log_ce_blowup();
+    const size_t ce = n << log_ceb, ce_per = ce / (size_t)G;
+    if (rows_per < 64 * b || ce_per < 64) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "trace too short to shard over %d ranks", G);
+    const bool validate = ctx->validate && !air.is_fib;   // wf_ctx_set_validation, as prove_air; wf_prove_fib_sharded is not checked
+    Channel ch(h, context_seed(air, n, o));  // every rank replays the whole transcript
+
+    wf_mat *polys = nullptr, *shard = nullptr, *mtrace = nullptr, *atrace = nullptr, *apolys = nullptr, *arows = nullptr,
+           *comp_l = nullptr, *comp = nullptr, *cpolys = nullptr, *clde = nullptr, *deep = nullptr, *fri_in = nullptr;
+    ShardTree ttree, atree, ctree;
+    wf_fri* fri = nullptr;
+    ProofScope scope(ctx);   // holds the ADDRESSES of these pointers: every owned pointer lives as long as the scope
+    scope.own({&polys, &shard, &mtrace, &atrace, &apolys, &arows, &comp_l, &comp, &cpolys, &clde, &deep, &fri_in});
+    scope.own({&ttree.local, &atree.local, &ctree.local});
+    scope.fri = &fri;
+    struct SLayer { u64* vals; size_t m_l, m_g; ShardTree tree; };
+    std::vector<SLayer> slayers;   // FRI layers folded on row shards
+    std::vector<void*> owned;      // device buffers of the sharded FRI phase
+    struct Cleanup {
+        wf_ctx* ctx; std::vector<SLayer>& sl; std::vector<void*>& ow;
+        ~Cleanup() { for (auto& l : sl) wf_tree_free(ctx, l.tree.local); for (void* p : ow) wf_dev_free(ctx, p); }
+    } cleanup{ctx, slayers, owned};
+
+    // ---- 1. interpolate the local columns, extend them coset by coset (no communication: columns are independent) and turn
+    //         them into my row shard with its halo (shard_trace_lde) ----
+    wf_mark(ctx, "start");
+    CKI(shard_trace_lde(sc, local_cols, d_local, mont, log_n, c, log_b, seg0, segs, polys, shard));
     // ---- 2. leaves + subtree over my rows, all-gather of the subtree roots ----
     Digest root;
     CKI(wf_commit_rows_partitioned(ctx, h, shard, o.part_words(c, 1), &ttree.local));
@@ -1968,29 +2035,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
     wf_mat aview;               // my aux rows
     if (aw) {
         for (u32 i = 0; i < air.nr; i++) { GlExt<D> e = draw_ext<D>(ch.coin); for (int q = 0; q < D; q++) rnd_flat.push_back(e.v[q]); }
-        CKI(wf_mat_alloc_w(ctx, n, c, 8, &mtrace));
-        if (cl) {
-            wf_mat* ev;
-            CKI(wf_mat_evaluate(ctx, polys, &ev));
-            SegMatrix dv = mtrace->m;
-            dv.base += (size_t)fs * dv.seg_stride;
-            dv.cols = cl;
-            const cudaError_t e = layout_select_cols(ev->m, 0, dv, ctx->st);
-            ctx->launches++;
-            wf_mat_free(ctx, ev);
-            CK(e);
-        }
-        {
-            std::vector<int> sp, rp;
-            std::vector<const void*> sv;
-            std::vector<void*> rv;
-            for (int q = 0; q < G; q++) {
-                if (q == r) continue;
-                for (u32 sg = 0; sg < nsl; sg++) { sp.push_back(q); sv.push_back(mtrace->m.base + (size_t)(fs + sg) * mtrace->m.seg_stride); }
-                for (u32 sg = 0; sg < segs[q]; sg++) { rp.push_back(q); rv.push_back(mtrace->m.base + (size_t)(seg0[q] + sg) * mtrace->m.seg_stride); }
-            }
-            CKI(sc.exchange(sp, sv, rp, rv, n * 64));
-        }
+        CKI(gather_main_trace(sc, polys, log_n, c, seg0, segs, mtrace));
         wf_mark(ctx, "main_trace_gather");
         CKI(wf_aux_build_run(ctx, *aux_build, mtrace, c, air.periodic, rnd_flat.data(), air.nr, D, &atrace));
         if (!validate) scope.drop(mtrace);   // else: the whole main trace the trace check reads
@@ -2014,14 +2059,20 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
         ch.commit(root.b);
     }
     if (validate) {   // Trace::validate (lib.rs:355-356): the aux segment and its assertion values are final
-        CKI(sharded_check_trace<D>(sc, air, polys, mtrace, atrace, rnd_flat, log_n, seg0, segs));
+        TraceReport rep;
+        CKI(sharded_check_trace<D>(sc, air, polys, mtrace, atrace, rnd_flat, log_n, seg0, segs, rep));
+        CKI(validation_result(ctx, WF_OK, rep));
         scope.drop(mtrace);
         scope.drop(atrace);
     }
     // ---- 3. constraint evaluation over my CE rows ----
     std::vector<GlExt<D>> cc = draw_coeffs<D>(ch.coin, o.batch_c, air.num_constraints());
     CKI(eval_constraints<D>(ctx, air, shard, aw ? arows : nullptr, cc, rnd_flat, log_n, log_b, &comp_l, (size_t)r * ce_per, ce_per));
-    if (validate) CKI(sharded_check_degrees<D>(sc, air, shard, aw ? arows : nullptr, rnd_flat, log_n, log_b));   // evaluator/default.rs:114
+    if (validate) {   // evaluator/default.rs:114
+        TraceReport rep;
+        CKI(sharded_check_degrees<D>(sc, air, shard, aw ? arows : nullptr, rnd_flat, log_n, log_b, rep));
+        CKI(validation_result(ctx, WF_OK, rep));
+    }
     wf_mark(ctx, "constraint_eval");
     // ---- 4. composition polynomial: all-gather the CE evaluations (a few hundred MiB at most), interpolate on every rank (the
     //         transform is over the row index), extend and commit my row range ----
@@ -2226,7 +2277,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
         for (int i = 4; i < 8; i++) stats[i] = 0;
         stats[4] = (double)slayers.size();
         stats[5] = sc.bytes_overlapped;
-        stats[6] = push ? 1.0 : 0.0;
+        stats[6] = sc.peer_push ? 1.0 : 0.0;
     }
     return WF_OK;
 }
@@ -2451,6 +2502,16 @@ extern "C" int wf_prove_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* c
 }
 
 // ---- the reference's debug-build checks of a trace (validate.cu), standalone ----
+// the report of wf_trace_validate / wf_trace_validate_sharded
+static void write_validation(const TraceReport& rep, u32 n_tr, int check_degrees, wf_validation* report, uint64_t* first_failing_step,
+                             uint64_t* expected_degrees, uint64_t* actual_degrees, char* msg, size_t msg_cap) {
+    report->kind = rep.kind; report->index = rep.index; report->step = rep.step; report->column = rep.column;
+    report->num_transition_constraints = n_tr;
+    if (first_failing_step) std::copy(rep.first_fail.begin(), rep.first_fail.end(), first_failing_step);
+    if (check_degrees && expected_degrees) std::copy(rep.expected.begin(), rep.expected.end(), expected_degrees);
+    if (check_degrees && actual_degrees) std::copy(rep.actual.begin(), rep.actual.end(), actual_degrees);
+    if (msg && msg_cap) { strncpy(msg, rep.msg.c_str(), msg_cap - 1); msg[msg_cap - 1] = 0; }
+}
 extern "C" int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len,
                                  const uint64_t* const* aux_cols, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont,
                                  const uint64_t* rand, uint32_t log_n, uint32_t ext, int check_degrees, wf_validation* report,
@@ -2502,12 +2563,117 @@ extern "C" int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t a
         }
         CKI(wf_check_degrees(ctx, air, lde, alde, rnd.data(), log_n, log_ceb, (int)ext, rep));
     }
-    report->kind = rep.kind; report->index = rep.index; report->step = rep.step; report->column = rep.column;
-    report->num_transition_constraints = n_tr;
-    if (first_failing_step) std::copy(rep.first_fail.begin(), rep.first_fail.end(), first_failing_step);
-    if (check_degrees && expected_degrees) std::copy(rep.expected.begin(), rep.expected.end(), expected_degrees);
-    if (check_degrees && actual_degrees) std::copy(rep.actual.begin(), rep.actual.end(), actual_degrees);
-    if (msg && msg_cap) { strncpy(msg, rep.msg.c_str(), msg_cap - 1); msg[msg_cap - 1] = 0; }
+    write_validation(rep, n_tr, check_degrees, report, first_failing_step, expected_degrees, actual_degrees, msg, msg_cap);
+    return WF_OK;
+}
+
+// wf_trace_validate over the ranks of `cm`, each rank with its block of main columns (as prove_sharded takes them): the
+// sharded prover's two checks without the proof. The degree check reads LDE row shards at the CE blowup, as the one-GPU
+// validator reads its whole LDE at that blowup; the aux segment is built (aux_build, from the gathered main trace) or
+// uploaded (aux_cols) whole on every rank, and its LDE sharded as the prover's.
+template <int D>
+static int validate_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air, const AuxBuildHost* aux_build, const uint64_t* const* aux_cols,
+                            const uint64_t* const* local_cols, const uint64_t* d_local, int mont, const std::vector<u64>& rnd, u32 log_n,
+                            bool check_degrees, TraceReport& rep) {
+    ShardCtx sc{ctx, cm, cm->world, cm->rank};
+    const int G = sc.G, r = sc.r;
+    const size_t n = (size_t)1 << log_n;
+    const u32 c = air.w, log_ceb = air.log_ce_blowup();
+    std::vector<u32> seg0(G), segs(G);
+    for (int q = 0; q < G; q++) shard_segments(c, (u32)G, (u32)q, seg0[q], segs[q]);
+    u32 first, cl;
+    shard_columns(c, (u32)G, (u32)r, first, cl);
+    wf_mat *trace = nullptr, *polys = nullptr, *shard = nullptr, *mtrace = nullptr, *atrace = nullptr, *apolys = nullptr, *arows = nullptr;
+    ProofScope scope(ctx);
+    scope.own({&trace, &polys, &shard, &mtrace, &atrace, &apolys, &arows});
+    if (check_degrees) {
+        CKI(shard_trace_lde(sc, local_cols, d_local, mont, log_n, c, log_ceb, seg0, segs, polys, shard));
+    } else if (cl) {
+        if (d_local) CKI(wf_mat_from_device_columns(ctx, d_local, cl, n, &trace));
+        else CKI(wf_mat_from_host_columns(ctx, local_cols, cl, n, 1, mont, &trace));
+        CKI(wf_mat_interpolate(ctx, trace, &polys));
+        scope.drop(trace);
+    }
+    if (aux_build) {
+        CKI(gather_main_trace(sc, polys, log_n, c, seg0, segs, mtrace));
+        CKI(wf_aux_build_run(ctx, *aux_build, mtrace, c, air.periodic, rnd.data(), air.nr, D, &atrace));
+    } else if (aux_cols) {
+        CKI(wf_mat_from_host_columns(ctx, aux_cols, air.aw, n, D, mont, &atrace));
+    }
+    CKI(sharded_check_trace<D>(sc, air, polys, mtrace, atrace, rnd, log_n, seg0, segs, rep));
+    scope.drop(mtrace);
+    scope.drop(polys);
+    if (!check_degrees) return WF_OK;
+    if (atrace) {
+        wf_mat aview;
+        CKI(wf_mat_interpolate(ctx, atrace, &apolys));
+        scope.drop(atrace);
+        CKI(shard_lde_rows(sc, apolys, log_ceb, true, &arows, aview));
+        scope.drop(apolys);
+    }
+    return sharded_check_degrees<D>(sc, air, shard, arows, rnd, log_n, log_ceb, rep);
+}
+
+extern "C" int wf_trace_validate_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* air_desc, size_t air_desc_len,
+                                         const uint64_t* aux_build, size_t aux_build_len, const uint64_t* const* aux_cols,
+                                         const uint64_t* const* local_cols, const uint64_t* d_local, uint32_t local_count, int mont,
+                                         const uint64_t* rand, uint32_t log_n, uint32_t ext, int check_degrees, wf_validation* report,
+                                         uint64_t* first_failing_step, uint64_t* expected_degrees, uint64_t* actual_degrees, char* msg,
+                                         size_t msg_cap) {
+    if (msg && msg_cap) msg[0] = 0;
+    if (!ctx) return WF_ERR_INVALID;
+    if (!comm || !comm->exchange || !comm->all_gather_host) return wf_fail(ctx, WF_ERR_INVALID, "bad communicator");
+    // Checks on what every rank shares (description, aux segment, random elements, log_n, world size): the same verdict
+    // everywhere, before any collective, so a refusal leaves no rank waiting.
+    const int G = comm->world;
+    if (G < 2 || (G & (G - 1)) || comm->rank < 0 || comm->rank >= G) return wf_fail(ctx, WF_ERR_INVALID, "world size must be a power of two >= 2");
+    if (!air_desc || !report || log_n < 3 || log_n > 30 || ext < 1 || ext > 3) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    AirHost air;
+    if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
+    const u32 log_ceb = air.log_ce_blowup();
+    CKI(air_check_host(ctx, air, log_n, 1u << log_ceb));
+    AuxBuildHost b;
+    if (air.aw) {
+        if (!aux_build == !aux_cols) return wf_fail(ctx, WF_ERR_INVALID, "two-segment AIR: pass exactly one of aux_build and aux_cols");
+        if (air.nr && !rand) return wf_fail(ctx, WF_ERR_INVALID, "random elements missing");
+        if (aux_build) {
+            CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
+            for (auto& col : b.cols)
+                for (u32 q = ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
+        }
+    } else if (aux_build || aux_cols) {
+        return wf_fail(ctx, WF_ERR_INVALID, "single-segment AIR: it has no aux segment");
+    }
+    // the row shard of the prover (rows_per >= 64 blowup, ce_per >= 64) with the CE blowup in place of the proof's: n >= 64 G
+    const size_t rows_per = ((size_t)1 << (log_n + log_ceb)) / (size_t)G;
+    if (log_n + log_ceb > 32 || rows_per < ((size_t)64 << log_ceb))
+        return wf_fail(ctx, WF_ERR_UNSUPPORTED, "trace too short to shard over %d ranks", G);
+    // this rank's own arguments (its column block): every rank learns every rank's verdict in the first collective, and all of
+    // them return when one refuses
+    u32 first, count;
+    shard_columns(air.w, (u32)G, (u32)comm->rank, first, count);
+    int mine = WF_OK;
+    if (local_count != count)
+        mine = wf_fail(ctx, WF_ERR_INVALID, "rank %d owns %u columns of %u (wf_shard_columns), not %u", comm->rank, count, air.w, local_count);
+    else if (count && !local_cols == !d_local)
+        mine = wf_fail(ctx, WF_ERR_INVALID, "bad arguments: pass exactly one of local_cols and d_local");
+    std::vector<int> verdicts(G);
+    if (comm->all_gather_host(comm->user, &mine, verdicts.data(), sizeof(int)) != 0) return wf_fail(ctx, WF_ERR_STATE, "all_gather_host callback failed");
+    if (mine != WF_OK) return mine;
+    for (int q = 0; q < G; q++)
+        if (verdicts[q] != WF_OK) return wf_fail(ctx, WF_ERR_INVALID, "rank %d refused its column block", q);
+    const std::vector<u64> rnd(rand, rand + (air.aw ? (size_t)air.nr * ext : 0));
+    const AuxBuildHost* bp = air.aw && aux_build ? &b : nullptr;
+    TraceReport rep;
+    int r;
+    switch (ext) {
+        case 1: r = validate_sharded<1>(ctx, comm, air, bp, aux_cols, local_cols, d_local, mont, rnd, log_n, check_degrees != 0, rep); break;
+        case 2: r = validate_sharded<2>(ctx, comm, air, bp, aux_cols, local_cols, d_local, mont, rnd, log_n, check_degrees != 0, rep); break;
+        default: r = validate_sharded<3>(ctx, comm, air, bp, aux_cols, local_cols, d_local, mont, rnd, log_n, check_degrees != 0, rep); break;
+    }
+    CKI(r);
+    const u32 n_tr = (u32)(air.degrees.size() + (air.aw ? air.aux_degrees.size() : 0));
+    write_validation(rep, n_tr, check_degrees, report, first_failing_step, expected_degrees, actual_degrees, msg, msg_cap);
     return WF_OK;
 }
 

@@ -251,7 +251,7 @@ int check_trace_part(wf_ctx* ctx, const AirHost& air, const TraceCheckPart& w, c
         }
         if (coff.back() == 0) continue;
         AssertionCheck c;
-        c.m = seg ? aux->m : w.amain; c.D = d; c.na = (u32)as.size(); c.res = res + seg;
+        c.m = !seg ? w.amain : w.aasrt.base ? w.aasrt : aux->m; c.D = d; c.na = (u32)as.size(); c.res = res + seg;
         CKI(up.put(coff, &c.coff)); CKI(up.put(col, &c.col)); CKI(up.put(fs, &c.first_step)); CKI(up.put(st, &c.stride));
         CKI(up.put(voff, &c.voff)); CKI(up.put(nv, &c.nvals)); CKI(up.put(vals, &c.vals));
         assertion_check_kernel<<<(unsigned)((coff.back() + 255) / 256), 256, 0, ctx->st>>>(c);

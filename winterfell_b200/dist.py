@@ -347,6 +347,49 @@ def prove_air_sharded(ctx, comm, desc, local_trace, log_n, opts, aux_build=None,
     return buf[: ln.value].tobytes()
 
 
+def trace_validate_sharded(ctx, comm, desc, local_trace, log_n, ext=1, rand=None, aux=None, aux_build=None, mont=False, check_degrees=True,
+                           device_ptr=None, local_count=None):
+    """wf_trace_validate_sharded: Context.trace_validate over comm.world GPUs, without a proof. local_trace: this rank's columns
+    [count, n] uint64 (host; count from shard_columns), or device_ptr = raw pointer to the same block column-major in HBM
+    (canonical). A two-segment AIR takes rand [num_rands, ext] and either aux (the whole aux segment, host columns
+    [aux_width, n, ext]) or aux_build, all the same on every rank. Returns Context.trace_validate's dict for the whole trace,
+    the same on every rank. local_count: the column count passed to the library (default: the rows of local_trace, or
+    shard_columns' count with device_ptr)."""
+    L = wf.lib()
+    d_ = np.ascontiguousarray(desc, dtype=np.uint64)
+    ptrs, dptr = None, None
+    if device_ptr is None:
+        a = np.ascontiguousarray(local_trace if local_trace is not None else [], dtype=np.uint64).reshape(-1, 1 << log_n)
+        count = a.shape[0] if local_count is None else local_count
+        if a.shape[0]:
+            ptrs = (wf.u64p * a.shape[0])(*[a[j].ctypes.data_as(wf.u64p) for j in range(a.shape[0])])
+    else:
+        count = shard_columns(int(d_[0]), comm.world, comm.rank)[1] if local_count is None else local_count
+        dptr = C.c_void_p(device_ptr) if device_ptr else None
+    rp = aps = bp = None
+    bl = 0
+    if rand is not None:
+        r_ = np.ascontiguousarray(rand, dtype=np.uint64).reshape(-1)
+        rp = r_.ctypes.data_as(wf.u64p)
+    if aux is not None:
+        x_ = np.ascontiguousarray(aux, dtype=np.uint64)
+        aps = (wf.u64p * x_.shape[0])(*[x_[j].ctypes.data_as(wf.u64p) for j in range(x_.shape[0])])
+    if aux_build is not None:
+        b_ = np.ascontiguousarray(aux_build, dtype=np.uint64)
+        bp, bl = b_.ctypes.data_as(wf.u64p), b_.size
+    cap = 1 + d_.size   # constraint counts are bounded by the description's length
+    first, exp, act = (np.zeros(cap, dtype=np.uint64) for _ in range(3))
+    rep = wf.Validation()
+    msg = C.create_string_buffer(1 << 16)
+    rc = L.wf_trace_validate_sharded(ctx.h, C.byref(comm.struct), d_.ctypes.data_as(wf.u64p), d_.size, bp, bl, aps, ptrs, dptr, count,
+                                     int(mont), rp, log_n, ext, int(check_degrees), C.byref(rep), first.ctypes.data_as(wf.u64p),
+                                     exp.ctypes.data_as(wf.u64p), act.ctypes.data_as(wf.u64p), msg, 1 << 16)
+    if comm.error is not None:
+        raise comm.error
+    ctx.check(rc)
+    return wf.validation_dict(rep, first, exp, act, msg, check_degrees)
+
+
 def bench_sharded(ctx, stream, cfg, steps, warmup, configs, proof_opts, flush, clock_sampler_cls, local_rank):
     """bench.py's N > 1 arm: ONE proof of `cfg` sharded over the ranks (strong scaling). Returns bench.py's record:
     ms per proof with this rank's column block resident in HBM, e2e ms from pinned host columns, stage times, the
