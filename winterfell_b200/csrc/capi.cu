@@ -1211,7 +1211,6 @@ int wf_fri_build_layers(wf_ctx* ctx, int hash_id, const wf_mat* evals, int d, ui
         CKI(wf_get_twiddles(ctx, log2_ceil(len), &master));
         void* nxt;
         CKI(g.tmp.alloc(m * ld * 8, &nxt));
-        if (ld > d) CK(cudaMemsetAsync(nxt, 0, m * ld * 8, ctx->st));
         CK(fri_fold_layer((u64*)cur, len, d, ld, (int)folding, alpha, master, (u64*)nxt, ld, ctx->st));
         ctx->launches++;
         f->layers.push_back(FriLayer{(u64*)g.tmp.keep(cur), len, t});   // the wf_fri owns layer and tree from here
@@ -1244,8 +1243,10 @@ int wf_fri_build_layers(wf_ctx* ctx, int hash_id, const wf_mat* evals, int d, ui
 // host synchronises ONCE at the end, replays commit_fri_layer / draw_fri_alpha on its own coin and checks
 // that it draws the alphas the device used. (The callback form above pays a device-to-host round trip
 // per layer: ~20 us x 8 layers on the 2^23-point codeword of cfg2.)
+// consume: the layer-0 evaluations are the buffer of `evals` itself (a single segment), which the wf_fri takes over: the matrix
+// is left without a buffer, and wf_mat_free then releases only the handle. Else layer 0 is a copy (the caller keeps its matrix).
 int wf_fri_build_layers_coin(wf_ctx* ctx, int hash_id, const wf_mat* evals, int d, uint32_t folding, uint32_t rem_max_deg,
-                             uint32_t blowup, PublicCoin& coin, std::vector<Digest>& commitments, wf_fri** out) {
+                             uint32_t blowup, PublicCoin& coin, std::vector<Digest>& commitments, wf_fri** out, wf_mat* consume) {
     if (!ctx || !evals || !out) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     if (d < 1 || d > 3 || (int)evals->m.cols != d) return wf_fail(ctx, WF_ERR_INVALID, "evaluations must have ext_degree base columns");
     if (folding != 2 && folding != 4 && folding != 8 && folding != 16) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "folding factor %u", folding);
@@ -1261,8 +1262,14 @@ int wf_fri_build_layers_coin(wf_ctx* ctx, int hash_id, const wf_mat* evals, int 
     size_t nlayers = 0;
     for (size_t l = len; l > max_rem; l /= folding) nlayers++;
     void *cur, *dstate, *dalpha, *dlog;
-    CKI(g.tmp.alloc(len * ld * 8, &cur));
-    CK(cudaMemcpyAsync(cur, evals->m.base, len * ld * 8, cudaMemcpyDeviceToDevice, ctx->st));
+    if (consume == evals && evals->m.nseg() == 1) {
+        cur = consume->m.base;
+        consume->m.base = nullptr;
+        g.tmp.bufs.push_back(cur);
+    } else {
+        CKI(g.tmp.alloc(len * ld * 8, &cur));
+        CK(cudaMemcpyAsync(cur, evals->m.base, len * ld * 8, cudaMemcpyDeviceToDevice, ctx->st));
+    }
     CKI(g.tmp.alloc(8 * 8, &dstate));
     CKI(g.tmp.alloc(8 * 8, &dalpha));
     CKI(g.tmp.alloc(std::max<size_t>(nlayers, 1) * 8 * 8, &dlog));
@@ -1283,7 +1290,6 @@ int wf_fri_build_layers_coin(wf_ctx* ctx, int hash_id, const wf_mat* evals, int 
         CKI(wf_get_twiddles(ctx, log2_ceil(len), &master));
         void* nxt;
         CKI(g.tmp.alloc(m * ld * 8, &nxt));
-        if (ld > d) CK(cudaMemsetAsync(nxt, 0, m * ld * 8, ctx->st));
         CK(fri_fold_layer((u64*)cur, len, d, ld, (int)folding, nullptr, master, (u64*)nxt, ld, ctx->st, (const u64*)dalpha));
         ctx->launches++;
         f->layers.push_back(FriLayer{(u64*)g.tmp.keep(cur), len, t});   // the wf_fri owns layer and tree from here

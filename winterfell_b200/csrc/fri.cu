@@ -106,6 +106,7 @@ __global__ void __launch_bounds__(256) fri_fold_kernel(const u64* __restrict__ e
     acc = ext_mul_base(acc, inv_nf);
 #pragma unroll
     for (int c = 0; c < D; c++) next[i * next_ld + c] = acc.v[c];
+    for (int c = D; c < next_ld; c++) next[i * next_ld + c] = 0;   // pad lane (next_ld = 4 for D = 3)
 }
 
 cudaError_t fri_hash_layer(int hash_id, const u64* evals, size_t len, int d, int ld, int nf, u64* digests,

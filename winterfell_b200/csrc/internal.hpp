@@ -164,7 +164,8 @@ struct PublicCoin;
 struct Digest;
 struct wf_fri;
 int wf_fri_build_layers_coin(wf_ctx* ctx, int hash_id, const wf_mat* evals, int d, uint32_t folding, uint32_t rem_max_deg,
-                             uint32_t blowup, PublicCoin& coin, std::vector<Digest>& commitments, wf_fri** out);
+                             uint32_t blowup, PublicCoin& coin, std::vector<Digest>& commitments, wf_fri** out,
+                             wf_mat* consume = nullptr);
 int wf_get_twiddles(wf_ctx* ctx, u32 log_n, const u64** out);
 struct wf_tree;
 int wf_fri_layer_tree(wf_ctx* ctx, int hash_id, const u64* vals, size_t len, int d, int ld, int nf, wf_tree** out);

@@ -169,40 +169,40 @@ __global__ void coset0_rows_kernel(const u64* src, size_t n, int W, u32 b, u64* 
 // poly_table.rs:68-76). Block = 32 row groups x 8 lanes (lane = column of the segment); a thread owns OOD_RPT
 // consecutive coefficients of ONE column and accumulates sum_r a_r z^r for both points on delayed-reduction
 // accumulators against a shared table of z^r (one base-by-extension product per coefficient and point, no reduction
-// inside the loop); the row-group power (z^OOD_RPT)^rg and the block power z^(first row of the block) — the latter
-// from a table filled by ood_pow_kernel, an ext_pow per thread there instead of per coefficient chunk here — are
-// applied once per thread / once per block. partial[col][chunk][point] = sum_{m in chunk} a_m z^m.
+// inside the loop); the row-group power (z^OOD_RPT)^rg and the block power z^(first row of the block) are applied once
+// per thread / once per block. All three power tables are filled once per call by ood_pow_kernel: built per block, their
+// ext_pow chains cost about as many instructions as the block's coefficient loop and held its loads back behind a
+// barrier. partial[col][chunk][point] = sum_{m in chunk} a_m z^m.
 #define OOD_RPT 64
 #define OOD_ROWS_PER_BLOCK (32 * OOD_RPT)
+#define OOD_TAB (OOD_RPT + 32)   // per point: z^r (r < OOD_RPT), then z^(OOD_RPT * rg) (rg < 32)
 template <int D>
-__global__ void ood_pow_kernel(GlExt<D> z0, GlExt<D> z1, u32 chunks, u64* zb /*[2][chunks][D]*/) {
+__global__ void ood_pow_kernel(GlExt<D> z0, GlExt<D> z1, u32 chunks, u64* zb /*[2][chunks][D]*/, u64* zt /*[2][OOD_TAB][D]*/) {
     const u32 idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= 2 * chunks) return;
-    const u32 pt = idx / chunks, c = idx % chunks;
-    const GlExt<D> v = ext_pow(pt ? z1 : z0, (u64)c * OOD_ROWS_PER_BLOCK);
+    if (idx < 2 * chunks) {
+        const u32 pt = idx / chunks, c = idx % chunks;
+        const GlExt<D> v = ext_pow(pt ? z1 : z0, (u64)c * OOD_ROWS_PER_BLOCK);
 #pragma unroll
-    for (int d = 0; d < D; d++) zb[(size_t)idx * D + d] = v.v[d];
+        for (int d = 0; d < D; d++) zb[(size_t)idx * D + d] = v.v[d];
+    } else if (idx < 2 * chunks + 2 * OOD_TAB) {
+        const u32 u = idx - 2 * chunks, pt = u / OOD_TAB, r = u % OOD_TAB;
+        const GlExt<D> v = ext_pow(pt ? z1 : z0, r < OOD_RPT ? r : (u64)(r - OOD_RPT) * OOD_RPT);
+#pragma unroll
+        for (int d = 0; d < D; d++) zt[(size_t)u * D + d] = v.v[d];
+    }
 }
 template <int D>
-__global__ void __launch_bounds__(256) ood_partial_kernel(SegMatrix polys, GlExt<D> z0, GlExt<D> z1, const u64* zb,
+__global__ void __launch_bounds__(256) ood_partial_kernel(SegMatrix polys, const u64* zt, const u64* zb,
                                                           u64* partial /*[cols][chunks][2][D]*/, u32 chunks) {
     const u32 g = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x;
     const int W = polys.W;
     const size_t n = polys.rows;
     const u64* base = polys.base + (size_t)g * polys.seg_stride;
-    __shared__ u64 zpow[2][OOD_RPT][D];   // z^r
-    __shared__ u64 zrg[2][32][D];         // z^(OOD_RPT * rg)
+    __shared__ u64 tab[2][OOD_TAB][D];
     __shared__ u64 red[2][32][8][D];
-    if (t < 2 * OOD_RPT) {
-        const GlExt<D> v = ext_pow(t < OOD_RPT ? z0 : z1, t % OOD_RPT);
-#pragma unroll
-        for (int d = 0; d < D; d++) zpow[t / OOD_RPT][t % OOD_RPT][d] = v.v[d];
-    } else if (t < 2 * OOD_RPT + 64) {
-        const u32 u = t - 2 * OOD_RPT, pt = u / 32, rg = u % 32;
-        const GlExt<D> v = ext_pow(pt ? z1 : z0, (u64)rg * OOD_RPT);
-#pragma unroll
-        for (int d = 0; d < D; d++) zrg[pt][rg][d] = v.v[d];
-    }
+    auto zpow = [&](u32 pt, u32 r) -> const u64* { return tab[pt][r]; };                // z^r
+    auto zrg = [&](u32 pt, u32 rg) -> const u64* { return tab[pt][OOD_RPT + rg]; };    // z^(OOD_RPT * rg)
+    for (u32 i = t; i < 2 * OOD_TAB * D; i += 256) (&tab[0][0][0])[i] = zt[i];
     __syncthreads();
     const u32 rg = t >> 3, lane = t & 7;
     const size_t start = (size_t)chunk * OOD_ROWS_PER_BLOCK + (size_t)rg * OOD_RPT;
@@ -213,17 +213,26 @@ __global__ void __launch_bounds__(256) ood_partial_kernel(SegMatrix polys, GlExt
         for (int d = 0; d < D; d++) acc[pt][d] = acc_zero();
     if (lane < (u32)W) {
         const u64* src = base + start * W + lane;
+        // the next 8 coefficients are requested before this 8's products: loaded in the step that consumes them, each load
+        // was issued right before its first product and the warp waited out a full memory latency per coefficient
+        u64 nx[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) nx[k] = (start + k < n) ? __ldg(src + (size_t)k * W) : 0;
 #pragma unroll 1
         for (int r0 = 0; r0 < OOD_RPT; r0 += 8) {
             u64 cf[8];
 #pragma unroll
-            for (int k = 0; k < 8; k++) cf[k] = (start + r0 + k < n) ? __ldg(src + (size_t)(r0 + k) * W) : 0;
+            for (int k = 0; k < 8; k++) cf[k] = nx[k];
+            if (r0 + 8 < OOD_RPT) {
+#pragma unroll
+                for (int k = 0; k < 8; k++) nx[k] = (start + r0 + 8 + k < n) ? __ldg(src + (size_t)(r0 + 8 + k) * W) : 0;
+            }
 #pragma unroll
             for (int k = 0; k < 8; k++) {
 #pragma unroll
                 for (int d = 0; d < D; d++) {
-                    acc_mad(acc[0][d], zpow[0][r0 + k][d], cf[k]);
-                    acc_mad(acc[1][d], zpow[1][r0 + k][d], cf[k]);
+                    acc_mad(acc[0][d], zpow(0, r0 + k)[d], cf[k]);
+                    acc_mad(acc[1][d], zpow(1, r0 + k)[d], cf[k]);
                 }
             }
         }
@@ -233,7 +242,7 @@ __global__ void __launch_bounds__(256) ood_partial_kernel(SegMatrix polys, GlExt
         GlExt<D> v;
 #pragma unroll
         for (int d = 0; d < D; d++) v.v[d] = acc_reduce(acc[pt][d]);
-        v = ext_mul(v, ld_ext<D>(&zrg[pt][rg][0]));
+        v = ext_mul(v, ld_ext<D>(zrg(pt, rg)));
 #pragma unroll
         for (int d = 0; d < D; d++) red[pt][rg][lane][d] = v.v[d];
     }
@@ -484,21 +493,36 @@ static bool deep_point(const GlExt<D>& z, DeepPoint<D>& pt) {
 // reference subtracts them, composer/mod.rs:202-210, and the remainder it then drops is zero).
 // The rows [u, v) map q_(v-1) to q_(u-1) = a + p q_(v-1), a = sum_{k in [u, v)} s_k b^(k-u), p = b^(v-u); adjacent runs L = [u, v)
 // and R = [v, w) compose to (a_L + p_L a_R, p_L p_R). The recurrence is a suffix scan of these runs, in the three-launch shape of
-// auxbuild.cu's prefix scans, both points in the same launches:
-//   syn_div_reduce  per tile of SYN_TILE rows: the a of the tile's run (its p is b^SYN_TILE);
-//   syn_div_carry   one block: exclusive suffix scan of the tile runs = q at the top row of every tile;
-//   syn_div_apply   per tile: block-wide exclusive suffix scan with the tile's carry-in, then the recurrence down each thread's
-//                   SYN_ITEMS rows, q_z + q_zg written in place.
+// auxbuild.cu's prefix scans, both points in the same launches. Inside a tile every run has a known length, so its p is a known
+// power of b and only the a's are scanned: combining two runs is one extension product by a power that is constant per scan level.
+//   syn_div_reduce  per tile of SYN_TILE rows: each thread's run a over its SYN_ITEMS rows (Horner), a warp suffix scan of those
+//                   (level k multiplies by b^(8·2^k)), a suffix scan of the 8 warp totals; it keeps, per thread, the a of the
+//                   rest of its warp above it and, per warp, the a of the warps above it, and writes the tile's a (p = b^SYN_TILE);
+//   syn_div_carry   one block: exclusive suffix scan of the tile runs = q at the top row of every tile; it also fills the table
+//                   b^(8k), k < 32, and b^(256 j), j < 8, that apply reads;
+//   syn_div_apply   per tile: q at the top row of each warp from the kept warp suffix and the carry (one lane, then shuffled to
+//                   the warp), q at each thread's top row from the kept in-warp suffix, then the recurrence down the thread's
+//                   SYN_ITEMS rows, q_z + q_zg written in place. No run is computed twice.
 // Rows >= n read as zero, which changes no q (q_(n-1) = 0 either way). Field arithmetic is exact, so the association order of the
 // scan changes no bit, and the LDE of the quotient equals deep_div_kernel's rows.
 #define SYN_THREADS 256
 #define SYN_ITEMS 8
 #define SYN_TILE (SYN_THREADS * SYN_ITEMS)
+#define SYN_WARPS (SYN_THREADS / 32)
+#define SYN_PW (32 + SYN_WARPS)   // table per point: b^(SYN_ITEMS k), k < 32, then b^(32 SYN_ITEMS j), j < SYN_WARPS
 template <int D>
 struct SynDivParams {
     GlExt<D> b[2];        // z, zg
     GlExt<D> b_items[2];  // b^SYN_ITEMS
     GlExt<D> b_tile[2];   // b^SYN_TILE
+    GlExt<D> lvl[2][8];   // b^(SYN_ITEMS 2^k): k < 5 for the warp scan levels, 5..7 for the scan over the warps
+};
+// scratch of one division, in one allocation of (tiles (1 + SYN_WARPS + SYN_THREADS) + SYN_PW) 2 D words
+struct SynDivBufs {
+    u64* agg;   // [tiles][2][D]: tile run a, then (after syn_div_carry) q at the tile's top row
+    u64* wsuf;  // [tiles][SYN_WARPS][2][D]: a of the warps above this one in its tile
+    u64* tsuf;  // [tiles][SYN_THREADS][2][D]: a of the threads above this one in its warp
+    u64* pw;    // [2][SYN_PW][D]
 };
 template <int D>
 struct SynRun {  // x -> a + p x for each point
@@ -588,35 +612,78 @@ __device__ __forceinline__ void syn_st(u64* m, size_t i, const GlExt<D>& v) {
         o[1] = make_ulonglong2(v.v[2], 0);
     }
 }
-// the run of this thread's rows [r0, r0 + SYN_ITEMS): a by Horner from the top row down
+// this thread's run a over its rows [r0, r0 + SYN_ITEMS), both points, by Horner from the top row down (its p is b^SYN_ITEMS)
 template <int D>
-__device__ __forceinline__ SynRun<D> syn_thread_run(const u64* m, size_t n, size_t r0, const SynDivParams<D>& sp) {
-    SynRun<D> r;
+__device__ __forceinline__ void syn_thread_run(const u64* m, size_t n, size_t r0, const SynDivParams<D>& sp, GlExt<D> a[2]) {
 #pragma unroll
-    for (int pt = 0; pt < 2; pt++) { r.a[pt] = ext_zero<D>(); r.p[pt] = sp.b_items[pt]; }
+    for (int pt = 0; pt < 2; pt++) a[pt] = ext_zero<D>();
 #pragma unroll
     for (int k = SYN_ITEMS - 1; k >= 0; k--) {
         const GlExt<D> s = r0 + k < n ? syn_ld<D>(m, r0 + k) : ext_zero<D>();
 #pragma unroll
-        for (int pt = 0; pt < 2; pt++) r.a[pt] = ext_add(s, ext_mul(sp.b[pt], r.a[pt]));
+        for (int pt = 0; pt < 2; pt++) a[pt] = ext_add(s, ext_mul(sp.b[pt], a[pt]));
     }
+}
+template <int D>
+__device__ __forceinline__ GlExt<D> syn_shfl_ext(const GlExt<D>& v, u32 off) {
+    GlExt<D> r;
+#pragma unroll
+    for (int q = 0; q < D; q++) r.v[q] = __shfl_down_sync(0xffffffffu, v.v[q], off);
     return r;
 }
 template <int D>
-__global__ void __launch_bounds__(SYN_THREADS) syn_div_reduce(const u64* s, size_t n, SynDivParams<D> sp, u64* agg /*[tiles][2][D]*/) {
-    const size_t r0 = (size_t)blockIdx.x * SYN_TILE + (size_t)threadIdx.x * SYN_ITEMS;
-    SynRun<D> total;
-    syn_block_suffix<D>(syn_thread_run<D>(s, n, r0, sp), total);
-    if (threadIdx.x == 0) {
+__device__ __forceinline__ void syn_st_ext(u64* p, const GlExt<D>& v) {
 #pragma unroll
-        for (int pt = 0; pt < 2; pt++)
+    for (int q = 0; q < D; q++) p[q] = v.v[q];
+}
+template <int D>
+__global__ void __launch_bounds__(SYN_THREADS) syn_div_reduce(const u64* s, size_t n, SynDivParams<D> sp, SynDivBufs bufs) {
+    __shared__ GlExt<D> wtot[2][SYN_WARPS];
+    const u32 t = threadIdx.x, lane = t & 31, wid = t >> 5;
+    const size_t tile = blockIdx.x, r0 = tile * SYN_TILE + (size_t)t * SYN_ITEMS;
+    GlExt<D> x[2];
+    syn_thread_run<D>(s, n, r0, sp, x);
+    // inclusive suffix over the warp: x = a of the rows of lanes lane..31. Where level k combines, x covers exactly 2^k lanes.
 #pragma unroll
-            for (int q = 0; q < D; q++) agg[((size_t)blockIdx.x * 2 + pt) * D + q] = total.a[pt].v[q];
+    for (int k = 0; k < 5; k++) {
+#pragma unroll
+        for (int pt = 0; pt < 2; pt++) {
+            const GlExt<D> y = syn_shfl_ext(x[pt], 1u << k);
+            if (lane + (1u << k) < 32) x[pt] = ext_add(x[pt], ext_mul(sp.lvl[pt][k], y));
+        }
+    }
+    u64* ts = bufs.tsuf + (tile * SYN_THREADS + t) * 2 * D;
+#pragma unroll
+    for (int pt = 0; pt < 2; pt++) {
+        GlExt<D> ex = syn_shfl_ext(x[pt], 1);   // the lanes above this one
+        if (lane == 31) ex = ext_zero<D>();
+        syn_st_ext(ts + pt * D, ex);
+        if (lane == 0) wtot[pt][wid] = x[pt];
+    }
+    __syncthreads();
+    if (wid == 0) {   // the same over the warp totals
+#pragma unroll
+        for (int pt = 0; pt < 2; pt++) {
+            GlExt<D> w = lane < SYN_WARPS ? wtot[pt][lane] : ext_zero<D>();
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                const GlExt<D> y = syn_shfl_ext(w, 1u << k);
+                if (lane + (1u << k) < SYN_WARPS) w = ext_add(w, ext_mul(sp.lvl[pt][5 + k], y));
+            }
+            GlExt<D> ex = syn_shfl_ext(w, 1);   // the warps above
+            if (lane + 1 >= SYN_WARPS) ex = ext_zero<D>();
+            if (lane < SYN_WARPS) syn_st_ext(bufs.wsuf + ((tile * SYN_WARPS + lane) * 2 + pt) * D, ex);
+            if (lane == 0) syn_st_ext(bufs.agg + (tile * 2 + pt) * D, w);
+        }
     }
 }
 // one block; tile runs -> carry-in of every tile (q at its top row), in place. Thread t owns a run of consecutive tiles.
 template <int D>
-__global__ void __launch_bounds__(SYN_THREADS) syn_div_carry(u64* agg, size_t ntiles, SynDivParams<D> sp) {
+__global__ void __launch_bounds__(SYN_THREADS) syn_div_carry(u64* agg, size_t ntiles, SynDivParams<D> sp, u64* pw) {
+    if (threadIdx.x < 2 * SYN_PW) {   // apply's power table
+        const u32 pt = threadIdx.x / SYN_PW, j = threadIdx.x % SYN_PW;
+        syn_st_ext(pw + (size_t)threadIdx.x * D, ext_pow(pt ? sp.b_items[1] : sp.b_items[0], j < 32 ? j : 32 * (j - 32)));
+    }
     const size_t per = (ntiles + SYN_THREADS - 1) / SYN_THREADS;
     const size_t b = threadIdx.x * per < ntiles ? threadIdx.x * per : ntiles, e = b + per < ntiles ? b + per : ntiles;
     SynRun<D> mine;
@@ -644,18 +711,27 @@ __global__ void __launch_bounds__(SYN_THREADS) syn_div_carry(u64* agg, size_t nt
     }
 }
 template <int D>
-__global__ void __launch_bounds__(SYN_THREADS) syn_div_apply(u64* s, size_t n, SynDivParams<D> sp, const u64* carry) {
-    const size_t r0 = (size_t)blockIdx.x * SYN_TILE + (size_t)threadIdx.x * SYN_ITEMS;
-    SynRun<D> total;
-    const SynRun<D> above = syn_block_suffix<D>(syn_thread_run<D>(s, n, r0, sp), total);
+__global__ void __launch_bounds__(SYN_THREADS) syn_div_apply(u64* s, size_t n, SynDivParams<D> sp, SynDivBufs bufs) {
+    const u32 t = threadIdx.x, lane = t & 31, wid = t >> 5;
+    const size_t tile = blockIdx.x, r0 = tile * SYN_TILE + (size_t)t * SYN_ITEMS;
     GlExt<D> q[2];  // q at row r0 + SYN_ITEMS - 1
 #pragma unroll
-    for (int pt = 0; pt < 2; pt++) q[pt] = ext_add(above.a[pt], ext_mul(above.p[pt], ld_ext<D>(carry + ((size_t)blockIdx.x * 2 + pt) * D)));
+    for (int pt = 0; pt < 2; pt++) {
+        const u64* pw = bufs.pw + (size_t)pt * SYN_PW * D;
+        // q at the top row of this warp's rows: the warps above it in the tile, then the tile's carry-in (one lane computes it)
+        GlExt<D> zw = ext_zero<D>();
+        if (lane == 0)
+            zw = ext_add(ld_ext<D>(bufs.wsuf + ((tile * SYN_WARPS + wid) * 2 + pt) * D),
+                         ext_mul(ld_ext<D>(pw + (32 + SYN_WARPS - 1 - wid) * D), ld_ext<D>(bufs.agg + (tile * 2 + pt) * D)));
+#pragma unroll
+        for (int c = 0; c < D; c++) zw.v[c] = __shfl_sync(0xffffffffu, zw.v[c], 0);
+        q[pt] = ext_add(ld_ext<D>(bufs.tsuf + ((tile * SYN_THREADS + t) * 2 + pt) * D), ext_mul(ld_ext<D>(pw + (31 - lane) * D), zw));
+    }
 #pragma unroll
     for (int k = SYN_ITEMS - 1; k >= 0; k--) {
         const size_t i = r0 + k;
         if (i >= n) continue;
-        const GlExt<D> si = syn_ld<D>(s, i);  // read before the row is overwritten
+        const GlExt<D> si = syn_ld<D>(s, i);
         syn_st<D>(s, i, ext_add(q[0], q[1]));
 #pragma unroll
         for (int pt = 0; pt < 2; pt++) q[pt] = ext_add(si, ext_mul(sp.b[pt], q[pt]));
@@ -781,9 +857,10 @@ int ood_eval(wf_ctx* ctx, const std::vector<const wf_mat*>& mats, const GlExt<D>
         const u32 chunks = (u32)((n + OOD_ROWS_PER_BLOCK - 1) / OOD_ROWS_PER_BLOCK);
         const u32 cols = mats[m]->m.cols;
         CKI(tmp.alloc((size_t)cols * chunks * 2 * D * 8, &part[m]));
-        CKI(tmp.alloc((size_t)2 * chunks * D * 8, &zbs[m]));
-        ood_pow_kernel<D><<<(2 * chunks + 127) / 128, 128, 0, ctx->st>>>(z0, z1, chunks, (u64*)zbs[m]);
-        ood_partial_kernel<D><<<dim3(chunks, mats[m]->m.nseg()), 256, 0, ctx->st>>>(mats[m]->m, z0, z1, (const u64*)zbs[m], (u64*)part[m], chunks);
+        CKI(tmp.alloc((size_t)2 * (chunks + OOD_TAB) * D * 8, &zbs[m]));
+        u64* zt = (u64*)zbs[m] + (size_t)2 * chunks * D;
+        ood_pow_kernel<D><<<(2 * (chunks + OOD_TAB) + 127) / 128, 128, 0, ctx->st>>>(z0, z1, chunks, (u64*)zbs[m], zt);
+        ood_partial_kernel<D><<<dim3(chunks, mats[m]->m.nseg()), 256, 0, ctx->st>>>(mats[m]->m, zt, (const u64*)zbs[m], (u64*)part[m], chunks);
         ood_reduce_kernel<D><<<(2 * cols * 32 + 255) / 256, 256, 0, ctx->st>>>((const u64*)part[m], cols, chunks, (u64*)res + off);
         ctx->launches += 3;
         CK(cudaGetLastError());
@@ -1210,7 +1287,12 @@ int deep_compose_polys(wf_ctx* ctx, const wf_mat* polys, const wf_mat* apolys, c
     CKI(upload_ext<D>(ctx, dc, 0, ct + kc, &d_dt));
     tmp.bufs.push_back(d_dt);
     void* d_agg;
-    CKI(tmp.alloc(ntiles * 2 * D * 8, &d_agg));
+    CKI(tmp.alloc((ntiles * (1 + SYN_WARPS + SYN_THREADS) + SYN_PW) * 2 * D * 8, &d_agg));
+    SynDivBufs sb;
+    sb.agg = (u64*)d_agg;
+    sb.wsuf = sb.agg + ntiles * 2 * D;
+    sb.tsuf = sb.wsuf + ntiles * SYN_WARPS * 2 * D;
+    sb.pw = sb.tsuf + ntiles * SYN_THREADS * 2 * D;
     wf_mat* quot;
     CKI(wf_mat_alloc(ctx, n, D, &quot));
     DeepParams p{};
@@ -1220,10 +1302,15 @@ int deep_compose_polys(wf_ctx* ctx, const wf_mat* polys, const wf_mat* apolys, c
     deep_sum_kernel<D><<<(unsigned)((n + DEEP_SUM_THREADS - 1) / DEEP_SUM_THREADS), DEEP_SUM_THREADS, (size_t)(ct + kc) * D * 8, ctx->st>>>(p);
     SynDivParams<D> sp;
     sp.b[0] = z; sp.b[1] = zg;
-    for (int pt = 0; pt < 2; pt++) { sp.b_items[pt] = ext_pow(sp.b[pt], SYN_ITEMS); sp.b_tile[pt] = ext_pow(sp.b[pt], SYN_TILE); }
-    syn_div_reduce<D><<<(unsigned)ntiles, SYN_THREADS, 0, ctx->st>>>(quot->m.base, n, sp, (u64*)d_agg);
-    syn_div_carry<D><<<1, SYN_THREADS, 0, ctx->st>>>((u64*)d_agg, ntiles, sp);
-    syn_div_apply<D><<<(unsigned)ntiles, SYN_THREADS, 0, ctx->st>>>(quot->m.base, n, sp, (const u64*)d_agg);
+    for (int pt = 0; pt < 2; pt++) {
+        sp.b_items[pt] = ext_pow(sp.b[pt], SYN_ITEMS);
+        sp.b_tile[pt] = ext_pow(sp.b[pt], SYN_TILE);
+        sp.lvl[pt][0] = sp.b_items[pt];
+        for (int k = 1; k < 8; k++) sp.lvl[pt][k] = ext_mul(sp.lvl[pt][k - 1], sp.lvl[pt][k - 1]);
+    }
+    syn_div_reduce<D><<<(unsigned)ntiles, SYN_THREADS, 0, ctx->st>>>(quot->m.base, n, sp, sb);
+    syn_div_carry<D><<<1, SYN_THREADS, 0, ctx->st>>>(sb.agg, ntiles, sp, sb.pw);
+    syn_div_apply<D><<<(unsigned)ntiles, SYN_THREADS, 0, ctx->st>>>(quot->m.base, n, sp, sb);
     ctx->launches += 4;
     const cudaError_t e = cudaGetLastError();
     // the quotient and the scratch go back to the pool in stream order, behind the LDE that reads them
@@ -1400,7 +1487,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     // ---- 6. FRI (lib.rs:442-448) ----
     {   // transcript replicated on the device: one synchronisation for the whole commit phase (capi.cu)
         std::vector<Digest> fri_roots;
-        CKI(wf_fri_build_layers_coin(ctx, h, deep, D, o.folding, o.rem_max_deg, o.blowup, ch.coin, fri_roots, &fri));
+        CKI(wf_fri_build_layers_coin(ctx, h, deep, D, o.folding, o.rem_max_deg, o.blowup, ch.coin, fri_roots, &fri, deep));
         for (auto& r : fri_roots) ch.commitments.bytes(r.b, WF_DIGEST_BYTES(h));
     }
     scope.drop(deep);
