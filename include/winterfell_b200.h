@@ -165,6 +165,44 @@ size_t wf_fri_remainder(const wf_fri* f, uint64_t* coeffs, size_t cap_words);
 int wf_fri_build_proof(wf_ctx* ctx, wf_fri* f, const uint64_t* positions, size_t k, uint8_t* out, size_t* len);
 int wf_fri_free(wf_ctx* ctx, wf_fri* f);
 
+/* ---- verifying standalone FRI proofs (FriVerifier, fri/src/verifier/mod.rs:107-331) ------------------------------------
+ * verdicts[j] is the FIRST error FriVerifier::new and then verify return for proof j, in the reference's order: the
+ * deserialization of DefaultVerifierChannel::new, new()'s draws and DegreeTruncation checks, then per layer the opening
+ * (LayerCommitmentMismatch) and InvalidLayerFolding, then RemainderDegreeMismatch and InvalidRemainderFolding. The codes
+ * are the fri::VerifierError variants the verifier returns; INVALID_LAYER_FOLDING and DEGREE_TRUNCATION carry their layer
+ * in bits 8 and up (WF_FRI_VERIFY_LAYER). The remainder commitment is never compared with the remainder (read_remainder,
+ * fri/src/verifier/channel.rs:112-116): it only reseeds the coin. */
+#define WF_FRI_VERIFY_ACCEPT                     0
+#define WF_FRI_VERIFY_MALFORMED                  1   /* DeserializationError, a layer missing from the proof, or layer indexes
+                                                        (map_positions_to_indexes) that repeat or leave the layer's tree */
+#define WF_FRI_VERIFY_LAYER_COMMITMENT_MISMATCH  2   /* LayerCommitmentMismatch */
+#define WF_FRI_VERIFY_INVALID_LAYER_FOLDING      3   /* InvalidLayerFolding(layer); layer 0: the caller's evaluations */
+#define WF_FRI_VERIFY_REMAINDER_DEGREE_MISMATCH  4   /* RemainderDegreeMismatch */
+#define WF_FRI_VERIFY_INVALID_REMAINDER_FOLDING  5   /* InvalidRemainderFolding */
+#define WF_FRI_VERIFY_DEGREE_TRUNCATION          6   /* DegreeTruncation(.., folding, layer) */
+#define WF_FRI_VERIFY_RANDOM_COIN                7   /* RandomCoinError: no alpha in 1000 draws */
+#define WF_FRI_VERIFY_CODE(v)  ((v) & 0xffu)
+#define WF_FRI_VERIFY_LAYER(v) ((v) >> 8)
+/* FriVerifier::new + verify with DefaultVerifierChannel (fri/src/verifier/channel.rs) for `batch` proofs of one shape:
+ * hasher, extension degree (1, 2, 3), FriOptions(blowup, folding_factor, remainder_max_degree) and max_poly_degree; the
+ * domain is max_poly_degree.next_power_of_two() * blowup (at most 2^32), offset 7. Per proof j: proofs[j] (proof_lens[j]
+ * bytes) holds the serialized FriProof and nothing after it; commitments[j] holds num_commitments[j] x 32 bytes, the layer
+ * roots then the remainder commitment as wf_fri_build_layers_default_channel writes them (num_layers + 1 of them);
+ * coin_seeds[j] is the 32-byte seed of the public coin when FriVerifier::new starts reseeding it (coin_seeds NULL, or a NULL
+ * entry: DefaultRandomCoin::new(&[])); positions[j] and evaluations[j] hold the num_queries[j] query positions and the
+ * values at them, [k][ext] canonical words. The proof's num_partitions is honoured (map_positions_to_indexes,
+ * fri/src/utils.rs:9-33). WF_ERR_INVALID for caller errors (NULL pointers, a shape with a layer of fewer than two rows or
+ * no remainder, a commitment count other than num_layers + 1, a non-canonical evaluation, a position outside the domain),
+ * naming the proof; WF_ERR_UNSUPPORTED for a folding factor other than 2, 4, 8 or 16 or an unknown hash. A refused proof
+ * is a result: the call returns WF_OK whenever verdicts were written. No device buffer stays live after any return. The
+ * host parses and plans without hashing; the device checks the whole batch together, and the number of kernel launches
+ * does not depend on `batch` for proofs of one shape. */
+int wf_fri_verify_batch(wf_ctx* ctx, int hash_id, int ext_degree, uint32_t folding_factor, uint32_t remainder_max_degree,
+                        uint32_t blowup, uint64_t max_poly_degree, uint32_t batch, const uint8_t* const* proofs,
+                        const size_t* proof_lens, const uint8_t* const* commitments, const uint32_t* num_commitments,
+                        const uint8_t* const* coin_seeds, const uint64_t* const* positions,
+                        const uint64_t* const* evaluations, const size_t* num_queries, uint32_t* verdicts);
+
 /* ---- full proof (Prover::prove / generate_proof, prover/src/lib.rs:250-492) --------------------- */
 /* Proves the built-in AIR family "FibSmall x k" (k copies of examples/src/fibonacci/fib_small/air.rs
  * side by side, trace width 2k; k = 1 is the reference's fib_small example) and writes the

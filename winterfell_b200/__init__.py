@@ -35,6 +35,21 @@ AUX_ASSERTIONS_BATCH = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, u64p, u64p)
 VERIFY_ACCEPT, VERIFY_MALFORMED, VERIFY_OOD, VERIFY_POW, VERIFY_TRACE_QUERY, VERIFY_CONSTRAINT_QUERY, VERIFY_FRI_LAYER, \
     VERIFY_FRI_FOLD, VERIFY_FRI_REMAINDER, VERIFY_CONTEXT, VERIFY_UNACCEPTABLE_OPTIONS = range(11)
 
+# wf_fri_verify_batch verdicts (include/winterfell_b200.h WF_FRI_VERIFY_*); INVALID_LAYER_FOLDING and DEGREE_TRUNCATION carry
+# their layer in bits 8 and up (fri_verdict_layer)
+FRI_VERIFY_ACCEPT, FRI_VERIFY_MALFORMED, FRI_VERIFY_LAYER_COMMITMENT_MISMATCH, FRI_VERIFY_INVALID_LAYER_FOLDING, \
+    FRI_VERIFY_REMAINDER_DEGREE_MISMATCH, FRI_VERIFY_INVALID_REMAINDER_FOLDING, FRI_VERIFY_DEGREE_TRUNCATION, \
+    FRI_VERIFY_RANDOM_COIN = range(8)
+
+
+def fri_verdict_code(v):
+    return int(v) & 0xFF
+
+
+def fri_verdict_layer(v):
+    return int(v) >> 8
+
+
 # wf_validation (include/winterfell_b200.h): the first violation wf_trace_validate found, in the reference's order
 VALID, VIOLATION_MAIN_ASSERTION, VIOLATION_AUX_ASSERTION, VIOLATION_MAIN_TRANSITION, VIOLATION_AUX_TRANSITION, VIOLATION_DEGREES, \
     VIOLATION_CE_DOMAIN = range(7)
@@ -98,6 +113,9 @@ _SIGS = [
     ("wf_fri_remainder", C.c_size_t, [vp, u64p, C.c_size_t]),
     ("wf_fri_build_proof", C.c_int, [vp, vp, u64p, C.c_size_t, u8p, C.POINTER(C.c_size_t)]),
     ("wf_fri_free", C.c_int, [vp, vp]),
+    ("wf_fri_verify_batch", C.c_int, [vp, C.c_int, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint32, C.POINTER(u8p),
+                                      C.POINTER(C.c_size_t), C.POINTER(u8p), C.POINTER(C.c_uint32), C.POINTER(u8p), C.POINTER(u64p),
+                                      C.POINTER(u64p), C.POINTER(C.c_size_t), C.POINTER(C.c_uint32)]),
     ("wf_prove_fib", C.c_int, [vp, C.POINTER(u64p), C.c_int, C.c_uint32, C.c_uint32, u64p, C.POINTER(C.c_uint32), u8p, C.POINTER(C.c_size_t)]),
     ("wf_prove_air", C.c_int, [vp, u64p, C.c_size_t, C.POINTER(u64p), C.c_int, C.c_uint32, C.POINTER(C.c_uint32), u8p, C.POINTER(C.c_size_t)]),
     ("wf_prove_air_aux", C.c_int, [vp, u64p, C.c_size_t, C.POINTER(u64p), C.c_int, C.c_uint32, C.POINTER(C.c_uint32), AUX_BUILDER, vp,
@@ -603,6 +621,39 @@ class Context:
         self.check(self.L.wf_verify_air_batch(self.h, batch, dps, dls, pps, pls, int(hash_id), accp, nacc, cb, None,
                                               out.ctypes.data_as(C.POINTER(C.c_uint32))))
         return out
+
+    def fri_verify_batch(self, hash_id, ext, folding, rem_max_deg, blowup, max_poly_degree, proofs, commitments, positions,
+                         evaluations, coin_seeds=None):
+        """wf_fri_verify_batch: the verdict (FRI_VERIFY_*, layer in bits 8 and up) of each FriProof in `proofs` (bytes), all of
+        one shape. Per proof: commitments [num_layers + 1, 32] uint8 (layer roots, then the remainder's), positions (k ints) and
+        evaluations [k, ext] canonical words; coin_seeds: None, or per proof None or the coin's 32-byte seed. Returns a list."""
+        batch = len(proofs)
+        if not (len(commitments) == len(positions) == len(evaluations) == batch) or (coin_seeds is not None and len(coin_seeds) != batch):
+            raise ValueError("one set of commitments, positions, evaluations (and coin seed) per proof")
+        ps = [np.frombuffer(p, dtype=np.uint8) if len(p) else np.zeros(1, dtype=np.uint8) for p in proofs]
+        cs = [np.ascontiguousarray(np.asarray(c, dtype=np.uint8).reshape(-1, 32)) for c in commitments]
+        qs = [np.ascontiguousarray(np.asarray(q, dtype=np.uint64).reshape(-1)) for q in positions]
+        es = [np.ascontiguousarray(np.asarray(e, dtype=np.uint64).reshape(-1)) for e in evaluations]
+        ss = None
+        if coin_seeds is not None:
+            ss = [None if s is None else np.frombuffer(bytes(s), dtype=np.uint8) for s in coin_seeds]
+            if any(s is not None and s.size != 32 for s in ss):
+                raise ValueError("a coin seed is 32 bytes")
+        for q, e in zip(qs, es):
+            if e.size != q.size * ext:
+                raise ValueError("evaluations must be [k, ext] for k positions")
+        pps = (u8p * batch)(*[p.ctypes.data_as(u8p) for p in ps])
+        pls = (C.c_size_t * batch)(*[len(p) for p in proofs])
+        cps = (u8p * batch)(*[c.ctypes.data_as(u8p) for c in cs])
+        cns = (C.c_uint32 * batch)(*[c.shape[0] for c in cs])
+        sps = None if ss is None else (u8p * batch)(*[None if s is None else s.ctypes.data_as(u8p) for s in ss])
+        qps = (u64p * batch)(*[q.ctypes.data_as(u64p) for q in qs])
+        eps = (u64p * batch)(*[e.ctypes.data_as(u64p) for e in es])
+        nqs = (C.c_size_t * batch)(*[q.size for q in qs])
+        out = np.zeros(batch, dtype=np.uint32)
+        self.check(self.L.wf_fri_verify_batch(self.h, int(hash_id), int(ext), folding, rem_max_deg, blowup, int(max_poly_degree), batch,
+                                              pps, pls, cps, cns, sps, qps, eps, nqs, out.ctypes.data_as(C.POINTER(C.c_uint32))))
+        return [int(v) for v in out]
 
     def trace_validate(self, desc, trace, ext=1, rand=None, aux=None, aux_build=None, n=None, mont=False, check_degrees=True):
         """wf_trace_validate: checks a trace against its AIR as the reference's debug builds do (Trace::validate, then

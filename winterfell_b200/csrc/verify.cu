@@ -1,4 +1,7 @@
-// verify.cu — verifier::verify (verifier/src/lib.rs:82-260) for a batch of proofs of one AIR (wf_verify_air_batch).
+// verify.cu — verifier::verify (verifier/src/lib.rs:82-260) for a batch of proofs of one AIR (wf_verify_air_batch), and
+// FriVerifier::new + verify (fri/src/verifier/mod.rs:107-331) for a batch of standalone FRI proofs of one shape
+// (wf_fri_verify_batch). Both share the FRI part: the FriProof parser, the query-phase plan (plan_fri), the device records
+// and kernels, and the batch runner (run_plan).
 //
 // Host, per proof in batch order: parse the proof bytes (the inverse of prove_air's writer), check the options against the
 // acceptable set, check the AIR at the trace length the proof declares, replay the transcript (PublicCoin), check the OOD
@@ -8,7 +11,8 @@
 // the DEEP composition at the queries, one FRI launch per depth, the remainder and the verdicts.
 //
 // A proof's verdict is its FIRST failed check in the reference's order. Every check that fails writes (rank << 4 | code) with
-// atomicMin into the proof's word; ranks follow the order of the checks, codes are WF_VERIFY_*. A check the host can decide
+// atomicMin into the proof's word; ranks follow the order of the checks, codes are WF_VERIFY_* (WF_FRI_VERIFY_* for the
+// standalone FRI verifier). A check the host can decide
 // (a malformed opening, a position map that does not fit) seeds that word and ends the plan of the proof there: the device
 // still runs the proof's earlier checks, which win when they fail.
 #include <cstring>
@@ -131,7 +135,7 @@ constexpr __device__ u32 cbrev_v(u32 v, int bits) {
 // (fri.cu fri_fold_kernel), x = 7 w_dom^fpos.
 template <int D, int LOGNF>
 __device__ void fold_one(const ProofDev& pd, const u64* __restrict__ up, const FoldItem& it, const CheckItem* __restrict__ chk,
-                         u64* __restrict__ evals, u32* fail) {
+                         u64* __restrict__ evals, u32* fail, u32 code) {
     constexpr int NF = 1 << LOGNF;
     u64 x[D][NF];
 #pragma unroll
@@ -142,7 +146,7 @@ __device__ void fold_one(const ProofDev& pd, const u64* __restrict__ up, const F
         const CheckItem ck = chk[it.chk0 + q];
         bool e = true;
         for (int c = 0; c < D; c++) e = e && up[it.off + (size_t)(ck.col * D + c) * it.stride] == evals[(size_t)ck.cur * 3 + c];
-        if (!e) atomicMin(fail + pd.slot, fail_word(fri_layer_rank(it.depth) + 1, WF_VERIFY_FRI_FOLD));
+        if (!e) atomicMin(fail + pd.slot, fail_word(fri_layer_rank(it.depth) + 1, code));
     }
 #pragma unroll
     for (int c = 0; c < D; c++) mini_dft<LOGNF>(x[c]);
@@ -161,47 +165,49 @@ __device__ void fold_one(const ProofDev& pd, const u64* __restrict__ up, const F
     st3<D>(evals + (size_t)it.out * 3, ext_mul_base(acc, GL_P - ((GL_P - 1) >> LOGNF)));
 }
 template <int D>
-__device__ void fold_d(const ProofDev& pd, const u64* up, const FoldItem& it, const CheckItem* chk, u64* evals, u32* fail) {
+__device__ void fold_d(const ProofDev& pd, const u64* up, const FoldItem& it, const CheckItem* chk, u64* evals, u32* fail, u32 code) {
     switch (it.nf_log) {
-        case 1: fold_one<D, 1>(pd, up, it, chk, evals, fail); break;
-        case 2: fold_one<D, 2>(pd, up, it, chk, evals, fail); break;
-        case 3: fold_one<D, 3>(pd, up, it, chk, evals, fail); break;
-        default: fold_one<D, 4>(pd, up, it, chk, evals, fail); break;
+        case 1: fold_one<D, 1>(pd, up, it, chk, evals, fail, code); break;
+        case 2: fold_one<D, 2>(pd, up, it, chk, evals, fail, code); break;
+        case 3: fold_one<D, 3>(pd, up, it, chk, evals, fail, code); break;
+        default: fold_one<D, 4>(pd, up, it, chk, evals, fail, code); break;
     }
 }
+// code: the verdict code of a row that does not carry the current evaluations (InvalidLayerFolding)
 __global__ void __launch_bounds__(128) verify_fri_kernel(const ProofDev* __restrict__ pds, const u64* __restrict__ up,
                                                          const FoldItem* __restrict__ items, u32 count, const CheckItem* __restrict__ chk,
-                                                         u64* __restrict__ evals, u32* fail) {
+                                                         u64* __restrict__ evals, u32* fail, u32 code) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
     const FoldItem it = items[i];
     const ProofDev pd = pds[it.proof];
     switch (pd.d) {
-        case 1: fold_d<1>(pd, up, it, chk, evals, fail); break;
-        case 2: fold_d<2>(pd, up, it, chk, evals, fail); break;
-        default: fold_d<3>(pd, up, it, chk, evals, fail); break;
+        case 1: fold_d<1>(pd, up, it, chk, evals, fail, code); break;
+        case 2: fold_d<2>(pd, up, it, chk, evals, fail, code); break;
+        default: fold_d<3>(pd, up, it, chk, evals, fail, code); break;
     }
 }
 
 // the remainder polynomial (reversed coefficients, eval_horner_rev) at each final position
 template <int D>
-__device__ void rem_one(const ProofDev& pd, const u64* up, const RemItem& it, const u64* evals, u32* fail) {
+__device__ void rem_one(const ProofDev& pd, const u64* up, const RemItem& it, const u64* evals, u32* fail, u32 code) {
     const u64 x = gl_mul(gl_pow(gl_root_of_unity(it.log_dom), it.pos), GL_GENERATOR);
     const u64* r = up + pd.cst + pd.r_off;
     GlExt<D> acc = ext_zero<D>();
     for (u32 j = 0; j < pd.rn; j++) acc = ext_add(ext_mul_base(acc, x), ld3<D>(r + 3 * j));
-    if (!eq3<D>(acc, evals + (size_t)it.cur * 3)) atomicMin(fail + pd.slot, fail_word(R_REMAINDER, WF_VERIFY_FRI_REMAINDER));
+    if (!eq3<D>(acc, evals + (size_t)it.cur * 3)) atomicMin(fail + pd.slot, fail_word(R_REMAINDER, code));
 }
+// code: the verdict code of a remainder that does not take the folded value (InvalidRemainderFolding)
 __global__ void verify_remainder_kernel(const ProofDev* __restrict__ pds, const u64* __restrict__ up, const RemItem* __restrict__ items,
-                                        u32 count, const u64* __restrict__ evals, u32* fail) {
+                                        u32 count, const u64* __restrict__ evals, u32* fail, u32 code) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
     const RemItem it = items[i];
     const ProofDev pd = pds[it.proof];
     switch (pd.d) {
-        case 1: rem_one<1>(pd, up, it, evals, fail); break;
-        case 2: rem_one<2>(pd, up, it, evals, fail); break;
-        default: rem_one<3>(pd, up, it, evals, fail); break;
+        case 1: rem_one<1>(pd, up, it, evals, fail, code); break;
+        case 2: rem_one<2>(pd, up, it, evals, fail, code); break;
+        default: rem_one<3>(pd, up, it, evals, fail, code); break;
     }
 }
 
@@ -263,14 +269,34 @@ bool all_canonical(const Bytes& b, size_t skip = 0) {
     }
     return true;
 }
+// FriProof (fri/src/proof.rs): per layer the queried rows and their batch opening, the remainder, num_partitions as a
+// power of two (proof.rs:36,101-103)
+struct FriBytes {
+    std::vector<Bytes> fv, fp;
+    Bytes rem;
+    u8 log_parts = 0;
+};
+// FriProof::read_from (proof.rs:166-179, 295-310) without the value checks: false when the bytes end early
+bool read_fri_proof(Reader& r, FriBytes& f) {
+    const u8 fl = r.u8_();
+    f.fv.resize(fl); f.fp.resize(fl);
+    for (u32 i = 0; i < fl; i++) {
+        f.fv[i].n = r.le(4); f.fv[i].p = r.take(f.fv[i].n);
+        if (!r.ok) return false;
+        f.fp[i].n = r.le(4); f.fp[i].p = r.take(f.fp[i].n);
+        if (!r.ok) return false;
+    }
+    f.rem.n = r.le(2); f.rem.p = r.take(f.rem.n);
+    f.log_parts = r.u8_();
+    return r.ok;
+}
 struct Parsed {
     u32 logn = 0;
     Options o{};
     u32 nuq = 0, nl = 0;
     std::vector<Digest> cm;       // commitments in 32-byte slots (Blake3_192 zero-padded, as ByteDigest::as_bytes)
-    Bytes tq_v, tq_p, aq_v, aq_p, cq_v, cq_p, ood_t, ood_q, rem;
-    std::vector<Bytes> fv, fp;
-    u8 fri_log_parts = 0;
+    Bytes tq_v, tq_p, aq_v, aq_p, cq_v, cq_p, ood_t, ood_q;
+    FriBytes fri;
     u64 nonce = 0;
 };
 
@@ -322,26 +348,16 @@ u32 parse_proof(const AirHost& air, int hash_id, const u8* proof, size_t len, Pa
     pp.ood_q.n = r.le(2); pp.ood_q.p = r.take(pp.ood_q.n);
     if (!r.ok || pp.ood_t.n != 1 + 2 * ct * d * 8 || pp.ood_q.n != 1 + 2 * kc * d * 8 || pp.ood_t.p[0] != 2 || pp.ood_q.p[0] != 2)
         return WF_VERIFY_MALFORMED;
-    const u8 fl = r.u8_();
-    if (fl != pp.nl) return WF_VERIFY_MALFORMED;
-    pp.fv.resize(fl); pp.fp.resize(fl);
-    for (u32 i = 0; i < fl; i++) {
-        pp.fv[i].n = r.le(4); pp.fv[i].p = r.take(pp.fv[i].n);
-        if (!r.ok) return WF_VERIFY_MALFORMED;
-        pp.fp[i].n = r.le(4); pp.fp[i].p = r.take(pp.fp[i].n);
-        if (!r.ok) return WF_VERIFY_MALFORMED;
-    }
-    pp.rem.n = r.le(2); pp.rem.p = r.take(pp.rem.n);
-    pp.fri_log_parts = r.u8_();   // FriProof::num_partitions as a power of two (fri/src/proof.rs:36,101-103)
+    if (!read_fri_proof(r, pp.fri) || pp.fri.fv.size() != pp.nl) return WF_VERIFY_MALFORMED;
     pp.nonce = r.le(8);
-    if (!r.ok || r.pos != len || pp.rem.n % (8 * d)) return WF_VERIFY_MALFORMED;
+    if (!r.ok || r.pos != len || pp.fri.rem.n % (8 * d)) return WF_VERIFY_MALFORMED;
     return WF_VERIFY_ACCEPT;
 }
 bool values_canonical(const Parsed& pp) {
-    for (const Bytes* b : {&pp.tq_v, &pp.aq_v, &pp.cq_v, &pp.rem})
+    for (const Bytes* b : {&pp.tq_v, &pp.aq_v, &pp.cq_v, &pp.fri.rem})
         if (!all_canonical(*b)) return false;
     if (!all_canonical(pp.ood_t, 1) || !all_canonical(pp.ood_q, 1)) return false;   // after the frame-size byte
-    for (const Bytes& b : pp.fv)
+    for (const Bytes& b : pp.fri.fv)
         if (!all_canonical(b)) return false;
     return true;
 }
@@ -367,6 +383,7 @@ struct Plan {
     std::vector<std::vector<CheckItem>> checks;  // per depth
     std::vector<RemItem> rems;
     u32 nevals = 0;
+    std::vector<u64> ev0;                      // evaluations the caller gives, 3 words each: slots 0, 1, ... (standalone FRI)
 
     u32 add_row(u32 words, u32 part, const u8* row) {
         auto key = std::make_pair(words, part);
@@ -494,6 +511,69 @@ GlExt<D> horner(const std::vector<GlExt<D>>& p, const GlExt<D>& x) {
     GlExt<D> acc = ext_zero<D>();
     for (size_t i = p.size(); i-- > 0;) acc = ext_add(ext_mul(acc, x), p[i]);
     return acc;
+}
+
+// The verdict codes of the FRI checks: WF_VERIFY_* inside a full proof, WF_FRI_VERIFY_* for a standalone FRI proof
+struct FriCodes { u32 malformed, layer, fold, rem_degree, rem_fold; };
+constexpr FriCodes FULL_PROOF_CODES{WF_VERIFY_MALFORMED, WF_VERIFY_FRI_LAYER, WF_VERIFY_FRI_FOLD, WF_VERIFY_FRI_REMAINDER,
+                                    WF_VERIFY_FRI_REMAINDER};
+constexpr FriCodes FRI_CODES{WF_FRI_VERIFY_MALFORMED, WF_FRI_VERIFY_LAYER_COMMITMENT_MISMATCH, WF_FRI_VERIFY_INVALID_LAYER_FOLDING,
+                             WF_FRI_VERIFY_REMAINDER_DEGREE_MISMATCH, WF_FRI_VERIFY_INVALID_REMAINDER_FOLDING};
+// The commitment indexes a layer's folded positions are opened at (map_positions_to_indexes, fri/src/utils.rs:9-33): 0 with
+// idx filled, or the code of a failure
+using IndexMap = std::function<u32(const std::vector<u64>& fpos, size_t row_len, std::vector<u64>& idx)>;
+
+// The query phase of FriVerifier::verify (fri/src/verifier/mod.rs:199-331) for one proof as device work. Per layer: the rows of
+// the folded positions opened against the layer's root at the indexes `index_map` gives (read_layer_queries), the current
+// evaluations compared with the rows (get_query_values) and every row folded at its alpha; then the remainder's length
+// against max_degree_plus_1, and its value at the final positions. `cur`: the evaluation slots of `positions`; mdp1:
+// max_poly_degree + 1. verify_generic's DegreeTruncation is not planned: FriVerifier::new already refused every degree it
+// would. A failure the host decides seeds `fail` and ends the plan.
+template <int D>
+void plan_fri(Plan& pl, int h, u32 j, u32 pidx, const FriBytes& fb, const Digest* roots, size_t N, u32 nf, u32 nl, size_t mdp1,
+              const FriCodes& codes, const IndexMap& index_map, std::vector<u64> positions, std::vector<u32> cur, u32& fail) {
+    const u32 nf_log = log2_ceil(nf);
+    size_t dom = N;
+    u32 root;
+    for (u32 depth = 0; depth < nl; depth++) {
+        const size_t row_len = dom / nf;
+        const std::vector<u64> fpos = fold_positions(positions, row_len);
+        const u32 layer = fri_layer_rank(depth);
+        if (depth >= fb.fv.size()) { fail = fail_word(layer, codes.malformed); return; }   // no layer left to read
+        std::vector<u64> idx;
+        if (const u32 bad = index_map(fpos, row_len, idx)) { fail = fail_word(layer, bad); return; }
+        std::vector<u32> refs;
+        if (!pl.rows(fb.fv[depth], fpos.size(), nf * D, 0, refs) || !pl.opening(fb.fp[depth], h, row_len, idx, refs, &root)) {
+            fail = fail_word(layer, codes.layer);
+            return;
+        }
+        pl.cmps.push_back({j, fail_word(layer, codes.layer), root, pl.upload(roots[depth])});
+        if (pl.folds.size() <= depth) { pl.folds.resize(depth + 1); pl.checks.resize(depth + 1); }
+        std::vector<std::vector<CheckItem>> per_row(fpos.size());
+        for (size_t i = 0; i < positions.size(); i++) {
+            const size_t row = std::find(fpos.begin(), fpos.end(), positions[i] % row_len) - fpos.begin();
+            per_row[row].push_back({cur[i], (u32)(positions[i] / row_len)});
+        }
+        std::vector<u32> next(fpos.size());
+        const u32 log_dom = log2_ceil(dom);
+        for (size_t i = 0; i < fpos.size(); i++) {
+            Plan::Fold f{};
+            f.it.proof = pidx; f.it.depth = depth; f.it.log_dom = log_dom; f.it.out = next[i] = pl.nevals++;
+            f.it.fpos = fpos[i]; f.it.nf_log = nf_log;
+            f.it.chk0 = (u32)pl.checks[depth].size(); f.it.nchk = (u32)per_row[i].size();
+            pl.checks[depth].insert(pl.checks[depth].end(), per_row[i].begin(), per_row[i].end());
+            f.leaf = refs[i] & REF_MASK;
+            pl.folds[depth].push_back(f);
+        }
+        cur = next;
+        positions = fpos;
+        dom = row_len;
+    }
+    const size_t rn = fb.rem.n / (8 * D);
+    for (u32 i = 0; i < nl; i++) mdp1 /= nf;   // max_degree_plus_1 after folding (verifier/mod.rs:296-300)
+    if (rn > mdp1) { fail = fail_word(R_REMAINDER, codes.rem_degree); return; }
+    const u32 log_dom = log2_ceil(dom);
+    for (size_t i = 0; i < positions.size(); i++) pl.rems.push_back({pidx, cur[i], log_dom, 0, positions[i]});
 }
 
 // the boundary terms of one segment (verifier/src/evaluator.rs:60-83): cc (T(z) - P(z x_offset)) / (z^a - b) per assertion,
@@ -629,7 +709,7 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
     if (pos.size() != pp.nuq) { fail = fail_word(0, WF_VERIFY_MALFORMED); return WF_OK; }
 
     // ---- device work ----
-    const u32 rn = (u32)(pp.rem.n / (8 * D));
+    const u32 rn = (u32)(pp.fri.rem.n / (8 * D));
     ProofDev pd{};
     pd.d = D; pd.c = c; pd.aw = aw; pd.kc = kc; pd.log_N = pp.logn + lb; pd.rn = rn; pd.slot = j;
     pd.cst = pl.cst.size();
@@ -642,7 +722,7 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
         pd.a_off = (u32)(w.size() - pd.cst);
         for (auto& e : alphas) push_elem<D>(w, e);
         pd.r_off = (u32)(w.size() - pd.cst);
-        for (u32 i = 0; i < rn; i++) push_elem<D>(w, read_elem<D>(pp.rem.p, i));
+        for (u32 i = 0; i < rn; i++) push_elem<D>(w, read_elem<D>(pp.fri.rem.p, i));
     }
     const u32 pidx = (u32)pl.pds.size();
     pl.pds.push_back(pd);
@@ -662,53 +742,20 @@ int host_part(const Call& call, u32 j, const AirHost& air_in, const Parsed& pp, 
         cur[i] = pl.nevals++;
         pl.deep.push_back({pidx, cur[i], t_refs[i] & REF_MASK, aw ? a_refs[i] & REF_MASK : 0, c_refs[i] & REF_MASK, pos[i]});
     }
-    // FRI (fri/src/verifier/mod.rs:210-331)
-    const u32 nf = o.folding;
-    const u32 nf_log = log2_ceil(nf);
-    std::vector<u64> positions = pos;
-    size_t dom = N;
-    for (u32 depth = 0; depth < nl; depth++) {
-        const size_t row_len = dom / nf;
-        const std::vector<u64> fpos = fold_positions(positions, row_len);
-        const u32 layer = fri_layer_rank(depth);
-        if (pp.fri_log_parts) {   // map_positions_to_indexes (fri/src/utils.rs:9-33)
-            if (pp.fri_log_parts >= 32) { fail = fail_word(layer, WF_VERIFY_MALFORMED); return WF_OK; }
-            const u64 P_ = (u64)1 << pp.fri_log_parts, psize = row_len / P_;
+    // FRI (fri/src/verifier/mod.rs:210-331). The prover commits every layer in domain order (one partition): a proof whose
+    // partition count maps a folded position anywhere else cannot open its layer
+    const u8 lp = pp.fri.log_parts;
+    auto index_map = [lp](const std::vector<u64>& fpos, size_t row_len, std::vector<u64>& idx) -> u32 {
+        if (lp) {
+            if (lp >= 32) return WF_VERIFY_MALFORMED;
+            const u64 P_ = (u64)1 << lp, psize = row_len / P_;
             for (u64 p : fpos)
-                if ((p % P_) * psize + (p - p % P_) / P_ != p) { fail = fail_word(layer, WF_VERIFY_FRI_LAYER); return WF_OK; }
+                if ((p % P_) * psize + (p - p % P_) / P_ != p) return WF_VERIFY_FRI_LAYER;
         }
-        std::vector<u32> refs;
-        if (!pl.rows(pp.fv[depth], fpos.size(), nf * D, 0, refs) || !pl.opening(pp.fp[depth], h, row_len, fpos, refs, &root)) {
-            fail = fail_word(layer, WF_VERIFY_FRI_LAYER);
-            return WF_OK;
-        }
-        pl.cmps.push_back({j, fail_word(layer, WF_VERIFY_FRI_LAYER), root, pl.upload(pp.cm[nseg + 1 + depth])});
-        if (pl.folds.size() <= depth) { pl.folds.resize(depth + 1); pl.checks.resize(depth + 1); }
-        std::vector<std::vector<CheckItem>> per_row(fpos.size());
-        for (size_t i = 0; i < positions.size(); i++) {
-            const size_t row = std::find(fpos.begin(), fpos.end(), positions[i] % row_len) - fpos.begin();
-            per_row[row].push_back({cur[i], (u32)(positions[i] / row_len)});
-        }
-        std::vector<u32> next(fpos.size());
-        const u32 log_dom = log2_ceil(dom);
-        for (size_t i = 0; i < fpos.size(); i++) {
-            Plan::Fold f{};
-            f.it.proof = pidx; f.it.depth = depth; f.it.log_dom = log_dom; f.it.out = next[i] = pl.nevals++;
-            f.it.fpos = fpos[i]; f.it.nf_log = nf_log;
-            f.it.chk0 = (u32)pl.checks[depth].size(); f.it.nchk = (u32)per_row[i].size();
-            pl.checks[depth].insert(pl.checks[depth].end(), per_row[i].begin(), per_row[i].end());
-            f.leaf = refs[i] & REF_MASK;
-            pl.folds[depth].push_back(f);
-        }
-        cur = next;
-        positions = fpos;
-        dom = row_len;
-    }
-    size_t mdp1 = n;   // max_degree_plus_1 after folding (verifier/mod.rs:296-300)
-    for (u32 i = 0; i < nl; i++) mdp1 /= nf;
-    if (rn > mdp1) { fail = fail_word(R_REMAINDER, WF_VERIFY_FRI_REMAINDER); return WF_OK; }
-    const u32 log_dom = log2_ceil(dom);
-    for (size_t i = 0; i < positions.size(); i++) pl.rems.push_back({pidx, cur[i], log_dom, 0, positions[i]});
+        idx = fpos;
+        return 0;
+    };
+    plan_fri<D>(pl, h, j, pidx, pp.fri, &pp.cm[nseg + 1], N, o.folding, nl, n, FULL_PROOF_CODES, index_map, pos, cur, fail);
     return WF_OK;
 }
 
@@ -722,52 +769,15 @@ bool options_match(const Options& o, const uint32_t* words) {
 
 size_t align2(size_t words) { return (words + 1) & ~(size_t)1; }
 
-}  // namespace
 
-extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
-                                   const uint8_t* const* proofs, const size_t* proof_lens, int hash_id, const uint32_t* acceptable_opts,
-                                   uint32_t num_acceptable, wf_aux_assertions_batch_fn aux_assertions, void* aux_user, uint32_t* verdicts) {
-    if (!ctx || batch == 0 || !air_descs || !air_desc_lens || !proofs || !proof_lens || !verdicts || (acceptable_opts && !num_acceptable))
-        return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
-    if (!WF_HASH_IS_KNOWN(hash_id)) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "unknown hash %d", hash_id);
-    for (u32 i = 0; acceptable_opts && i < num_acceptable; i++)
-        if ((int)(acceptable_opts[9 * i + 8] & 0xff) != hash_id)
-            return wf_fail(ctx, WF_ERR_INVALID, "acceptable option set %u is for hash %u, not %d", i, acceptable_opts[9 * i + 8] & 0xff, hash_id);
-    // the batch rule of wf_air_batch_check, without the trace length: it comes from each proof
-    std::vector<AirHost> airs(batch);
-    for (u32 j = 0; j < batch; j++) {
-        if (!air_descs[j] || !parse_air_host(air_descs[j], air_desc_lens[j], airs[j]))
-            return wf_fail(ctx, WF_ERR_INVALID, "proof %u: malformed AIR description", j);
-        if (const char* why = j ? air_structure_mismatch(airs[0], airs[j]) : nullptr)
-            return wf_fail(ctx, WF_ERR_INVALID, "proof %u differs from proof 0 in its %s", j, why);
-        if (!proofs[j]) return wf_fail(ctx, WF_ERR_INVALID, "proof %u: no proof bytes", j);
-    }
-    wf_mark(ctx, "start");
-    const Call call{ctx, hash_id, aux_assertions, aux_user};
-    Plan pl;
-    std::vector<u32> fail(batch, NO_FAIL);
-    for (u32 j = 0; j < batch; j++) {
-        Parsed pp;
-        u32 v = parse_proof(airs[j], hash_id, proofs[j], proof_lens[j], pp);
-        if (v == WF_VERIFY_ACCEPT && acceptable_opts) {
-            bool ok = false;
-            for (u32 i = 0; i < num_acceptable && !ok; i++) ok = options_match(pp.o, acceptable_opts + 9 * i);
-            if (!ok) v = WF_VERIFY_UNACCEPTABLE_OPTIONS;
-        }
-        if (v == WF_VERIFY_ACCEPT) {   // Air::new at the declared length: what the reference panics on
-            wf_ctx note{};
-            if (air_check_host(&note, airs[j], pp.logn, pp.o.blowup) != WF_OK) v = WF_VERIFY_CONTEXT;
-        }
-        if (v == WF_VERIFY_ACCEPT && !values_canonical(pp)) v = WF_VERIFY_MALFORMED;
-        if (v != WF_VERIFY_ACCEPT) { fail[j] = fail_word(0, v); continue; }
-        int r = pp.o.ext == 1 ? host_part<1>(call, j, airs[j], pp, pl, fail[j])
-              : pp.o.ext == 2 ? host_part<2>(call, j, airs[j], pp, pl, fail[j]) : host_part<3>(call, j, airs[j], pp, pl, fail[j]);
-        if (r != WF_OK) return r;
-    }
-    wf_mark(ctx, "verify_host");
-
-    // ---- layout: [pds | cst | fail | row groups | deep | folds | checks | rems | cmps | ops | uploaded digests] is uploaded,
-    //      then [leaf digests | merged digests | evaluations | verdicts] ----
+// One batch on the device: one upload; the leaf hashes of every opened row (one launch per row shape); one merge launch per
+// tree level; the root compares; the evaluations at the queries (DEEP composition for full proofs, the caller's copied in for
+// standalone FRI proofs); one FRI launch per depth; the remainder. Then, in one download and one synchronisation, the proofs'
+// fail words, or with verdict_kernel their WF_VERIFY_* verdicts. fail: the words the host seeded; out: batch words.
+int run_plan(wf_ctx* ctx, int hash_id, Plan& pl, const std::vector<u32>& fail, u32 batch, const FriCodes& codes, bool verdict_kernel,
+             u32* out) {
+    // ---- layout: [pds | cst | fail | row groups | deep | folds | checks | rems | cmps | ops | caller evaluations | uploaded
+    //      digests] is uploaded, then [leaf digests | merged digests | evaluations | verdicts] ----
     const u32 U = (u32)pl.up.size(), Lf = (u32)pl.leaves.size();
     std::vector<size_t> gbase(pl.groups.size()), goff(pl.groups.size());
     size_t w = 0;
@@ -792,7 +802,7 @@ extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* 
     const size_t o_deep = take(pl.deep.size() * sizeof(DeepItem) / 8), o_fold = take(nfold * sizeof(FoldItem) / 8),
                  o_chk = take(nchk * sizeof(CheckItem) / 8), o_rem = take(pl.rems.size() * sizeof(RemItem) / 8),
                  o_cmp = take(pl.cmps.size() * sizeof(CmpItem) / 8), o_ops = take((nops * sizeof(uint3) + 7) / 8),
-                 o_arena = take((size_t)U * 4);
+                 o_ev0 = take(pl.ev0.size()), o_arena = take((size_t)U * 4);
     const size_t up_words = w;
     take((size_t)Lf * 4);
     take((size_t)pl.nodes * 4);
@@ -851,6 +861,7 @@ extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* 
                 const uint3 op = pl.levels[l][i];
                 oi[lvl_at[l] + i] = make_uint3(slot(op.x), slot(op.y), slot(op.z));
             }
+        memcpy(hb + o_ev0, pl.ev0.data(), pl.ev0.size() * 8);
         for (u32 i = 0; i < U; i++) memcpy(hb + o_arena + (size_t)i * 4, pl.up[i].b, 32);
     }
     DevScratch tmp(ctx);
@@ -881,25 +892,259 @@ extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* 
         verify_deep_kernel<<<blocks(pl.deep.size(), 128), 128, 0, ctx->st>>>(dpds, dv, (const DeepItem*)(dv + o_deep), (u32)pl.deep.size(), evals);
         ctx->launches++;
     }
+    if (!pl.ev0.empty()) CK(cudaMemcpyAsync(evals, dv + o_ev0, pl.ev0.size() * 8, cudaMemcpyDeviceToDevice, ctx->st));
     for (size_t d = 0; d < pl.folds.size(); d++) {
         if (pl.folds[d].empty()) continue;
         verify_fri_kernel<<<blocks(pl.folds[d].size(), 128), 128, 0, ctx->st>>>(dpds, dv, (const FoldItem*)(dv + o_fold) + fold_at[d],
-                                                                               (u32)pl.folds[d].size(), (const CheckItem*)(dv + o_chk), evals, dfail);
+                                                                               (u32)pl.folds[d].size(), (const CheckItem*)(dv + o_chk), evals, dfail,
+                                                                               codes.fold);
         ctx->launches++;
     }
     if (!pl.rems.empty()) {
         verify_remainder_kernel<<<blocks(pl.rems.size(), 128), 128, 0, ctx->st>>>(dpds, dv, (const RemItem*)(dv + o_rem), (u32)pl.rems.size(),
-                                                                                 evals, dfail);
+                                                                                 evals, dfail, codes.rem_fold);
         ctx->launches++;
     }
-    u32* dverdict = (u32*)(dv + o_verdict);
-    verify_verdict_kernel<<<blocks(batch, 256), 256, 0, ctx->st>>>(dfail, batch, dverdict);
-    ctx->launches++;
+    const u32* dout = dfail;
+    if (verdict_kernel) {
+        u32* dverdict = (u32*)(dv + o_verdict);
+        verify_verdict_kernel<<<blocks(batch, 256), 256, 0, ctx->st>>>(dfail, batch, dverdict);
+        ctx->launches++;
+        dout = dverdict;
+    }
     CK(cudaGetLastError());
     u32* hv = (u32*)(hb + up_words);
-    CK(cudaMemcpyAsync(hv, dverdict, batch * 4, cudaMemcpyDeviceToHost, ctx->st));
+    CK(cudaMemcpyAsync(hv, dout, batch * 4, cudaMemcpyDeviceToHost, ctx->st));
     CK(cudaStreamSynchronize(ctx->st));
-    memcpy(verdicts, hv, batch * 4);
+    memcpy(out, hv, batch * 4);
+    return WF_OK;
+}
+
+
+// ---- standalone FRI proofs (wf_fri_verify_batch) ----
+// BatchMerkleProof::read_from (crypto/src/merkle/proofs.rs:403-423) with the bounds Plan::opening keeps, every byte used: false
+// when it does not parse
+bool batch_proof_depth(const Bytes& path, int hash_id, u32* depth) {
+    Reader r{path.p, path.n};
+    const u8 dp = r.u8_();
+    const u64 nv = r.usize();
+    if (!r.ok || nv > 100000 || dp < 1 || dp > 40) return false;
+    const size_t dl = WF_DIGEST_BYTES(hash_id);
+    for (u64 i = 0; i < nv; i++) {
+        const u64 ln = r.usize();
+        if (!r.ok || ln > 64 || !r.take(ln * dl)) return false;
+    }
+    *depth = dp;
+    return r.pos == path.n;
+}
+
+struct FriShape {
+    int hash_id;
+    u32 nf, nl;
+    size_t domain, mdp1;   // max_poly_degree.next_power_of_two() * blowup; max_poly_degree + 1
+};
+// (domain, number of layers) of FriVerifier::new for these options; false when a layer would have fewer than two rows (no
+// Merkle tree) or the remainder no element
+bool fri_shape(u32 nf, u32 rem_max_deg, u32 blowup, u64 max_poly_degree, FriShape& s) {
+    if (blowup == 0 || (blowup & (blowup - 1)) || max_poly_degree >= ((u64)1 << 32)) return false;
+    u64 np2 = 1;
+    while (np2 < max_poly_degree) np2 <<= 1;
+    if (np2 * blowup > ((u64)1 << 32)) return false;
+    size_t dom = np2 * blowup;
+    const size_t max_rem = ((size_t)rem_max_deg + 1) * blowup;   // FriOptions::num_fri_layers (fri/src/options.rs:85-93)
+    s.nl = 0;
+    while (dom > max_rem) {
+        if (dom / nf < 2) return false;
+        dom /= nf;
+        s.nl++;
+    }
+    if (dom / blowup == 0) return false;
+    s.nf = nf;
+    s.domain = np2 * blowup;
+    s.mdp1 = max_poly_degree + 1;
+    return true;
+}
+
+// Everything of proof j the host decides: DefaultVerifierChannel::new's deserialization (fri/src/verifier/channel.rs:146-170,
+// fri/src/proof.rs:98-146), FriVerifier::new (reseed, draw, DegreeTruncation), then the query phase through plan_fri. Its
+// positions' evaluations sit in slots ev_base ... A failure the host decides seeds `fail`; one of rank 0 (deserialization,
+// FriVerifier::new) also writes its verdict to `verdict`.
+template <int D>
+void fri_host_part(const FriShape& s, u32 j, const u8* proof, size_t len, const u8* cms, const u8* seed, const u64* positions,
+                   size_t k, u32 ev_base, Plan& pl, u32& fail, u32& verdict) {
+    const int h = s.hash_id;
+    const u32 nf = s.nf;
+    auto refuse = [&](u32 code, u32 layer = 0) { fail = fail_word(0, code); verdict = code | layer << 8; };
+    Reader r{proof, len};
+    FriBytes fb;
+    if (!read_fri_proof(r, fb) || r.pos != len || fb.log_parts >= 64) return refuse(WF_FRI_VERIFY_MALFORMED);   // 2^64 partitions
+    const size_t rn = fb.rem.n / (8 * D);   // parse_remainder
+    if (fb.rem.n % (8 * D) || rn == 0 || (rn & (rn - 1)) || !all_canonical(fb.rem)) return refuse(WF_FRI_VERIFY_MALFORMED);
+    size_t ds = s.domain;   // parse_layers, FriProofLayer::read_from / parse
+    for (size_t i = 0; i < fb.fv.size(); i++) {
+        ds /= nf;
+        u32 depth;
+        if (fb.fv[i].n == 0 || fb.fv[i].n % (8 * D * nf) || !all_canonical(fb.fv[i]) || !batch_proof_depth(fb.fp[i], h, &depth) ||
+            ((size_t)1 << depth) != ds)
+            return refuse(WF_FRI_VERIFY_MALFORMED);
+    }
+    // FriVerifier::new (fri/src/verifier/mod.rs:107-152)
+    PublicCoin coin(h, nullptr, 0);
+    if (seed) memcpy(coin.seed.b, seed, 32);
+    std::vector<Digest> cm(s.nl + 1);
+    for (u32 i = 0; i <= s.nl; i++) { cm[i] = Digest{}; read_digest(h, cms + 32 * i, cm[i]); }
+    std::vector<GlExt<D>> alphas;
+    size_t mdp1 = s.mdp1;
+    for (u32 i = 0; i <= s.nl; i++) {
+        coin.reseed(cm[i]);
+        GlExt<D> a = ext_zero<D>();
+        if (!coin.draw(D, a.v)) return refuse(WF_FRI_VERIFY_RANDOM_COIN);
+        alphas.push_back(a);
+        if (i != s.nl && mdp1 % nf) return refuse(WF_FRI_VERIFY_DEGREE_TRUNCATION, i);
+        mdp1 /= nf;
+    }
+    ProofDev pd{};
+    pd.d = D; pd.log_N = log2_ceil(s.domain); pd.rn = (u32)rn; pd.slot = j;
+    pd.cst = pl.cst.size();
+    pd.a_off = 0;
+    for (auto& e : alphas) push_elem<D>(pl.cst, e);
+    pd.r_off = (u32)(pl.cst.size() - pd.cst);
+    for (size_t i = 0; i < rn; i++) push_elem<D>(pl.cst, read_elem<D>(fb.rem.p, i));
+    const u32 pidx = (u32)pl.pds.size();
+    pl.pds.push_back(pd);
+    std::vector<u32> cur(k);
+    for (size_t i = 0; i < k; i++) cur[i] = ev_base + (u32)i;
+    const u8 lp = fb.log_parts;
+    auto index_map = [lp](const std::vector<u64>& fpos, size_t row_len, std::vector<u64>& idx) -> u32 {
+        idx = fpos;
+        if (!lp) return 0;
+        const u64 P_ = (u64)1 << lp, psize = row_len / P_;
+        for (u64& q : idx) q = (q % P_) * psize + (q - q % P_) / P_;
+        const std::set<u64> seen(idx.begin(), idx.end());
+        return seen.size() != idx.size() || (!seen.empty() && *seen.rbegin() >= row_len) ? WF_FRI_VERIFY_MALFORMED : 0;
+    };
+    plan_fri<D>(pl, h, j, pidx, fb, cm.data(), s.domain, nf, s.nl, s.mdp1, FRI_CODES, index_map,
+                std::vector<u64>(positions, positions + k), cur, fail);
+}
+
+}  // namespace
+
+extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
+                                   const uint8_t* const* proofs, const size_t* proof_lens, int hash_id, const uint32_t* acceptable_opts,
+                                   uint32_t num_acceptable, wf_aux_assertions_batch_fn aux_assertions, void* aux_user, uint32_t* verdicts) {
+    if (!ctx || batch == 0 || !air_descs || !air_desc_lens || !proofs || !proof_lens || !verdicts || (acceptable_opts && !num_acceptable))
+        return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    if (!WF_HASH_IS_KNOWN(hash_id)) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "unknown hash %d", hash_id);
+    for (u32 i = 0; acceptable_opts && i < num_acceptable; i++)
+        if ((int)(acceptable_opts[9 * i + 8] & 0xff) != hash_id)
+            return wf_fail(ctx, WF_ERR_INVALID, "acceptable option set %u is for hash %u, not %d", i, acceptable_opts[9 * i + 8] & 0xff, hash_id);
+    // the batch rule of wf_air_batch_check, without the trace length: it comes from each proof
+    std::vector<AirHost> airs(batch);
+    for (u32 j = 0; j < batch; j++) {
+        if (!air_descs[j] || !parse_air_host(air_descs[j], air_desc_lens[j], airs[j]))
+            return wf_fail(ctx, WF_ERR_INVALID, "proof %u: malformed AIR description", j);
+        if (const char* why = j ? air_structure_mismatch(airs[0], airs[j]) : nullptr)
+            return wf_fail(ctx, WF_ERR_INVALID, "proof %u differs from proof 0 in its %s", j, why);
+        if (!proofs[j]) return wf_fail(ctx, WF_ERR_INVALID, "proof %u: no proof bytes", j);
+    }
+    wf_mark(ctx, "start");
+    const Call call{ctx, hash_id, aux_assertions, aux_user};
+    Plan pl;
+    std::vector<u32> fail(batch, NO_FAIL);
+    for (u32 j = 0; j < batch; j++) {
+        Parsed pp;
+        u32 v = parse_proof(airs[j], hash_id, proofs[j], proof_lens[j], pp);
+        if (v == WF_VERIFY_ACCEPT && acceptable_opts) {
+            bool ok = false;
+            for (u32 i = 0; i < num_acceptable && !ok; i++) ok = options_match(pp.o, acceptable_opts + 9 * i);
+            if (!ok) v = WF_VERIFY_UNACCEPTABLE_OPTIONS;
+        }
+        if (v == WF_VERIFY_ACCEPT) {   // Air::new at the declared length: what the reference panics on
+            wf_ctx note{};
+            if (air_check_host(&note, airs[j], pp.logn, pp.o.blowup) != WF_OK) v = WF_VERIFY_CONTEXT;
+        }
+        if (v == WF_VERIFY_ACCEPT && !values_canonical(pp)) v = WF_VERIFY_MALFORMED;
+        if (v != WF_VERIFY_ACCEPT) { fail[j] = fail_word(0, v); continue; }
+        int r = pp.o.ext == 1 ? host_part<1>(call, j, airs[j], pp, pl, fail[j])
+              : pp.o.ext == 2 ? host_part<2>(call, j, airs[j], pp, pl, fail[j]) : host_part<3>(call, j, airs[j], pp, pl, fail[j]);
+        if (r != WF_OK) return r;
+    }
+    wf_mark(ctx, "verify_host");
+
+    CKI(run_plan(ctx, hash_id, pl, fail, batch, FULL_PROOF_CODES, true, verdicts));
+    wf_mark(ctx, "verify_device");
+    return WF_OK;
+}
+
+extern "C" int wf_fri_verify_batch(wf_ctx* ctx, int hash_id, int ext_degree, uint32_t folding_factor, uint32_t remainder_max_degree,
+                                   uint32_t blowup, uint64_t max_poly_degree, uint32_t batch, const uint8_t* const* proofs,
+                                   const size_t* proof_lens, const uint8_t* const* commitments, const uint32_t* num_commitments,
+                                   const uint8_t* const* coin_seeds, const uint64_t* const* positions,
+                                   const uint64_t* const* evaluations, const size_t* num_queries, uint32_t* verdicts) {
+    if (!ctx || batch == 0 || !proofs || !proof_lens || !commitments || !num_commitments || !positions || !evaluations || !num_queries ||
+        !verdicts)
+        return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    if (!WF_HASH_IS_KNOWN(hash_id)) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "unknown hash %d", hash_id);
+    if (folding_factor != 2 && folding_factor != 4 && folding_factor != 8 && folding_factor != 16)
+        return wf_fail(ctx, WF_ERR_UNSUPPORTED, "folding factor %u is not supported", folding_factor);
+    if (ext_degree < 1 || ext_degree > 3) return wf_fail(ctx, WF_ERR_INVALID, "extension degree %d", ext_degree);
+    FriShape s{};
+    s.hash_id = hash_id;
+    if (!fri_shape(folding_factor, remainder_max_degree, blowup, max_poly_degree, s))
+        return wf_fail(ctx, WF_ERR_INVALID, "no FRI proof has this shape (blowup %u, folding %u, remainder degree %u, max degree %llu)",
+                       blowup, folding_factor, remainder_max_degree, (unsigned long long)max_poly_degree);
+    const u32 D = (u32)ext_degree;
+    size_t total = 0;
+    for (u32 j = 0; j < batch; j++) {
+        if (!proofs[j] || !commitments[j]) return wf_fail(ctx, WF_ERR_INVALID, "proof %u: no proof bytes or commitments", j);
+        if (num_commitments[j] != s.nl + 1)
+            return wf_fail(ctx, WF_ERR_INVALID, "proof %u: %u commitments, the shape has %u layers and a remainder", j, num_commitments[j], s.nl);
+        const size_t k = num_queries[j];
+        if (k && (!positions[j] || !evaluations[j])) return wf_fail(ctx, WF_ERR_INVALID, "proof %u: no positions or evaluations", j);
+        for (size_t i = 0; i < k; i++) {
+            if (positions[j][i] >= s.domain)
+                return wf_fail(ctx, WF_ERR_INVALID, "proof %u: position %llu is outside the domain of %zu", j,
+                               (unsigned long long)positions[j][i], s.domain);
+            for (u32 c = 0; c < D; c++)
+                if (evaluations[j][i * D + c] >= GL_P) return wf_fail(ctx, WF_ERR_INVALID, "proof %u: evaluation %zu is not canonical", j, i);
+        }
+        total += k;
+    }
+    if (total >= ((size_t)1 << 31)) return wf_fail(ctx, WF_ERR_INVALID, "too many queries in one batch");
+    wf_mark(ctx, "start");
+    // the caller's evaluations in slots 0 .. total - 1, proof by proof; the folds' evaluations follow
+    Plan pl;
+    pl.ev0.assign(total * 3, 0);
+    std::vector<u32> ev_base(batch);
+    {
+        size_t at = 0;
+        for (u32 j = 0; j < batch; j++) {
+            ev_base[j] = (u32)at;
+            for (size_t i = 0; i < num_queries[j]; i++, at++)
+                for (u32 c = 0; c < D; c++) pl.ev0[at * 3 + c] = evaluations[j][i * D + c];
+        }
+        pl.nevals = (u32)total;
+    }
+    std::vector<u32> fail(batch, NO_FAIL), host(batch, WF_FRI_VERIFY_ACCEPT);
+    for (u32 j = 0; j < batch; j++) {
+        const u8* seed = coin_seeds ? coin_seeds[j] : nullptr;
+        const size_t k = num_queries[j];
+        if (D == 1) fri_host_part<1>(s, j, proofs[j], proof_lens[j], commitments[j], seed, positions[j], k, ev_base[j], pl, fail[j], host[j]);
+        else if (D == 2) fri_host_part<2>(s, j, proofs[j], proof_lens[j], commitments[j], seed, positions[j], k, ev_base[j], pl, fail[j], host[j]);
+        else fri_host_part<3>(s, j, proofs[j], proof_lens[j], commitments[j], seed, positions[j], k, ev_base[j], pl, fail[j], host[j]);
+    }
+    wf_mark(ctx, "verify_host");
+    std::vector<u32> words(batch);
+    CKI(run_plan(ctx, hash_id, pl, fail, batch, FRI_CODES, false, words.data()));
+    // a rank-0 word is the deserialization's or FriVerifier::new's verdict, which may carry a layer; the later words carry their
+    // code, and InvalidLayerFolding its depth in the rank
+    for (u32 j = 0; j < batch; j++) {
+        const u32 w = words[j];
+        if (w == NO_FAIL) verdicts[j] = WF_FRI_VERIFY_ACCEPT;
+        else if ((w >> 4) == 0) verdicts[j] = host[j];
+        else if ((w & 15u) == WF_FRI_VERIFY_INVALID_LAYER_FOLDING) verdicts[j] = WF_FRI_VERIFY_INVALID_LAYER_FOLDING | ((w >> 4) - R_FRI - 1) / 2 << 8;
+        else verdicts[j] = w & 15u;
+    }
     wf_mark(ctx, "verify_device");
     return WF_OK;
 }
