@@ -360,6 +360,8 @@ int wf_air_batch_check(uint32_t batch, const uint64_t* const* air_descs, const s
 #define WF_VERIFY_FRI_REMAINDER        8   /* FriVerificationFailed(InvalidRemainderFolding / RemainderDegreeMismatch) */
 #define WF_VERIFY_CONTEXT              9   /* the proof's context does not fit the AIR (InconsistentBaseField, widths, constraint count) */
 #define WF_VERIFY_UNACCEPTABLE_OPTIONS 10  /* AcceptableOptions::OptionSet refused the proof's options */
+#define WF_VERIFY_INSUFFICIENT_CONJECTURED_SECURITY 11  /* AcceptableOptions::MinConjecturedSecurity refused the proof */
+#define WF_VERIFY_INSUFFICIENT_PROVEN_SECURITY      12  /* AcceptableOptions::MinProvenSecurity refused the proof */
 /* Air::get_aux_assertions(aux_rand_elements) of proof `proof` (its index in the batch): rand_elements [nr][ext], values
  * [number of aux assertion values][ext], in: the description's values, out: the values to assert. Non-zero = failure. */
 typedef int (*wf_aux_assertions_batch_fn)(void* user, uint32_t proof, const uint64_t* rand_elements, uint64_t* values);
@@ -372,11 +374,43 @@ typedef int (*wf_aux_assertions_batch_fn)(void* user, uint32_t proof, const uint
  * (may be NULL): called on the host once per proof that reaches Air::get_aux_assertions, with its index. WF_ERR_INVALID for
  * caller errors (NULL pointers, a description that does not parse or breaks the batch rule, a failing callback), naming the
  * proof; no device buffer stays live after any return. The surviving proofs are checked on the device together: the number
- * of kernel launches does not depend on `batch` for proofs of one shape. */
+ * of kernel launches does not depend on `batch` for proofs of one shape. For the other two AcceptableOptions variants,
+ * MinConjecturedSecurity and MinProvenSecurity, see wf_verify_air_batch_min_security. */
 int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
                         const uint8_t* const* proofs, const size_t* proof_lens, int hash_id,
                         const uint32_t* acceptable_opts, uint32_t num_acceptable,
                         wf_aux_assertions_batch_fn aux_assertions, void* aux_user, uint32_t* verdicts);
+/* wf_verify_air_batch with AcceptableOptions::MinConjecturedSecurity(min_bits) (regime WF_SECURITY_CONJECTURED) or
+ * MinProvenSecurity(min_bits) (WF_SECURITY_PROVEN) in place of an option set (verifier/src/lib.rs:333-354). The estimate is
+ * Proof::conjectured_security / proven_security of hash_id (wf_proof_security), checked where wf_verify_air_batch checks its
+ * option set: after the proof parses (MALFORMED and the parse-time CONTEXT verdicts come first), before the AIR is built at
+ * the proof's length. A proof below min_bits gets WF_VERIFY_INSUFFICIENT_CONJECTURED_SECURITY / _PROVEN_SECURITY and never
+ * reaches the device; the others are verified exactly as wf_verify_air_batch verifies them. The proven rule accepts when
+ * either the list-decoding or the unique-decoding bound reaches min_bits. security_bits (may be NULL): per proof, the bits
+ * the reference's error carries (the conjectured bits, or max(ldr, udr)), also for an accepted proof; ~0u for a proof refused
+ * before the check. min_bits = 0 gives wf_verify_air_batch(acceptable_opts = NULL)'s verdicts and launches. WF_ERR_INVALID
+ * for another regime; every other error is wf_verify_air_batch's. The estimate is memoised per distinct (options, trace
+ * length) within a call. */
+#define WF_SECURITY_CONJECTURED 1
+#define WF_SECURITY_PROVEN      2
+int wf_verify_air_batch_min_security(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
+                                     const uint8_t* const* proofs, const size_t* proof_lens, int hash_id, int regime, uint32_t min_bits,
+                                     wf_aux_assertions_batch_fn aux_assertions, void* aux_user, uint32_t* verdicts,
+                                     uint32_t* security_bits);
+/* The reference's security estimate (air/src/proof/security.rs) for the Goldilocks field, without a device:
+ * ConjecturedSecurity::compute(options, 64, collision_resistance) and ProvenSecurity::compute(options, 64, trace_length,
+ * collision_resistance, num_constraints, num_committed_polys), with their own arguments. opts: the opts[9] vector of the
+ * proving entry points; words 0-7 are read. collision_resistance: Hasher::COLLISION_RESISTANCE (128 for Blake3_256, Sha3_256,
+ * Rp64_256 and RpJive64_256, 96 for Blake3_192). WF_OK, or WF_ERR_INVALID for options outside ProofOptions::new's ranges,
+ * a trace length that is not a power of two in [8, 2^32], zero constraints or committed polynomials, or a NULL pointer. */
+int wf_security_estimate(const uint32_t* opts, uint64_t trace_length, uint32_t collision_resistance, uint64_t num_constraints,
+                         uint64_t num_committed_polys, uint32_t* conjectured, uint32_t* proven_ldr, uint32_t* proven_udr);
+/* Proof::conjectured_security::<H>() and proven_security::<H>() (air/src/proof/mod.rs:96-126) of a serialized proof, without
+ * a device: the Context at the head of the proof (trace info, modulus, options, constraint count) gives the estimate's
+ * inputs; num_committed_polys is the trace width (main + aux) plus the blowup factor. The rest of the proof is not read.
+ * WF_ERR_INVALID for a context Context::read_from refuses or a field other than Goldilocks (or a NULL pointer);
+ * WF_ERR_UNSUPPORTED for an unknown hash. */
+int wf_proof_security(int hash_id, const uint8_t* proof, size_t len, uint32_t* conjectured, uint32_t* proven_ldr, uint32_t* proven_udr);
 
 /* ---- checking a trace against its AIR: the reference's debug builds (Trace::validate, prover/src/trace/mod.rs:86-201;
  *      ConstraintEvaluationTable::validate_transition_degrees, prover/src/constraints/evaluation_table.rs:181-230) ----------

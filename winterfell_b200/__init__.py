@@ -33,7 +33,10 @@ AUX_ASSERTIONS_BATCH = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, u64p, u64p)
 
 # wf_verify_air_batch verdicts (include/winterfell_b200.h WF_VERIFY_*)
 VERIFY_ACCEPT, VERIFY_MALFORMED, VERIFY_OOD, VERIFY_POW, VERIFY_TRACE_QUERY, VERIFY_CONSTRAINT_QUERY, VERIFY_FRI_LAYER, \
-    VERIFY_FRI_FOLD, VERIFY_FRI_REMAINDER, VERIFY_CONTEXT, VERIFY_UNACCEPTABLE_OPTIONS = range(11)
+    VERIFY_FRI_FOLD, VERIFY_FRI_REMAINDER, VERIFY_CONTEXT, VERIFY_UNACCEPTABLE_OPTIONS, VERIFY_INSUFFICIENT_CONJECTURED_SECURITY, \
+    VERIFY_INSUFFICIENT_PROVEN_SECURITY = range(13)
+# wf_verify_air_batch_min_security regimes (WF_SECURITY_*)
+SECURITY_CONJECTURED, SECURITY_PROVEN = 1, 2
 
 # wf_fri_verify_batch verdicts (include/winterfell_b200.h WF_FRI_VERIFY_*); INVALID_LAYER_FOLDING and DEGREE_TRUNCATION carry
 # their layer in bits 8 and up (fri_verdict_layer)
@@ -165,6 +168,12 @@ _SIGS = [
     ("wf_air_batch_check", C.c_int, [C.c_uint32, C.POINTER(u64p), C.POINTER(C.c_size_t), C.c_uint32, C.c_uint32, C.c_char_p, C.c_size_t]),
     ("wf_verify_air_batch", C.c_int, [vp, C.c_uint32, C.POINTER(u64p), C.POINTER(C.c_size_t), C.POINTER(u8p), C.POINTER(C.c_size_t), C.c_int,
                                       C.POINTER(C.c_uint32), C.c_uint32, AUX_ASSERTIONS_BATCH, vp, C.POINTER(C.c_uint32)]),
+    ("wf_verify_air_batch_min_security", C.c_int, [vp, C.c_uint32, C.POINTER(u64p), C.POINTER(C.c_size_t), C.POINTER(u8p),
+                                                   C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_uint32, AUX_ASSERTIONS_BATCH, vp,
+                                                   C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    ("wf_security_estimate", C.c_int, [C.POINTER(C.c_uint32), C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, C.POINTER(C.c_uint32),
+                                       C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    ("wf_proof_security", C.c_int, [C.c_int, u8p, C.c_size_t, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     ("wf_host_hash_elements", C.c_int, [C.c_int, u64p, C.c_size_t, u8p]),
     ("wf_host_merge", C.c_int, [C.c_int, u8p, u8p]),
     ("wf_host_merge_with_int", C.c_int, [C.c_int, u8p, C.c_uint64, u8p]),
@@ -583,10 +592,9 @@ class Context:
                                              o_.ctypes.data_as(C.POINTER(C.c_uint32)), outs, lens))
         return [buf[j, : lens[j]].tobytes() for j in range(batch)]
 
-    def verify_air_batch(self, descs, proofs, hash_id, acceptable=None, aux_values_fn=None):
-        """wf_verify_air_batch: the verdict (VERIFY_*) of each proof in `proofs` (bytes) against the description of the same
-        index in `descs` (one AIR structure). acceptable: None (accept the options a proof carries) or a list of opts[9] arrays.
-        aux_values_fn(j, rand [nr, d], values [nv, d]) -> values: Air::get_aux_assertions of proof j. Returns a uint32 array."""
+    def _air_batch_args(self, descs, proofs, aux_values_fn):
+        """The arguments wf_verify_air_batch and wf_verify_air_batch_min_security share: (batch, descriptions, their lengths,
+        proofs, their lengths, the aux assertion callback, the arrays they point into)."""
         ds = [np.ascontiguousarray(d, dtype=np.uint64) for d in descs]
         ps = [np.frombuffer(p, dtype=np.uint8) if len(p) else np.zeros(1, dtype=np.uint8) for p in proofs]
         batch = len(ds)
@@ -596,10 +604,6 @@ class Context:
         dls = (C.c_size_t * batch)(*[d.size for d in ds])
         pps = (u8p * batch)(*[p.ctypes.data_as(u8p) for p in ps])
         pls = (C.c_size_t * batch)(*[len(p) for p in proofs])
-        acc, accp, nacc = None, None, 0
-        if acceptable is not None:
-            acc = np.ascontiguousarray(np.stack([np.asarray(a, dtype=np.uint32) for a in acceptable]), dtype=np.uint32)
-            accp, nacc = acc.ctypes.data_as(C.POINTER(C.c_uint32)), acc.shape[0]
         cb = AUX_ASSERTIONS_BATCH()
         if aux_values_fn is not None:
             nv = _aux_value_count(ds[0])
@@ -617,10 +621,33 @@ class Context:
                     traceback.print_exc()
                     return 1
             cb = AUX_ASSERTIONS_BATCH(cb_values)
+        return batch, dps, dls, pps, pls, cb, (ds, ps)
+
+    def verify_air_batch(self, descs, proofs, hash_id, acceptable=None, aux_values_fn=None):
+        """wf_verify_air_batch: the verdict (VERIFY_*) of each proof in `proofs` (bytes) against the description of the same
+        index in `descs` (one AIR structure). acceptable: None (accept the options a proof carries) or a list of opts[9] arrays.
+        aux_values_fn(j, rand [nr, d], values [nv, d]) -> values: Air::get_aux_assertions of proof j. Returns a uint32 array."""
+        batch, dps, dls, pps, pls, cb, _keep = self._air_batch_args(descs, proofs, aux_values_fn)
+        acc, accp, nacc = None, None, 0
+        if acceptable is not None:
+            acc = np.ascontiguousarray(np.stack([np.asarray(a, dtype=np.uint32) for a in acceptable]), dtype=np.uint32)
+            accp, nacc = acc.ctypes.data_as(C.POINTER(C.c_uint32)), acc.shape[0]
         out = np.zeros(batch, dtype=np.uint32)
         self.check(self.L.wf_verify_air_batch(self.h, batch, dps, dls, pps, pls, int(hash_id), accp, nacc, cb, None,
                                               out.ctypes.data_as(C.POINTER(C.c_uint32))))
         return out
+
+    def verify_air_batch_min_security(self, descs, proofs, hash_id, regime, min_bits, aux_values_fn=None):
+        """wf_verify_air_batch_min_security: verify_air_batch under AcceptableOptions::MinConjecturedSecurity(min_bits)
+        (regime SECURITY_CONJECTURED) or MinProvenSecurity(min_bits) (SECURITY_PROVEN). Returns (verdicts, bits): uint32 arrays;
+        bits[j] is the conjectured bits or max(ldr, udr) of proof j, 0xffffffff for a proof refused before the check."""
+        batch, dps, dls, pps, pls, cb, _keep = self._air_batch_args(descs, proofs, aux_values_fn)
+        out = np.zeros(batch, dtype=np.uint32)
+        bits = np.zeros(batch, dtype=np.uint32)
+        self.check(self.L.wf_verify_air_batch_min_security(self.h, batch, dps, dls, pps, pls, int(hash_id), int(regime), int(min_bits),
+                                                           cb, None, out.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                                           bits.ctypes.data_as(C.POINTER(C.c_uint32))))
+        return out, bits
 
     def fri_verify_batch(self, hash_id, ext, folding, rem_max_deg, blowup, max_poly_degree, proofs, commitments, positions,
                          evaluations, coin_seeds=None):
@@ -937,6 +964,32 @@ def host_merge_with_int(hash_id, seed, value):
     o = np.zeros(32, dtype=np.uint8)
     lib().wf_host_merge_with_int(hash_id, tp, value, o.ctypes.data_as(u8p))
     return o.tobytes()
+
+
+def security_estimate(opts, trace_length, collision_resistance, num_constraints, num_committed_polys):
+    """wf_security_estimate: ConjecturedSecurity::compute and ProvenSecurity::compute for the Goldilocks field, without a
+    device. opts: an opts[9] vector (words 0-7 are read). Returns (conjectured, proven ldr, proven udr); WfError when the
+    arguments are out of range."""
+    o = np.zeros(9, dtype=np.uint32)
+    w = np.asarray(opts, dtype=np.uint32).reshape(-1)
+    o[:w.size] = w[:9]
+    out = [C.c_uint32() for _ in range(3)]
+    rc = lib().wf_security_estimate(o.ctypes.data_as(C.POINTER(C.c_uint32)), int(trace_length), int(collision_resistance),
+                                    int(num_constraints), int(num_committed_polys), C.byref(out[0]), C.byref(out[1]), C.byref(out[2]))
+    if rc != 0:
+        raise WfError(rc, "wf_security_estimate: arguments out of range")
+    return out[0].value, out[1].value, out[2].value
+
+
+def proof_security(hash_id, proof):
+    """wf_proof_security: Proof::conjectured_security / proven_security of a serialized proof under hash_id, without a device.
+    Returns (conjectured, proven ldr, proven udr); WfError for a context that does not deserialize or an unknown hash."""
+    p = np.frombuffer(bytes(proof), dtype=np.uint8) if len(proof) else np.zeros(1, dtype=np.uint8)
+    out = [C.c_uint32() for _ in range(3)]
+    rc = lib().wf_proof_security(int(hash_id), p.ctypes.data_as(u8p), len(proof), C.byref(out[0]), C.byref(out[1]), C.byref(out[2]))
+    if rc != 0:
+        raise WfError(rc, "wf_proof_security: the proof's context does not deserialize, or the hash is unknown")
+    return out[0].value, out[1].value, out[2].value
 
 
 def air_check(desc, log_n, blowup):

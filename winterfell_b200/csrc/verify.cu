@@ -4,7 +4,8 @@
 // and kernels, and the batch runner (run_plan).
 //
 // Host, per proof in batch order: parse the proof bytes (the inverse of prove_air's writer), check the options against the
-// acceptable set, check the AIR at the trace length the proof declares, replay the transcript (PublicCoin), check the OOD
+// acceptable set or the proof's security estimate against a minimum (security.hpp), check the AIR at the trace length the
+// proof declares, replay the transcript (PublicCoin), check the OOD
 // consistency (verifier/src/evaluator.rs) and turn every Merkle opening into a merge schedule without hashing anything.
 // Device, once per batch (one upload, one download, one synchronisation): the leaf hashes of every opened row
 // (commit_hash_rows), one merge launch per tree level for every tree of every proof (commit_merge_ops), the root compares,
@@ -20,6 +21,7 @@
 #include "internal.hpp"
 #include "air_host.hpp"
 #include "minidft.cuh"
+#include "security.hpp"
 
 namespace {
 
@@ -300,27 +302,49 @@ struct Parsed {
     u64 nonce = 0;
 };
 
-// Proof::from_bytes with the oracle's order of checks: WF_VERIFY_ACCEPT when the bytes parse. The Context it starts with is
-// the inverse of write_context (air_host.hpp)
-u32 parse_proof(const AirHost& air, int hash_id, const u8* proof, size_t len, Parsed& pp) {
-    Reader r{proof, len};
-    const u8 mw = r.u8_(), aw = r.u8_(), ar = r.u8_(), logn = r.u8_();
+// The Context at the head of a proof (context.rs:159-184), the inverse of write_context (air_host.hpp), read without checks:
+// head_ok when the bytes up to the modulus are there, ok when the options and the constraint count are too
+struct ProofContext {
+    u8 mw = 0, aw = 0, ar = 0, logn = 0, ml = 0;
+    const u8* mod = nullptr;
+    Options o{};
+    u64 ncons = 0;
+    bool head_ok = false, ok = false;
+    bool goldilocks() const {
+        const u64 p = GL_P;
+        return ml == 8 && !memcmp(mod, &p, 8);
+    }
+    // the options' asserts, TraceInfo::read_from (2^logn >= 8) and the two-adicity of the field
+    bool in_range() const { return options_in_range(o) && logn >= 3 && logn + log2_ceil(o.blowup) <= 32; }
+};
+void read_context(Reader& r, int hash_id, ProofContext& cx) {
+    cx.mw = r.u8_(); cx.aw = r.u8_(); cx.ar = r.u8_(); cx.logn = r.u8_();
     const u64 meta = r.le(2);
     r.take(meta);
-    const u8 ml = r.u8_();
-    const u8* mod = r.take(ml);
-    const u64 p = GL_P;
-    if (!r.ok || ml != 8 || memcmp(mod, &p, 8) || aw != air.aw || ar != air.nr) return WF_VERIFY_CONTEXT;
-    Options& o = pp.o;
+    cx.ml = r.u8_();
+    cx.mod = r.take(cx.ml);
+    cx.head_ok = r.ok;
+    Options& o = cx.o;
     o.num_queries = r.u8_(); o.blowup = r.u8_(); o.grinding = r.u8_(); o.ext = r.u8_(); o.folding = r.u8_();
     o.rem_max_deg = r.u8_(); o.batch_c = r.u8_(); o.batch_d = r.u8_(); o.num_partitions = r.u8_(); o.hash_rate = r.u8_();
     o.hash_id = hash_id;
-    const u64 ncons = r.usize();
-    if (!r.ok) return WF_VERIFY_MALFORMED;
-    // the options' asserts, TraceInfo::read_from (2^logn >= 8) and the two-adicity of the field
-    if (!options_in_range(o)) return WF_VERIFY_MALFORMED;
+    cx.ncons = r.usize();
+    cx.ok = r.ok;
+}
+
+// Proof::from_bytes with the oracle's order of checks: WF_VERIFY_ACCEPT when the bytes parse
+u32 parse_proof(const AirHost& air, int hash_id, const u8* proof, size_t len, Parsed& pp) {
+    Reader r{proof, len};
+    ProofContext cx;
+    read_context(r, hash_id, cx);
+    const u8 mw = cx.mw, logn = cx.logn;
+    if (!cx.head_ok || !cx.goldilocks() || cx.aw != air.aw || cx.ar != air.nr) return WF_VERIFY_CONTEXT;
+    if (!cx.ok) return WF_VERIFY_MALFORMED;
+    Options& o = pp.o;
+    o = cx.o;
+    const u64 ncons = cx.ncons;
+    if (!cx.in_range()) return WF_VERIFY_MALFORMED;
     const u32 lb = log2_ceil(o.blowup);
-    if (logn < 3 || logn + lb > 32) return WF_VERIFY_MALFORMED;
     pp.logn = logn;
     const size_t n = (size_t)1 << logn, N = n << lb;
     if (mw != air.w || ncons != air.num_constraints() || o.ext < 1 || o.ext > 3) return WF_VERIFY_CONTEXT;
@@ -1027,11 +1051,22 @@ void fri_host_part(const FriShape& s, u32 j, const u8* proof, size_t len, const 
                 std::vector<u64>(positions, positions + k), cur, fail);
 }
 
-}  // namespace
+// The acceptance policy of verifier::verify (AcceptableOptions, verifier/src/lib.rs:324-358): an OptionSet (opts, NULL: any
+// options), or a minimum security level in bits under one regime (regime 0: none). bits (may be NULL): per proof, the bits
+// the policy weighed, ~0u where the proof was refused before the check.
+struct Policy {
+    const uint32_t* opts = nullptr;
+    u32 num_opts = 0;
+    int regime = 0;
+    u32 min_bits = 0;
+    uint32_t* bits = nullptr;
+};
 
-extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
-                                   const uint8_t* const* proofs, const size_t* proof_lens, int hash_id, const uint32_t* acceptable_opts,
-                                   uint32_t num_acceptable, wf_aux_assertions_batch_fn aux_assertions, void* aux_user, uint32_t* verdicts) {
+int verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens, const uint8_t* const* proofs,
+                     const size_t* proof_lens, int hash_id, const Policy& pol, wf_aux_assertions_batch_fn aux_assertions, void* aux_user,
+                     uint32_t* verdicts) {
+    const uint32_t* acceptable_opts = pol.opts;
+    const u32 num_acceptable = pol.num_opts;
     if (!ctx || batch == 0 || !air_descs || !air_desc_lens || !proofs || !proof_lens || !verdicts || (acceptable_opts && !num_acceptable))
         return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     if (!WF_HASH_IS_KNOWN(hash_id)) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "unknown hash %d", hash_id);
@@ -1051,13 +1086,25 @@ extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* 
     const Call call{ctx, hash_id, aux_assertions, aux_user};
     Plan pl;
     std::vector<u32> fail(batch, NO_FAIL);
+    wf_security::EstimateCache estimates;
     for (u32 j = 0; j < batch; j++) {
+        if (pol.bits) pol.bits[j] = ~0u;
         Parsed pp;
         u32 v = parse_proof(airs[j], hash_id, proofs[j], proof_lens[j], pp);
         if (v == WF_VERIFY_ACCEPT && acceptable_opts) {
             bool ok = false;
             for (u32 i = 0; i < num_acceptable && !ok; i++) ok = options_match(pp.o, acceptable_opts + 9 * i);
             if (!ok) v = WF_VERIFY_UNACCEPTABLE_OPTIONS;
+        }
+        if (v == WF_VERIFY_ACCEPT && pol.regime) {
+            // Proof::conjectured_security / proven_security (air/src/proof/mod.rs:96-126). parse_proof has checked that the
+            // context's widths and constraint count are the AIR's.
+            const wf_security::Estimate e = estimates.get(pp.o, (u64)1 << pp.logn, wf_security::collision_resistance(hash_id),
+                                                          airs[j].num_constraints(), (u64)airs[j].w + airs[j].aw + pp.o.blowup);
+            const bool conj = pol.regime == WF_SECURITY_CONJECTURED;
+            if (pol.bits) pol.bits[j] = conj ? e.conjectured : std::max(e.ldr, e.udr);
+            if (conj && !wf_security::conjectured_at_least(e, pol.min_bits)) v = WF_VERIFY_INSUFFICIENT_CONJECTURED_SECURITY;
+            if (!conj && !wf_security::proven_at_least(e, pol.min_bits)) v = WF_VERIFY_INSUFFICIENT_PROVEN_SECURITY;
         }
         if (v == WF_VERIFY_ACCEPT) {   // Air::new at the declared length: what the reference panics on
             wf_ctx note{};
@@ -1073,6 +1120,66 @@ extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* 
 
     CKI(run_plan(ctx, hash_id, pl, fail, batch, FULL_PROOF_CODES, true, verdicts));
     wf_mark(ctx, "verify_device");
+    return WF_OK;
+}
+
+}  // namespace
+
+extern "C" int wf_verify_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
+                                   const uint8_t* const* proofs, const size_t* proof_lens, int hash_id, const uint32_t* acceptable_opts,
+                                   uint32_t num_acceptable, wf_aux_assertions_batch_fn aux_assertions, void* aux_user, uint32_t* verdicts) {
+    Policy pol;
+    pol.opts = acceptable_opts;
+    pol.num_opts = num_acceptable;
+    return verify_air_batch(ctx, batch, air_descs, air_desc_lens, proofs, proof_lens, hash_id, pol, aux_assertions, aux_user, verdicts);
+}
+
+extern "C" int wf_verify_air_batch_min_security(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
+                                                const uint8_t* const* proofs, const size_t* proof_lens, int hash_id, int regime,
+                                                uint32_t min_bits, wf_aux_assertions_batch_fn aux_assertions, void* aux_user,
+                                                uint32_t* verdicts, uint32_t* security_bits) {
+    if (regime != WF_SECURITY_CONJECTURED && regime != WF_SECURITY_PROVEN)
+        return wf_fail(ctx, WF_ERR_INVALID, "unknown security regime %d", regime);
+    Policy pol;
+    pol.regime = regime;
+    pol.min_bits = min_bits;
+    pol.bits = security_bits;
+    return verify_air_batch(ctx, batch, air_descs, air_desc_lens, proofs, proof_lens, hash_id, pol, aux_assertions, aux_user, verdicts);
+}
+
+extern "C" int wf_security_estimate(const uint32_t* opts, uint64_t trace_length, uint32_t collision_resistance, uint64_t num_constraints,
+                                    uint64_t num_committed_polys, uint32_t* conjectured, uint32_t* proven_ldr, uint32_t* proven_udr) {
+    if (!opts || !conjectured || !proven_ldr || !proven_udr) return WF_ERR_INVALID;
+    Options o = options_from_words(opts);
+    o.num_partitions = 1; o.hash_rate = 1;   // word 8 is not read
+    if (!options_in_range(o) || o.ext < 1 || o.ext > 3) return WF_ERR_INVALID;
+    if (trace_length < 8 || trace_length > ((u64)1 << 32) || (trace_length & (trace_length - 1))) return WF_ERR_INVALID;
+    if (num_constraints == 0 || num_committed_polys == 0) return WF_ERR_INVALID;
+    const wf_security::Estimate e = wf_security::estimate(o, trace_length, collision_resistance, num_constraints, num_committed_polys);
+    *conjectured = e.conjectured;
+    *proven_ldr = e.ldr;
+    *proven_udr = e.udr;
+    return WF_OK;
+}
+
+extern "C" int wf_proof_security(int hash_id, const uint8_t* proof, size_t len, uint32_t* conjectured, uint32_t* proven_ldr,
+                                 uint32_t* proven_udr) {
+    if (!proof || !conjectured || !proven_ldr || !proven_udr) return WF_ERR_INVALID;
+    const u32 cr = wf_security::collision_resistance(hash_id);
+    if (!WF_HASH_IS_KNOWN(hash_id) || cr == 0) return WF_ERR_UNSUPPORTED;
+    Reader r{proof, len};
+    ProofContext cx;
+    read_context(r, hash_id, cx);
+    // what Context::read_from refuses or panics on (TraceInfo::read_from and new_multi_segment, trace_info.rs:84-130,266-330;
+    // an empty modulus; ProofOptions::new's ranges), and a field other than Goldilocks. The rest of the proof is not read.
+    if (!cx.ok || cx.mw == 0 || (u32)cx.mw + cx.aw >= 255 || (cx.aw != 0) != (cx.ar != 0) || !cx.in_range() || cx.o.ext < 1 ||
+        cx.o.ext > 3 || !cx.goldilocks())
+        return WF_ERR_INVALID;
+    const wf_security::Estimate e =
+        wf_security::estimate(cx.o, (u64)1 << cx.logn, cr, cx.ncons, (u64)cx.mw + cx.aw + cx.o.blowup);
+    *conjectured = e.conjectured;
+    *proven_ldr = e.ldr;
+    *proven_udr = e.udr;
     return WF_OK;
 }
 
