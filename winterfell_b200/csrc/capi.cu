@@ -1165,29 +1165,55 @@ int wf_fri_free(wf_ctx* ctx, wf_fri* f) {
 
 }  // extern "C"
 // What a commit phase under construction owns: the wf_fri with its finished layers, the tree of the layer in flight and the
-// scratch buffers — all of it returns to the pool on every early error return.
+// scratch buffers — all of it returns to the pool on every early error return. Both commit phases below start it and end it
+// (the remainder) the same way; their layer loops differ in when they synchronise.
 struct FriBuild {
     wf_ctx* ctx;
     wf_fri* f;
     wf_tree* t = nullptr;
     DevScratch tmp;
-    FriBuild(wf_ctx* c, wf_fri* fr) : ctx(c), f(fr), tmp(c) {}
+    FriBuild(wf_ctx* c, int hash_id, const wf_mat* evals, int d, uint32_t folding, uint32_t blowup) : ctx(c), f(new wf_fri()), tmp(c) {
+        f->hash_id = hash_id; f->d = d; f->folding = folding; f->blowup = blowup;
+        f->ld = evals->m.W;  // d base columns live in one segment of width W >= d
+    }
     ~FriBuild() { if (t) wf_tree_free(ctx, t); if (f) wf_fri_free(ctx, f); }
+    // the remainder (fri/src/prover/mod.rs:230-239) from the last layer `cur` (len x ld words, freed here): copied down (one
+    // synchronisation, behind whatever the caller enqueued before), its d of ld words per point, the inverse DFT, the first
+    // len / blowup coefficients reversed; *rc <- their hash
+    int remainder(void* cur, size_t len, Digest* rc) {
+        const int d = f->d, ld = f->ld;
+        std::vector<u64> raw(len * ld), v(len * d);
+        CK(cudaMemcpyAsync(raw.data(), cur, len * ld * 8, cudaMemcpyDeviceToHost, ctx->st));
+        CK(cudaStreamSynchronize(ctx->st));
+        tmp.free(cur);
+        for (size_t i = 0; i < len; i++)
+            for (int c = 0; c < d; c++) v[i * d + c] = raw[i * ld + c];
+        wf_host_dft(v, len, d, true, GL_GENERATOR);
+        const size_t rsize = len / f->blowup;
+        f->remainder.resize(rsize * d);
+        for (size_t i = 0; i < rsize; i++)
+            for (int c = 0; c < d; c++) f->remainder[i * d + c] = v[(rsize - 1 - i) * d + c];
+        *rc = hh_hash_elements(f->hash_id, f->remainder.data(), f->remainder.size());
+        return WF_OK;
+    }
 };
+// the argument checks of both commit phases (the callbacks of wf_fri_build_layers apart)
+static int fri_build_check(wf_ctx* ctx, const wf_mat* evals, int d, uint32_t folding, wf_fri** out) {
+    if (!ctx || !evals || !out) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    if (d < 1 || d > 3 || (int)evals->m.cols != d) return wf_fail(ctx, WF_ERR_INVALID, "evaluations must have ext_degree base columns");
+    if (folding != 2 && folding != 4 && folding != 8 && folding != 16) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "folding factor %u", folding);
+    u32 logL;
+    if (log2_exact(evals->m.rows, &logL)) return wf_fail(ctx, WF_ERR_INVALID, "domain size must be a power of two");
+    return WF_OK;
+}
 extern "C" {
 int wf_fri_build_layers(wf_ctx* ctx, int hash_id, const wf_mat* evals, int d, uint32_t folding, uint32_t rem_max_deg,
                         uint32_t blowup, wf_fri_commit_fn commit, wf_fri_draw_fn draw_alpha, void* user, wf_fri** out) {
-    if (!ctx || !evals || !commit || !draw_alpha || !out) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
-    if (d < 1 || d > 3 || (int)evals->m.cols != d) return wf_fail(ctx, WF_ERR_INVALID, "evaluations must have ext_degree base columns");
-    if (folding != 2 && folding != 4 && folding != 8 && folding != 16) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "folding factor %u", folding);
+    if (!commit || !draw_alpha) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
+    CKI(fri_build_check(ctx, evals, d, folding, out));
     size_t len = evals->m.rows;
-    u32 logL;
-    if (log2_exact(len, &logL)) return wf_fail(ctx, WF_ERR_INVALID, "domain size must be a power of two");
-    wf_fri* f = new wf_fri();
-    FriBuild g(ctx, f);
-    f->hash_id = hash_id; f->d = d; f->folding = folding; f->blowup = blowup;
-    f->ld = evals->m.W;  // d base columns live in one segment of width W >= d
-    const int ld = f->ld;
+    FriBuild g(ctx, hash_id, evals, d, folding, blowup);
+    const int ld = g.f->ld;
     // layer 0 evaluations: copy of the segment (the prover keeps its own copy, fri/src/prover/mod.rs:217-221)
     void* cur;
     CKI(g.tmp.alloc(len * ld * 8, &cur));
@@ -1213,27 +1239,16 @@ int wf_fri_build_layers(wf_ctx* ctx, int hash_id, const wf_mat* evals, int d, ui
         CKI(g.tmp.alloc(m * ld * 8, &nxt));
         CK(fri_fold_layer((u64*)cur, len, d, ld, (int)folding, alpha, master, (u64*)nxt, ld, ctx->st));
         ctx->launches++;
-        f->layers.push_back(FriLayer{(u64*)g.tmp.keep(cur), len, t});   // the wf_fri owns layer and tree from here
+        g.f->layers.push_back(FriLayer{(u64*)g.tmp.keep(cur), len, t});   // the wf_fri owns layer and tree from here
         g.t = nullptr;
         cur = nxt;
         len = m;
     }
-    // remainder (fri/src/prover/mod.rs:230-239)
-    std::vector<u64> raw(len * ld), v(len * d);
-    CK(cudaMemcpyAsync(raw.data(), cur, len * ld * 8, cudaMemcpyDeviceToHost, ctx->st));
-    CK(cudaStreamSynchronize(ctx->st));
-    g.tmp.free(cur);
-    for (size_t i = 0; i < len; i++)
-        for (int c = 0; c < d; c++) v[i * d + c] = raw[i * ld + c];
-    wf_host_dft(v, len, d, true, GL_GENERATOR);
-    size_t rsize = len / blowup;
-    f->remainder.resize(rsize * d);
-    for (size_t i = 0; i < rsize; i++)
-        for (int c = 0; c < d; c++) f->remainder[i * d + c] = v[(rsize - 1 - i) * d + c];
-    Digest rc = hh_hash_elements(hash_id, f->remainder.data(), f->remainder.size());
+    Digest rc;
+    CKI(g.remainder(cur, len, &rc));
     commit(user, rc.b);
-    g.f = nullptr;   // the caller's now
-    *out = f;
+    *out = g.f;   // the caller's now
+    g.f = nullptr;
     return WF_OK;
 }
 
@@ -1247,17 +1262,10 @@ int wf_fri_build_layers(wf_ctx* ctx, int hash_id, const wf_mat* evals, int d, ui
 // is left without a buffer, and wf_mat_free then releases only the handle. Else layer 0 is a copy (the caller keeps its matrix).
 int wf_fri_build_layers_coin(wf_ctx* ctx, int hash_id, const wf_mat* evals, int d, uint32_t folding, uint32_t rem_max_deg,
                              uint32_t blowup, PublicCoin& coin, std::vector<Digest>& commitments, wf_fri** out, wf_mat* consume) {
-    if (!ctx || !evals || !out) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
-    if (d < 1 || d > 3 || (int)evals->m.cols != d) return wf_fail(ctx, WF_ERR_INVALID, "evaluations must have ext_degree base columns");
-    if (folding != 2 && folding != 4 && folding != 8 && folding != 16) return wf_fail(ctx, WF_ERR_UNSUPPORTED, "folding factor %u", folding);
+    CKI(fri_build_check(ctx, evals, d, folding, out));
     size_t len = evals->m.rows;
-    u32 logL;
-    if (log2_exact(len, &logL)) return wf_fail(ctx, WF_ERR_INVALID, "domain size must be a power of two");
-    wf_fri* f = new wf_fri();
-    FriBuild g(ctx, f);
-    f->hash_id = hash_id; f->d = d; f->folding = folding; f->blowup = blowup;
-    f->ld = evals->m.W;
-    const int ld = f->ld;
+    FriBuild g(ctx, hash_id, evals, d, folding, blowup);
+    const int ld = g.f->ld;
     const size_t max_rem = (size_t)(rem_max_deg + 1) * blowup;  // fri/src/options.rs:85-93
     size_t nlayers = 0;
     for (size_t l = len; l > max_rem; l /= folding) nlayers++;
@@ -1292,17 +1300,16 @@ int wf_fri_build_layers_coin(wf_ctx* ctx, int hash_id, const wf_mat* evals, int 
         CKI(g.tmp.alloc(m * ld * 8, &nxt));
         CK(fri_fold_layer((u64*)cur, len, d, ld, (int)folding, nullptr, master, (u64*)nxt, ld, ctx->st, (const u64*)dalpha));
         ctx->launches++;
-        f->layers.push_back(FriLayer{(u64*)g.tmp.keep(cur), len, t});   // the wf_fri owns layer and tree from here
+        g.f->layers.push_back(FriLayer{(u64*)g.tmp.keep(cur), len, t});   // the wf_fri owns layer and tree from here
         g.t = nullptr;
         cur = nxt;
         len = m;
         layer++;
     }
-    std::vector<u64> raw(len * ld), v(len * d), log(std::max<size_t>(nlayers, 1) * 8);
-    CK(cudaMemcpyAsync(raw.data(), cur, len * ld * 8, cudaMemcpyDeviceToHost, ctx->st));
+    std::vector<u64> log(std::max<size_t>(nlayers, 1) * 8);
     if (nlayers) CK(cudaMemcpyAsync(log.data(), dlog, nlayers * 8 * 8, cudaMemcpyDeviceToHost, ctx->st));
-    CK(cudaStreamSynchronize(ctx->st));
-    g.tmp.free(cur);
+    Digest rc;
+    CKI(g.remainder(cur, len, &rc));   // the one synchronisation of the commit phase
     g.tmp.free(dstate); g.tmp.free(dalpha); g.tmp.free(dlog);
     // replay on the host coin: commit_fri_layer, draw_fri_alpha (prover/src/channel.rs:215-234)
     for (size_t l = 0; l < nlayers; l++) {
@@ -1315,19 +1322,10 @@ int wf_fri_build_layers_coin(wf_ctx* ctx, int hash_id, const wf_mat* evals, int 
         for (int k = 0; k < d; k++) ok = ok && alpha[k] == log[8 * l + 4 + k];
         if (!ok) return wf_fail(ctx, WF_ERR_STATE, "device and host FRI transcripts diverged at layer %zu", l);
     }
-    // remainder (fri/src/prover/mod.rs:230-239)
-    for (size_t i = 0; i < len; i++)
-        for (int c = 0; c < d; c++) v[i * d + c] = raw[i * ld + c];
-    wf_host_dft(v, len, d, true, GL_GENERATOR);
-    size_t rsize = len / blowup;
-    f->remainder.resize(rsize * d);
-    for (size_t i = 0; i < rsize; i++)
-        for (int c = 0; c < d; c++) f->remainder[i * d + c] = v[(rsize - 1 - i) * d + c];
-    Digest rc = hh_hash_elements(hash_id, f->remainder.data(), f->remainder.size());
     commitments.push_back(rc);
     coin.reseed(rc);
-    g.f = nullptr;   // the caller's now
-    *out = f;
+    *out = g.f;   // the caller's now
+    g.f = nullptr;
     return WF_OK;
 }
 extern "C" {

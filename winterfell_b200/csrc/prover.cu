@@ -1326,22 +1326,101 @@ static int validation_result(wf_ctx* ctx, int r, const TraceReport& rep) {
 }
 
 // Device objects of one proof: whatever is still registered when prove_air leaves (normally or through
-// an error return) goes back to the context's pool.
+// an error return) goes back to the context's pool. `held` trees and `bufs` buffers are owned by value.
 struct ProofScope {
     wf_ctx* ctx;
     std::vector<wf_mat**> mats;
     std::vector<wf_tree**> trees;
+    std::vector<wf_tree*> held;
+    DevScratch bufs;
     wf_fri** fri = nullptr;
-    explicit ProofScope(wf_ctx* c) : ctx(c) {}
+    explicit ProofScope(wf_ctx* c) : ctx(c), bufs(c) {}
     void own(std::initializer_list<wf_mat**> l) { mats.insert(mats.end(), l); }
     void own(std::initializer_list<wf_tree**> l) { trees.insert(trees.end(), l); }
     void drop(wf_mat*& m) { wf_mat_free(ctx, m); m = nullptr; }
     ~ProofScope() {
+        for (wf_tree* t : held) wf_tree_free(ctx, t);
         if (fri && *fri) wf_fri_free(ctx, *fri);
         for (wf_mat** m : mats) if (*m) wf_mat_free(ctx, *m);
         for (wf_tree** t : trees) if (*t) wf_tree_free(ctx, *t);
     }
 };
+
+// ---- the steps both provers (prove_air, prove_sharded) take in the same way ----
+
+// Air::get_aux_rand_elements (air/src/air/mod.rs:292-306): rnd <- nr elements drawn from the coin, [nr][D] canonical;
+// rnd_user <- the same as the user's callbacks see them (x * R, R = 2^64 mod p, when `mont`)
+template <int D>
+static void draw_aux_rand(PublicCoin& coin, u32 nr, int mont, std::vector<u64>& rnd, std::vector<u64>& rnd_user) {
+    for (u32 i = 0; i < nr; i++) { GlExt<D> e = draw_ext<D>(coin); for (int q = 0; q < D; q++) rnd.push_back(e.v[q]); }
+    rnd_user = rnd;
+    if (mont) for (u64& v : rnd_user) v = gl_mul(v, 0xFFFFFFFFULL);
+}
+// Air::get_aux_assertions(aux_rand_elements) (air/src/air/mod.rs:279): the callback (none: nothing to do) rewrites the
+// aux assertion values of `air`
+static int apply_aux_assertions(wf_ctx* ctx, AirHost& air, wf_aux_assertions_fn aux_assertions, void* aux_user,
+                                const std::vector<u64>& rnd_user, int D, int mont) {
+    if (!aux_assertions) return WF_OK;
+    std::vector<u64> vals = get_aux_assertion_words(air, D, mont);
+    if (aux_assertions(aux_user, rnd_user.data(), vals.data()) != 0) return wf_fail(ctx, WF_ERR_INVALID, "aux assertion callback failed");
+    if (!set_aux_assertion_words(air, vals.data(), D, mont))
+        return wf_fail(ctx, WF_ERR_INVALID, "aux assertion value is not a canonical field element");
+    return WF_OK;
+}
+
+// The out-of-domain frames (lib.rs:392-401) and their serialisation
+template <int D>
+struct OodFrame { std::vector<GlExt<D>> t_cur, t_nxt, q_cur, q_nxt; ByteVec t, q; };
+// f.t_cur / f.t_nxt: the main columns at z / zg; q[0..1] (a[0..1]: the aux segment's, or none): the composition columns'
+// base components at z / zg. Trace frame rows = main then aux columns (ood_frame.rs:40-72); the coin is reseeded with the
+// frames' hash, which is not added to the commitments.
+template <int D>
+static void ood_frame(Channel& ch, OodFrame<D>& f, const std::vector<GlExt<D>>* q, const std::vector<GlExt<D>>* a) {
+    if (a) {
+        auto a_cur = ext_from_components<D>(a[0]), a_nxt = ext_from_components<D>(a[1]);
+        f.t_cur.insert(f.t_cur.end(), a_cur.begin(), a_cur.end());
+        f.t_nxt.insert(f.t_nxt.end(), a_nxt.begin(), a_nxt.end());
+    }
+    f.q_cur = ext_from_components<D>(q[0]);
+    f.q_nxt = ext_from_components<D>(q[1]);
+    ch.coin.reseed(ood_frames<D>(ch.coin.hash_id, f.t_cur, f.t_nxt, f.q_cur, f.q_nxt, &f.t, &f.q));
+}
+
+// grinding + query positions (channel.rs:151-184; serial semantics: smallest nonce) over an LDE domain of N points
+static int grind_and_query(wf_ctx* ctx, Channel& ch, const Options& o, size_t N, u64* nonce, std::vector<u64>& pos) {
+    CKI(grind_on_device(ctx, ch.coin.hash_id, ch.coin.seed, o.grinding, nonce));
+    if (ch.coin.check_leading_zeros(*nonce) < o.grinding) return wf_fail(ctx, WF_ERR_STATE, "grinding self-check failed");
+    if (!query_positions(ch.coin, o.num_queries, N, *nonce, pos)) return wf_fail(ctx, WF_ERR_STATE, "failed to draw query positions");
+    return WF_OK;
+}
+
+// The ids in a GatherBatch of the opened rows and their Merkle openings: trace, constraint, aux (with an aux segment). The
+// rows at positions `p` are queued here, the openings by the caller.
+struct QueryIds {
+    size_t tr_rows, cr_rows, ar_rows, tr_dig = 0, cr_dig = 0, ar_dig = 0;
+    QueryIds(GatherBatch& gb, const SegMatrix& t, const SegMatrix& c, const SegMatrix* a, const std::vector<u64>& p)
+        : tr_rows(gb.add_rows(t, p)), cr_rows(gb.add_rows(c, p)), ar_rows(a ? gb.add_rows(*a, p) : 0) {}
+};
+// The proof object (lib.rs:464-489; air/src/proof/mod.rs:189-200) once every gather of `gb` has run. `before`: the sharded
+// prover's FRI layers folded on its shards, which come ahead of the layers of `fri`.
+template <int D>
+static void write_proof(const AirHost& air, u32 log_n, const Options& o, const Channel& ch, const std::vector<u64>& pos,
+                        const GatherBatch& gb, const QueryIds& id, const OodFrame<D>& ood, const wf_fri* fri,
+                        const FriProofPlan& fplan, const FriProofPlan* before, u64 nonce, std::vector<u8>& proof_out) {
+    ByteVec w;
+    write_context(w, air, log_n, o);
+    w.u8_((u8)pos.size());
+    w.u16_((uint16_t)ch.commitments.v.size());
+    w.bytes(ch.commitments.v.data(), ch.commitments.v.size());
+    write_queries(gb, id.tr_rows, id.tr_dig, pos.size() * air.w, w);
+    if (air.aw) write_queries(gb, id.ar_rows, id.ar_dig, pos.size() * air.aw * D, w);  // trace_lde/default/mod.rs:199-218
+    write_queries(gb, id.cr_rows, id.cr_dig, pos.size() * air.num_comp_cols((size_t)1 << log_n) * D, w);
+    w.u16_((uint16_t)ood.t.v.size()); w.bytes(ood.t.v.data(), ood.t.v.size());
+    w.u16_((uint16_t)ood.q.v.size()); w.bytes(ood.q.v.data(), ood.q.v.size());
+    wf_fri_finish_proof(fri, gb, fplan, w, before);
+    w.u64_(nonce);
+    proof_out.swap(w.v);
+}
 
 template <int D>
 int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont, u32 log_n,
@@ -1395,11 +1474,9 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
 
     // ---- 1b. auxiliary segment (lib.rs:309-349; Air::get_aux_rand_elements air/src/air/mod.rs:292-306;
     //          DefaultTraceLde::set_aux_trace trace_lde/default/mod.rs:140-166) ----
-    std::vector<u64> rnd_flat;  // [nr][D], canonical
+    std::vector<u64> rnd_flat, rnd_user;  // [nr][D], canonical / as the callbacks see them
     if (aw) {
-        for (u32 i = 0; i < air.nr; i++) { GlExt<D> e = draw_ext<D>(ch.coin); for (int q = 0; q < D; q++) rnd_flat.push_back(e.v[q]); }
-        std::vector<u64> rnd_user = rnd_flat;
-        if (mont) for (u64& v : rnd_user) v = gl_mul(v, 0xFFFFFFFFULL);  // x * R, R = 2^64 mod p
+        draw_aux_rand<D>(ch.coin, air.nr, mont, rnd_flat, rnd_user);
         std::vector<u64> aux_host;  // [aw][n][D]: ColMatrix<E>, one Vec<E> per column
         if (aux_build) {
             // the described build reads the main trace's evaluations: kept from the device trace, or one forward NTT of the
@@ -1412,12 +1489,7 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
             aux_host.resize((size_t)aw * n * D);
             if (aux_builder(aux_user, rnd_user.data(), aux_host.data()) != 0) return wf_fail(ctx, WF_ERR_INVALID, "aux trace builder failed");
         }
-        if (aux_assertions) {
-            std::vector<u64> vals = get_aux_assertion_words(air_dyn, D, mont);
-            if (aux_assertions(aux_user, rnd_user.data(), vals.data()) != 0) return wf_fail(ctx, WF_ERR_INVALID, "aux assertion callback failed");
-            if (!set_aux_assertion_words(air_dyn, vals.data(), D, mont))
-                return wf_fail(ctx, WF_ERR_INVALID, "aux assertion value is not a canonical field element");
-        }
+        CKI(apply_aux_assertions(ctx, air_dyn, aux_assertions, aux_user, rnd_user, D, mont));
         if (!aux_build) {
             // E column j -> D base columns j*D + q (rows of the LDE then serialise exactly like [E] rows)
             std::vector<const u64*> cols(aw);
@@ -1469,16 +1541,9 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
         if (aw) mats.push_back(apolys);
         CKI(ood_eval<D>(ctx, mats, z, zg, ood));
     }
-    std::vector<GlExt<D>>&t_cur = ood[0], &t_nxt = ood[1];
-    std::vector<GlExt<D>> q_cur = ext_from_components<D>(ood[2]), q_nxt = ext_from_components<D>(ood[3]);
-    if (aw) {  // trace frame rows = main columns then aux columns (ood_frame.rs:40-72)
-        auto a_cur = ext_from_components<D>(ood[4]), a_nxt = ext_from_components<D>(ood[5]);
-        t_cur.insert(t_cur.end(), a_cur.begin(), a_cur.end());
-        t_nxt.insert(t_nxt.end(), a_nxt.begin(), a_nxt.end());
-    }
+    OodFrame<D> of{std::move(ood[0]), std::move(ood[1])};
+    ood_frame<D>(ch, of, &ood[2], aw ? &ood[4] : nullptr);
     const u32 ct = c + aw;
-    ByteVec ood_t, ood_q;
-    ch.coin.reseed(ood_frames<D>(h, t_cur, t_nxt, q_cur, q_nxt, &ood_t, &ood_q));  // not added to the commitments
     wf_mark(ctx, "ood_frames");
     // ---- 5. DEEP composition (lib.rs:403-440), coefficient form ----
     std::vector<GlExt<D>> dc = draw_coeffs<D>(ch.coin, o.batch_d, ct + kc);
@@ -1492,40 +1557,23 @@ int prove_air(wf_ctx* ctx, const AirHost& air_in, const uint64_t* const* trace_c
     }
     scope.drop(deep);
     wf_mark(ctx, "fri_layers");
-    // ---- 7. grinding + query positions (channel.rs:151-184; serial semantics: smallest nonce) ----
+    // ---- 7. grinding + query positions ----
     u64 nonce;
-    CKI(grind_on_device(ctx, h, ch.coin.seed, o.grinding, &nonce));
-    if (ch.coin.check_leading_zeros(nonce) < o.grinding) return wf_fail(ctx, WF_ERR_STATE, "grinding self-check failed");
     std::vector<u64> pos;
-    if (!query_positions(ch.coin, o.num_queries, N, nonce, pos)) return wf_fail(ctx, WF_ERR_STATE, "failed to draw query positions");
+    CKI(grind_and_query(ctx, ch, o, N, &nonce, pos));
     wf_mark(ctx, "grinding");
-    // ---- 8. proof object (lib.rs:464-489; air/src/proof/mod.rs:189-200) ----
-    ByteVec w;
-    write_context(w, air, log_n, o);
-    w.u8_((u8)pos.size());
-    w.u16_((uint16_t)ch.commitments.v.size());
-    w.bytes(ch.commitments.v.data(), ch.commitments.v.size());
-    // every gather of the proof (trace rows, constraint rows, all FRI layers + their Merkle paths)
-    // goes through one batch: one index upload, one download, one synchronisation
+    // ---- 8. proof object: every gather of the proof (trace rows, constraint rows, all FRI layers + their Merkle paths)
+    //         goes through one batch: one index upload, one download, one synchronisation ----
     GatherBatch gb;
     FriProofPlan fplan;
-    size_t tr_rows = gb.add_rows(lde->m, pos), cr_rows = gb.add_rows(clde->m, pos), tr_dig, cr_dig;
-    size_t ar_rows = 0, ar_dig = 0;
-    if (aw) ar_rows = gb.add_rows(alde->m, pos);
-    CKI(gb.add_opening(ctx, ttree, pos, &tr_dig));
-    CKI(gb.add_opening(ctx, ctree, pos, &cr_dig));
-    if (aw) CKI(gb.add_opening(ctx, atree, pos, &ar_dig));
+    QueryIds id(gb, lde->m, clde->m, aw ? &alde->m : nullptr, pos);
+    CKI(gb.add_opening(ctx, ttree, pos, &id.tr_dig));
+    CKI(gb.add_opening(ctx, ctree, pos, &id.cr_dig));
+    if (aw) CKI(gb.add_opening(ctx, atree, pos, &id.ar_dig));
     CKI(wf_fri_queue_proof(ctx, fri, pos, gb, fplan));
     CKI(gb.run(ctx));
-    write_queries(gb, tr_rows, tr_dig, pos.size() * c, w);
-    if (aw) write_queries(gb, ar_rows, ar_dig, pos.size() * aw * D, w);  // trace_lde/default/mod.rs:199-218
-    write_queries(gb, cr_rows, cr_dig, pos.size() * kc * D, w);
-    w.u16_((uint16_t)ood_t.v.size()); w.bytes(ood_t.v.data(), ood_t.v.size());
-    w.u16_((uint16_t)ood_q.v.size()); w.bytes(ood_q.v.data(), ood_q.v.size());
-    wf_fri_finish_proof(fri, gb, fplan, w);
-    w.u64_(nonce);
+    write_proof<D>(air, log_n, o, ch, pos, gb, id, of, fri, fplan, nullptr, nonce, proof_out);
     wf_mark(ctx, "queries_and_proof");
-    proof_out.swap(w.v);
     // `scope` returns every device object of this proof to the pool
     return WF_OK;
 }
@@ -1891,6 +1939,17 @@ static int shard_trace_lde(ShardCtx& sc, const uint64_t* const* local_cols, cons
     return WF_OK;
 }
 
+// dst (this rank's columns in 8-column segments) <- the evaluations of this rank's column polynomials on the trace domain
+static int evaluate_own_columns(wf_ctx* ctx, const wf_mat* polys, const SegMatrix& dst) {
+    wf_mat* ev;
+    CKI(wf_mat_evaluate(ctx, polys, &ev));
+    const cudaError_t e = layout_select_cols(ev->m, 0, dst, ctx->st);
+    ctx->launches++;
+    wf_mat_free(ctx, ev);
+    CK(e);
+    return WF_OK;
+}
+
 // *mtrace <- the whole n x c main trace on every rank (the aux build reads main rows i and i + 1 of every column): rank r
 // evaluates its columns (`polys`, none: NULL) on the trace domain and one all-gather by segment fills in everyone else's.
 static int gather_main_trace(ShardCtx& sc, const wf_mat* polys, u32 log_n, u32 c, const std::vector<u32>& seg0, const std::vector<u32>& segs,
@@ -1903,15 +1962,10 @@ static int gather_main_trace(ShardCtx& sc, const wf_mat* polys, u32 log_n, u32 c
     shard_columns(c, (u32)G, (u32)r, first, cl);
     CKI(wf_mat_alloc_w(ctx, n, c, 8, &mtrace));
     if (cl) {
-        wf_mat* ev;
-        CKI(wf_mat_evaluate(ctx, polys, &ev));
         SegMatrix dv = mtrace->m;
         dv.base += (size_t)fs * dv.seg_stride;
         dv.cols = cl;
-        const cudaError_t e = layout_select_cols(ev->m, 0, dv, ctx->st);
-        ctx->launches++;
-        wf_mat_free(ctx, ev);
-        CK(e);
+        CKI(evaluate_own_columns(ctx, polys, dv));
     }
     std::vector<int> sp, rp;
     std::vector<const void*> sv;
@@ -1958,14 +2012,7 @@ static int sharded_check_trace(ShardCtx& sc, const AirHost& air, const wf_mat* p
         part.aux = atrace;
     } else {
         CKI(wf_mat_alloc_w(ctx, n, cl, 8, &own));
-        if (cl) {
-            wf_mat* ev;
-            CKI(wf_mat_evaluate(ctx, polys, &ev));
-            const cudaError_t e = layout_select_cols(ev->m, 0, own->m, ctx->st);
-            ctx->launches++;
-            wf_mat_free(ctx, ev);
-            CK(e);
-        }
+        if (cl) CKI(evaluate_own_columns(ctx, polys, own->m));
         part.amain = own->m;
         CKI(wf_mat_alloc_w(ctx, nt + 1, air.w, 8, &rows));
         rows->m.rows = nt;   // row nt: the halo row
@@ -2021,7 +2068,8 @@ static int sharded_check_degrees(ShardCtx& sc, const AirHost& air, const wf_mat*
     u32 first, cnt;
     shard_columns(ncols, (u32)G, (u32)r, first, cnt);
     wf_mat *loc = nullptr, *mine = nullptr;
-    struct Free { wf_ctx* c; wf_mat** a; wf_mat** b; ~Free() { wf_mat_free(c, *a); wf_mat_free(c, *b); } } fr{ctx, &loc, &mine};
+    ProofScope scope(ctx);
+    scope.own({&loc, &mine});
     CKI(wf_mat_alloc_w(ctx, ce_per, ncols, 8, &loc));
     CKI(wf_transition_columns(ctx, air, lde, alde, rnd.data(), log_n, log_b, D, (size_t)r * ce_per, ce_per, loc->m));
     if (cnt) CKI(wf_mat_alloc_w(ctx, ce, cnt, 8, &mine));
@@ -2040,8 +2088,7 @@ static int sharded_check_degrees(ShardCtx& sc, const AirHost& air, const wf_mat*
         }
         CKI(sc.exchange(sp, sv, rp, rv, ce_per * 64));
     }
-    wf_mat_free(ctx, loc);
-    loc = nullptr;
+    scope.drop(loc);
     std::vector<u64> d1;
     if (cnt) CKI(wf_column_degrees(ctx, mine, d1));
     d1.resize(blk, 0);
@@ -2095,12 +2142,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
     scope.own({&ttree.local, &atree.local, &ctree.local});
     scope.fri = &fri;
     struct SLayer { u64* vals; size_t m_l, m_g; ShardTree tree; };
-    std::vector<SLayer> slayers;   // FRI layers folded on row shards
-    std::vector<void*> owned;      // device buffers of the sharded FRI phase
-    struct Cleanup {
-        wf_ctx* ctx; std::vector<SLayer>& sl; std::vector<void*>& ow;
-        ~Cleanup() { for (auto& l : sl) wf_tree_free(ctx, l.tree.local); for (void* p : ow) wf_dev_free(ctx, p); }
-    } cleanup{ctx, slayers, owned};
+    std::vector<SLayer> slayers;   // FRI layers folded on row shards (their buffers and trees: `scope`'s)
 
     // ---- 1. interpolate the local columns, extend them coset by coset (no communication: columns are independent) and turn
     //         them into my row shard with its halo (shard_trace_lde) ----
@@ -2118,23 +2160,16 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
     //          columns on the trace domain, one all-gather by segment gives every rank the whole n x c main trace, and every
     //          rank builds and interpolates the aux segment (replicated, deterministic); its LDE is sharded as the composition
     //          polynomial's, with the halo the constraint evaluation reads ----
-    std::vector<u64> rnd_flat;  // [nr][D], canonical
-    wf_mat aview;               // my aux rows
+    std::vector<u64> rnd_flat, rnd_user;  // [nr][D], canonical / as the callback sees them
+    wf_mat aview;                         // my aux rows
     if (aw) {
-        for (u32 i = 0; i < air.nr; i++) { GlExt<D> e = draw_ext<D>(ch.coin); for (int q = 0; q < D; q++) rnd_flat.push_back(e.v[q]); }
+        draw_aux_rand<D>(ch.coin, air.nr, mont, rnd_flat, rnd_user);
         CKI(gather_main_trace(sc, polys, log_n, c, seg0, segs, mtrace));
         wf_mark(ctx, "main_trace_gather");
         CKI(wf_aux_build_run(ctx, *aux_build, mtrace, c, air.periodic, rnd_flat.data(), air.nr, D, &atrace));
         if (!validate) scope.drop(mtrace);   // else: the whole main trace the trace check reads
         wf_mark(ctx, "aux_build");
-        if (aux_assertions) {
-            std::vector<u64> rnd_user = rnd_flat;
-            if (mont) for (u64& v : rnd_user) v = gl_mul(v, 0xFFFFFFFFULL);  // x * R, R = 2^64 mod p
-            std::vector<u64> vals = get_aux_assertion_words(air_dyn, D, mont);
-            if (aux_assertions(aux_user, rnd_user.data(), vals.data()) != 0) return wf_fail(ctx, WF_ERR_INVALID, "aux assertion callback failed");
-            if (!set_aux_assertion_words(air_dyn, vals.data(), D, mont))
-                return wf_fail(ctx, WF_ERR_INVALID, "aux assertion value is not a canonical field element");
-        }
+        CKI(apply_aux_assertions(ctx, air_dyn, aux_assertions, aux_user, rnd_user, D, mont));
         CKI(wf_mat_interpolate(ctx, atrace, &apolys));
         if (!validate) scope.drop(atrace);
         CKI(shard_lde_rows(sc, apolys, log_b, true, &arows, aview));
@@ -2188,7 +2223,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
         CKI(ood_eval<D>(ctx, mats, z, zg, ood));
     }
     const u32 ct = c + aw;
-    std::vector<GlExt<D>> t_cur(c), t_nxt(c);
+    OodFrame<D> of{std::vector<GlExt<D>>(c), std::vector<GlExt<D>>(c)};
     {
         std::vector<u64> mine((size_t)maxcl * 2 * D, 0), all((size_t)G * maxcl * 2 * D);
         const size_t mi = aw ? 4 : 2;   // my columns' values in `ood`
@@ -2199,23 +2234,16 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
             for (u32 jl = 0; jl < ncol[s]; jl++) {
                 const u32 j = col0[s] + jl;
                 const u64* v = &all[((size_t)s * maxcl + jl) * 2 * D];
-                for (int q = 0; q < D; q++) { t_cur[j].v[q] = v[q]; t_nxt[j].v[q] = v[D + q]; }
+                for (int q = 0; q < D; q++) { of.t_cur[j].v[q] = v[q]; of.t_nxt[j].v[q] = v[D + q]; }
             }
     }
-    if (aw) {  // trace frame rows = main columns then aux columns (ood_frame.rs:40-72)
-        auto a_cur = ext_from_components<D>(ood[2]), a_nxt = ext_from_components<D>(ood[3]);
-        t_cur.insert(t_cur.end(), a_cur.begin(), a_cur.end());
-        t_nxt.insert(t_nxt.end(), a_nxt.begin(), a_nxt.end());
-    }
-    std::vector<GlExt<D>> q_cur = ext_from_components<D>(ood[0]), q_nxt = ext_from_components<D>(ood[1]);
-    ByteVec ood_t, ood_q;
-    ch.coin.reseed(ood_frames<D>(h, t_cur, t_nxt, q_cur, q_nxt, &ood_t, &ood_q));
+    ood_frame<D>(ch, of, &ood[0], aw ? &ood[2] : nullptr);
     wf_mark(ctx, "ood_frames");
     // ---- 6. DEEP composition over my LDE rows (evaluation form is row-local) ----
     std::vector<GlExt<D>> dc = draw_coeffs<D>(ch.coin, o.batch_d, ct + kc);
     GlExt<D> Sz = ext_zero<D>(), Szg = ext_zero<D>();
-    for (u32 j = 0; j < ct; j++) { Sz = ext_add(Sz, ext_mul(dc[j], t_cur[j])); Szg = ext_add(Szg, ext_mul(dc[j], t_nxt[j])); }
-    for (u32 j = 0; j < kc; j++) { Sz = ext_add(Sz, ext_mul(dc[ct + j], q_cur[j])); Szg = ext_add(Szg, ext_mul(dc[ct + j], q_nxt[j])); }
+    for (u32 j = 0; j < ct; j++) { Sz = ext_add(Sz, ext_mul(dc[j], of.t_cur[j])); Szg = ext_add(Szg, ext_mul(dc[j], of.t_nxt[j])); }
+    for (u32 j = 0; j < kc; j++) { Sz = ext_add(Sz, ext_mul(dc[ct + j], of.q_cur[j])); Szg = ext_add(Szg, ext_mul(dc[ct + j], of.q_nxt[j])); }
     CKI(deep_compose<D>(ctx, shard, aw ? &aview : nullptr, &cview, kc, log_n + log_b, dc, z, zg, Sz, Szg, &deep, (size_t)r * rows_per, rows_per));
     wf_mark(ctx, "deep_composition");
     // ---- 7. FRI: layers folded on shards while they are large. A layer of L points is held as contiguous position
@@ -2235,8 +2263,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
         sl.m_g = L / nf;
         sl.m_l = sl.m_g / (size_t)G;
         void* vp;
-        CKI(wf_dev_alloc(ctx, (size_t)nf * sl.m_l * ld * 8, &vp));
-        owned.push_back(vp);
+        CKI(scope.bufs.alloc((size_t)nf * sl.m_l * ld * 8, &vp));
         sl.vals = (u64*)vp;
         std::vector<int> sp, rp;
         std::vector<const void*> sv;
@@ -2256,6 +2283,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
         }
         CKI(sc.exchange(sp, sv, rp, rv, sl.m_l * ld * 8));
         CKI(wf_fri_layer_tree(ctx, h, sl.vals, (size_t)nf * sl.m_l, D, ld, (int)nf, &sl.tree.local));
+        scope.held.push_back(sl.tree.local);
         sl.tree.n_global = sl.m_g;
         slayers.push_back(sl);
         CKI(shard_tree_finish(sc, h, slayers.back().tree, &root));
@@ -2265,8 +2293,7 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
         const u64* master;
         CKI(wf_get_twiddles(ctx, logL, &master));
         void* nx;
-        CKI(wf_dev_alloc(ctx, sl.m_l * ld * 8, &nx));
-        owned.push_back(nx);
+        CKI(scope.bufs.alloc(sl.m_l * ld * 8, &nx));
         if (ld > D) CK(cudaMemsetAsync(nx, 0, sl.m_l * ld * 8, ctx->st));
         u64 av[3] = {0, 0, 0};
         for (int q = 0; q < D; q++) av[q] = alpha.v[q];
@@ -2288,17 +2315,10 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
     wf_mark(ctx, "fri_layers");
     // ---- 8. grinding + query positions (every rank; deterministic) ----
     u64 nonce;
-    CKI(grind_on_device(ctx, h, ch.coin.seed, o.grinding, &nonce));
-    if (ch.coin.check_leading_zeros(nonce) < o.grinding) return wf_fail(ctx, WF_ERR_STATE, "grinding self-check failed");
     std::vector<u64> pos;
-    if (!query_positions(ch.coin, o.num_queries, N, nonce, pos)) return wf_fail(ctx, WF_ERR_STATE, "failed to draw query positions");
+    CKI(grind_and_query(ctx, ch, o, N, &nonce, pos));
     wf_mark(ctx, "grinding");
     // ---- 9. proof object: every rank queues the same gathers, contributes what it holds, the words are summed ----
-    ByteVec w;
-    write_context(w, air, log_n, o);
-    w.u8_((u8)pos.size());
-    w.u16_((uint16_t)ch.commitments.v.size());
-    w.bytes(ch.commitments.v.data(), ch.commitments.v.size());
     GatherBatch gb;
     gb.comm = cm;
     const u64 NONE = ~(u64)0;
@@ -2309,11 +2329,10 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
     };
     std::vector<std::pair<size_t, u64>> top_t, top_a, top_c;
     const std::vector<u64> mine = owned_rows(pos, rows_per);
-    size_t tr_rows = gb.add_rows(shard->m, mine), cr_rows = gb.add_rows(cview.m, mine), ar_rows = aw ? gb.add_rows(aview.m, mine) : 0;
-    size_t tr_dig, cr_dig, ar_dig = 0;
-    CKI(gb.add_opening_sharded(ctx, ttree.local, N, G, r, pos, &tr_dig, &top_t));
-    CKI(gb.add_opening_sharded(ctx, ctree.local, N, G, r, pos, &cr_dig, &top_c));
-    if (aw) CKI(gb.add_opening_sharded(ctx, atree.local, N, G, r, pos, &ar_dig, &top_a));
+    QueryIds id(gb, shard->m, cview.m, aw ? &aview.m : nullptr, mine);
+    CKI(gb.add_opening_sharded(ctx, ttree.local, N, G, r, pos, &id.tr_dig, &top_t));
+    CKI(gb.add_opening_sharded(ctx, ctree.local, N, G, r, pos, &id.cr_dig, &top_c));
+    if (aw) CKI(gb.add_opening_sharded(ctx, atree.local, N, G, r, pos, &id.ar_dig, &top_a));
     FriProofPlan splan;   // the sharded layers' gathers, and per layer the slots of the nodes above the subtree roots
     std::vector<std::vector<std::pair<size_t, u64>>> top_f(slayers.size());
     std::vector<u64> fpos = pos;
@@ -2345,19 +2364,12 @@ int prove_sharded(wf_ctx* ctx, const wf_comm* cm, const AirHost& air_in, const A
     auto patch = [&](size_t dig_id, const std::vector<std::pair<size_t, u64>>& slots, const ShardTree& t) {
         for (auto& se : slots) memcpy(gb.digest_words(dig_id) + se.first * 4, t.top[se.second].b, 32);
     };
-    patch(tr_dig, top_t, ttree);
-    patch(cr_dig, top_c, ctree);
-    if (aw) patch(ar_dig, top_a, atree);
+    patch(id.tr_dig, top_t, ttree);
+    patch(id.cr_dig, top_c, ctree);
+    if (aw) patch(id.ar_dig, top_a, atree);
     for (size_t l = 0; l < slayers.size(); l++) patch(splan.dig_ids[l], top_f[l], slayers[l].tree);
-    write_queries(gb, tr_rows, tr_dig, pos.size() * c, w);
-    if (aw) write_queries(gb, ar_rows, ar_dig, pos.size() * aw * D, w);  // trace_lde/default/mod.rs:199-218
-    write_queries(gb, cr_rows, cr_dig, pos.size() * kc * D, w);
-    w.u16_((uint16_t)ood_t.v.size()); w.bytes(ood_t.v.data(), ood_t.v.size());
-    w.u16_((uint16_t)ood_q.v.size()); w.bytes(ood_q.v.data(), ood_q.v.size());
-    wf_fri_finish_proof(fri, gb, fplan, w, &splan);   // the sharded layers, then the replicated ones
-    w.u64_(nonce);
+    write_proof<D>(air, log_n, o, ch, pos, gb, id, of, fri, fplan, &splan, nonce, proof_out);
     wf_mark(ctx, "queries_and_proof");
-    proof_out.swap(w.v);
     if (stats) {
         CK(cudaStreamSynchronize(ctx->st));
         stats[0] = sc.bytes_sent; stats[1] = sc.exchange_ms(); stats[2] = sc.ncoll + 1; stats[3] = sc.ms_small;
@@ -2396,15 +2408,19 @@ static int prove_bytes(wf_ctx* ctx, const AirHost& air, const uint64_t* const* t
     }
     return wf_fail(ctx, WF_ERR_UNSUPPORTED, "field extension %u", o.ext);
 }
+// the caller's proof buffer <- the proof bytes
+static int copy_proof_out(wf_ctx* ctx, const std::vector<u8>& out, uint8_t* proof, size_t* proof_len) {
+    if (out.size() > *proof_len) return wf_fail(ctx, WF_ERR_INVALID, "proof buffer too small (%zu needed)", out.size());
+    memcpy(proof, out.data(), out.size());
+    *proof_len = out.size();
+    return WF_OK;
+}
 static int prove_dispatch(wf_ctx* ctx, const AirHost& air, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont,
                           uint32_t log_n, const Options& o, uint8_t* proof, size_t* proof_len, wf_aux_builder_fn aux_builder = nullptr,
                           void* aux_user = nullptr, wf_aux_assertions_fn aux_assertions = nullptr, const AuxBuildHost* aux_build = nullptr) {
     std::vector<u8> out;
     CKI(prove_bytes(ctx, air, trace_cols, d_trace, mont, log_n, o, out, aux_builder, aux_user, aux_assertions, aux_build));
-    if (out.size() > *proof_len) return wf_fail(ctx, WF_ERR_INVALID, "proof buffer too small (%zu needed)", out.size());
-    memcpy(proof, out.data(), out.size());
-    *proof_len = out.size();
-    return WF_OK;
+    return copy_proof_out(ctx, out, proof, proof_len);
 }
 static int prove_fib_entry(wf_ctx* ctx, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont, uint32_t k,
                            uint32_t log_n, const uint64_t* results, const uint32_t* opts, uint8_t* proof, size_t* proof_len) {
@@ -2449,26 +2465,33 @@ extern "C" int wf_prove_air_aux_dyn(wf_ctx* ctx, const uint64_t* air_desc, size_
     return prove_dispatch(ctx, air, trace_cols, nullptr, mont, log_n, o, proof, proof_len, aux_builder, aux_user, aux_assertions);
 }
 
+// msg <- t, cut to msg_cap - 1 bytes (nothing without a buffer)
+static void copy_msg(char* msg, size_t msg_cap, const char* t) {
+    if (msg && msg_cap) { strncpy(msg, t, msg_cap - 1); msg[msg_cap - 1] = 0; }
+}
+
 // ---- aux segment from a described build (auxbuild.cu): the device analogue of Prover::build_aux_trace ----
-static int parse_aux_build(wf_ctx* ctx, const AirHost& air, const uint64_t* aux_build, size_t aux_build_len, AuxBuildHost& b) {
+// Refuses init words beyond extension degree `ext` (3: any degree)
+static int parse_aux_build(wf_ctx* ctx, const AirHost& air, const uint64_t* aux_build, size_t aux_build_len, u32 ext, AuxBuildHost& b) {
     if (!air.aw) return wf_fail(ctx, WF_ERR_INVALID, "single-segment AIR: it has no aux segment to build");
     if (const char* why = wf_aux_build_parse(aux_build, aux_build_len, air.w, air.aw, (u32)air.periodic.size(), air.nr, b))
         return wf_fail(ctx, WF_ERR_INVALID, "%s", why);
+    for (auto& col : b.cols)
+        for (u32 q = ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
     return WF_OK;
 }
 extern "C" int wf_aux_build_check(const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len,
                                   uint32_t log_n, char* msg, size_t msg_cap) {
-    auto say = [&](const char* t) { if (msg && msg_cap) { strncpy(msg, t, msg_cap - 1); msg[msg_cap - 1] = 0; } };
-    say("");
-    if (!air_desc || !aux_build || log_n < 3 || log_n > 32) { say("bad arguments"); return WF_ERR_INVALID; }
+    copy_msg(msg, msg_cap, "");
+    if (!air_desc || !aux_build || log_n < 3 || log_n > 32) { copy_msg(msg, msg_cap, "bad arguments"); return WF_ERR_INVALID; }
     AirHost air;
-    if (!parse_air_host(air_desc, air_desc_len, air)) { say("malformed AIR description"); return WF_ERR_INVALID; }
+    if (!parse_air_host(air_desc, air_desc_len, air)) { copy_msg(msg, msg_cap, "malformed AIR description"); return WF_ERR_INVALID; }
     wf_ctx note{};   // carries the message, nothing else
     AuxBuildHost b;
-    int r = parse_aux_build(&note, air, aux_build, aux_build_len, b);
+    int r = parse_aux_build(&note, air, aux_build, aux_build_len, 3, b);
     for (auto& col : air.periodic)
         if (r == WF_OK && col.size() > ((size_t)1 << log_n)) r = wf_fail(&note, WF_ERR_INVALID, "periodic column longer than the trace");
-    say(note.err.c_str());
+    copy_msg(msg, msg_cap, note.err.c_str());
     return r;
 }
 extern "C" int wf_aux_build(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len,
@@ -2477,7 +2500,7 @@ extern "C" int wf_aux_build(wf_ctx* ctx, const uint64_t* air_desc, size_t air_de
     AirHost air;
     if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
     AuxBuildHost b;
-    CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
+    CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, 3, b));   // wf_aux_build_run refuses init words beyond `ext`
     if (air.nr && !rand) return wf_fail(ctx, WF_ERR_INVALID, "random elements missing");
     return wf_aux_build_run(ctx, b, main_evals, air.w, air.periodic, rand, air.nr, (int)ext, aux);
 }
@@ -2492,9 +2515,7 @@ extern "C" int wf_prove_air_aux_built(wf_ctx* ctx, const uint64_t* air_desc, siz
     AirHost air;
     if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
     AuxBuildHost b;
-    CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
-    for (auto& col : b.cols)
-        for (u32 q = o.ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
+    CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, o.ext, b));
     return prove_dispatch(ctx, air, trace_cols, d_trace, mont, log_n, o, proof, proof_len, nullptr, aux_user, aux_assertions, &b);
 }
 
@@ -2508,21 +2529,20 @@ extern "C" int wf_jit_compile_air(const uint64_t* air_desc, size_t air_desc_len,
     std::string lg;
     const int rc = wf_jit_compile(wf_jit_source((int)ext, air.w, (u32)air.periodic.size(), air.num_regs, air.prog, air.consts, air.aw, air.nr,
                                                 air.aux_num_regs, air.aux_prog), cubin, lg);
-    if (log && log_cap) { strncpy(log, lg.c_str(), log_cap - 1); log[log_cap - 1] = 0; }
+    copy_msg(log, log_cap, lg.c_str());
     if (cubin_bytes) *cubin_bytes = cubin.size();
     if (const char* dump = getenv("WF_JIT_DUMP")) if (rc == 0) { FILE* f = fopen(dump, "wb"); if (f) { fwrite(cubin.data(), 1, cubin.size(), f); fclose(f); } }
     return rc == 0 ? WF_OK : WF_ERR_UNSUPPORTED;
 }
 
 extern "C" int wf_air_check(const uint64_t* air_desc, size_t air_desc_len, uint32_t log_n, uint32_t blowup, char* msg, size_t msg_cap) {
-    auto say = [&](const char* t) { if (msg && msg_cap) { strncpy(msg, t, msg_cap - 1); msg[msg_cap - 1] = 0; } };
-    say("");
-    if (!air_desc || log_n < 3 || log_n > 32 || blowup < 2 || blowup > 128 || (blowup & (blowup - 1))) { say("bad arguments"); return WF_ERR_INVALID; }
+    copy_msg(msg, msg_cap, "");
+    if (!air_desc || log_n < 3 || log_n > 32 || blowup < 2 || blowup > 128 || (blowup & (blowup - 1))) { copy_msg(msg, msg_cap, "bad arguments"); return WF_ERR_INVALID; }
     AirHost air;
-    if (!parse_air_host(air_desc, air_desc_len, air)) { say("malformed AIR description"); return WF_ERR_INVALID; }
+    if (!parse_air_host(air_desc, air_desc_len, air)) { copy_msg(msg, msg_cap, "malformed AIR description"); return WF_ERR_INVALID; }
     wf_ctx note{};   // carries the message of the shared validators, nothing else
     const int r = air_check_host(&note, air, log_n, blowup);
-    say(note.err.c_str());
+    copy_msg(msg, msg_cap, note.err.c_str());
     return r;
 }
 
@@ -2547,7 +2567,7 @@ extern "C" int wf_air_batch_check(uint32_t batch, const uint64_t* const* air_des
     wf_ctx note{};
     std::vector<AirHost> airs;
     const int r = air_batch_parse(&note, batch, air_descs, air_desc_lens, log_n, blowup, airs);
-    if (msg && msg_cap) { strncpy(msg, note.err.c_str(), msg_cap - 1); msg[msg_cap - 1] = 0; }
+    copy_msg(msg, msg_cap, note.err.c_str());
     return r;
 }
 extern "C" int wf_prove_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* const* air_descs, const size_t* air_desc_lens,
@@ -2562,9 +2582,7 @@ extern "C" int wf_prove_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* c
     for (u32 j = 0; j < batch; j++) if (!proofs[j]) return wf_fail(ctx, WF_ERR_INVALID, "proof %u: no output buffer", j);
     AuxBuildHost b;
     if (aux_build) {
-        CKI(parse_aux_build(ctx, airs[0], aux_build, aux_build_len, b));
-        for (auto& col : b.cols)
-            for (u32 q = o.ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
+        CKI(parse_aux_build(ctx, airs[0], aux_build, aux_build_len, o.ext, b));
     } else if (airs[0].aw) {
         return wf_fail(ctx, WF_ERR_INVALID, "multi-segment AIR: a batch builds its aux segments from aux_build");
     }
@@ -2590,14 +2608,29 @@ extern "C" int wf_prove_air_batch(wf_ctx* ctx, uint32_t batch, const uint64_t* c
 
 // ---- the reference's debug-build checks of a trace (validate.cu), standalone ----
 // the report of wf_trace_validate / wf_trace_validate_sharded
-static void write_validation(const TraceReport& rep, u32 n_tr, int check_degrees, wf_validation* report, uint64_t* first_failing_step,
+static void write_validation(const TraceReport& rep, const AirHost& air, int check_degrees, wf_validation* report, uint64_t* first_failing_step,
                              uint64_t* expected_degrees, uint64_t* actual_degrees, char* msg, size_t msg_cap) {
     report->kind = rep.kind; report->index = rep.index; report->step = rep.step; report->column = rep.column;
-    report->num_transition_constraints = n_tr;
+    report->num_transition_constraints = (u32)(air.degrees.size() + (air.aw ? air.aux_degrees.size() : 0));
     if (first_failing_step) std::copy(rep.first_fail.begin(), rep.first_fail.end(), first_failing_step);
     if (check_degrees && expected_degrees) std::copy(rep.expected.begin(), rep.expected.end(), expected_degrees);
     if (check_degrees && actual_degrees) std::copy(rep.actual.begin(), rep.actual.end(), actual_degrees);
-    if (msg && msg_cap) { strncpy(msg, rep.msg.c_str(), msg_cap - 1); msg[msg_cap - 1] = 0; }
+    copy_msg(msg, msg_cap, rep.msg.c_str());
+}
+// The checks of wf_trace_validate / wf_trace_validate_sharded on the description and the aux segment's source, in this order
+static int trace_validate_args(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len,
+                               const uint64_t* const* aux_cols, const uint64_t* rand, uint32_t log_n, uint32_t ext, AirHost& air,
+                               AuxBuildHost& b) {
+    if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
+    CKI(air_check_host(ctx, air, log_n, 1u << air.log_ce_blowup()));
+    if (air.aw) {
+        if (!aux_build == !aux_cols) return wf_fail(ctx, WF_ERR_INVALID, "two-segment AIR: pass exactly one of aux_build and aux_cols");
+        if (air.nr && !rand) return wf_fail(ctx, WF_ERR_INVALID, "random elements missing");
+        if (aux_build) CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, ext, b));
+    } else if (aux_build || aux_cols) {
+        return wf_fail(ctx, WF_ERR_INVALID, "single-segment AIR: it has no aux segment");
+    }
+    return WF_OK;
 }
 extern "C" int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t air_desc_len, const uint64_t* aux_build, size_t aux_build_len,
                                  const uint64_t* const* aux_cols, const uint64_t* const* trace_cols, const uint64_t* d_trace, int mont,
@@ -2607,23 +2640,11 @@ extern "C" int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t a
     if (!ctx || !air_desc || !report || log_n < 3 || log_n > 30 || ext < 1 || ext > 3) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     if (!trace_cols == !d_trace) return wf_fail(ctx, WF_ERR_INVALID, "pass exactly one of trace_cols (host) and d_trace (device)");
     AirHost air;
-    if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
-    const u32 log_ceb = air.log_ce_blowup();
-    CKI(air_check_host(ctx, air, log_n, 1u << log_ceb));
     AuxBuildHost b;
-    if (air.aw) {
-        if (!aux_build == !aux_cols) return wf_fail(ctx, WF_ERR_INVALID, "two-segment AIR: pass exactly one of aux_build and aux_cols");
-        if (air.nr && !rand) return wf_fail(ctx, WF_ERR_INVALID, "random elements missing");
-        if (aux_build) {
-            CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
-            for (auto& col : b.cols)
-                for (u32 q = ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
-        }
-    } else if (aux_build || aux_cols) {
-        return wf_fail(ctx, WF_ERR_INVALID, "single-segment AIR: it has no aux segment");
-    }
+    CKI(trace_validate_args(ctx, air_desc, air_desc_len, aux_build, aux_build_len, aux_cols, rand, log_n, ext, air, b));
+    const u32 log_ceb = air.log_ce_blowup();
     const size_t n = (size_t)1 << log_n;
-    const u32 c = air.w, n_tr = (u32)(air.degrees.size() + (air.aw ? air.aux_degrees.size() : 0));
+    const u32 c = air.w;
     const std::vector<u64> rnd(rand, rand + (air.aw ? (size_t)air.nr * ext : 0));
     wf_mat *trace = nullptr, *atrace = nullptr, *polys = nullptr, *apolys = nullptr, *lde = nullptr, *alde = nullptr;
     ProofScope scope(ctx);
@@ -2650,7 +2671,28 @@ extern "C" int wf_trace_validate(wf_ctx* ctx, const uint64_t* air_desc, size_t a
         }
         CKI(wf_check_degrees(ctx, air, lde, alde, rnd.data(), log_n, log_ceb, (int)ext, rep));
     }
-    write_validation(rep, n_tr, check_degrees, report, first_failing_step, expected_degrees, actual_degrees, msg, msg_cap);
+    write_validation(rep, air, check_degrees, report, first_failing_step, expected_degrees, actual_degrees, msg, msg_cap);
+    return WF_OK;
+}
+
+// A sharded call's checks on this rank's own arguments: its block of main columns and, for the prover, its output buffer
+// (out_ok; nullptr: the call has none). Every rank learns every rank's verdict in the call's first collective, and all of them
+// return when one refuses.
+static int agree_on_columns(wf_ctx* ctx, const wf_comm* comm, u32 w, u32 local_count, const uint64_t* const* local_cols,
+                            const uint64_t* d_local, const bool* out_ok) {
+    const int G = comm->world;
+    u32 first, count;
+    shard_columns(w, (u32)G, (u32)comm->rank, first, count);
+    int mine = WF_OK;
+    if (local_count != count)
+        mine = wf_fail(ctx, WF_ERR_INVALID, "rank %d owns %u columns of %u (wf_shard_columns), not %u", comm->rank, count, w, local_count);
+    else if ((count && !local_cols == !d_local) || (out_ok && !*out_ok))
+        mine = wf_fail(ctx, WF_ERR_INVALID, "bad arguments: pass exactly one of local_cols and d_local%s", out_ok ? ", and an output buffer" : "");
+    std::vector<int> verdicts(G);
+    if (comm->all_gather_host(comm->user, &mine, verdicts.data(), sizeof(int)) != 0) return wf_fail(ctx, WF_ERR_STATE, "all_gather_host callback failed");
+    if (mine != WF_OK) return mine;
+    for (int q = 0; q < G; q++)
+        if (verdicts[q] != WF_OK) return wf_fail(ctx, WF_ERR_INVALID, "rank %d refused its column block%s", q, out_ok ? " or output buffer" : "");
     return WF_OK;
 }
 
@@ -2716,39 +2758,14 @@ extern "C" int wf_trace_validate_sharded(wf_ctx* ctx, const wf_comm* comm, const
     if (G < 2 || (G & (G - 1)) || comm->rank < 0 || comm->rank >= G) return wf_fail(ctx, WF_ERR_INVALID, "world size must be a power of two >= 2");
     if (!air_desc || !report || log_n < 3 || log_n > 30 || ext < 1 || ext > 3) return wf_fail(ctx, WF_ERR_INVALID, "bad arguments");
     AirHost air;
-    if (!parse_air_host(air_desc, air_desc_len, air)) return wf_fail(ctx, WF_ERR_INVALID, "malformed AIR description");
-    const u32 log_ceb = air.log_ce_blowup();
-    CKI(air_check_host(ctx, air, log_n, 1u << log_ceb));
     AuxBuildHost b;
-    if (air.aw) {
-        if (!aux_build == !aux_cols) return wf_fail(ctx, WF_ERR_INVALID, "two-segment AIR: pass exactly one of aux_build and aux_cols");
-        if (air.nr && !rand) return wf_fail(ctx, WF_ERR_INVALID, "random elements missing");
-        if (aux_build) {
-            CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
-            for (auto& col : b.cols)
-                for (u32 q = ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
-        }
-    } else if (aux_build || aux_cols) {
-        return wf_fail(ctx, WF_ERR_INVALID, "single-segment AIR: it has no aux segment");
-    }
+    CKI(trace_validate_args(ctx, air_desc, air_desc_len, aux_build, aux_build_len, aux_cols, rand, log_n, ext, air, b));
+    const u32 log_ceb = air.log_ce_blowup();
     // the row shard of the prover (rows_per >= 64 blowup, ce_per >= 64) with the CE blowup in place of the proof's: n >= 64 G
     const size_t rows_per = ((size_t)1 << (log_n + log_ceb)) / (size_t)G;
     if (log_n + log_ceb > 32 || rows_per < ((size_t)64 << log_ceb))
         return wf_fail(ctx, WF_ERR_UNSUPPORTED, "trace too short to shard over %d ranks", G);
-    // this rank's own arguments (its column block): every rank learns every rank's verdict in the first collective, and all of
-    // them return when one refuses
-    u32 first, count;
-    shard_columns(air.w, (u32)G, (u32)comm->rank, first, count);
-    int mine = WF_OK;
-    if (local_count != count)
-        mine = wf_fail(ctx, WF_ERR_INVALID, "rank %d owns %u columns of %u (wf_shard_columns), not %u", comm->rank, count, air.w, local_count);
-    else if (count && !local_cols == !d_local)
-        mine = wf_fail(ctx, WF_ERR_INVALID, "bad arguments: pass exactly one of local_cols and d_local");
-    std::vector<int> verdicts(G);
-    if (comm->all_gather_host(comm->user, &mine, verdicts.data(), sizeof(int)) != 0) return wf_fail(ctx, WF_ERR_STATE, "all_gather_host callback failed");
-    if (mine != WF_OK) return mine;
-    for (int q = 0; q < G; q++)
-        if (verdicts[q] != WF_OK) return wf_fail(ctx, WF_ERR_INVALID, "rank %d refused its column block", q);
+    CKI(agree_on_columns(ctx, comm, air.w, local_count, local_cols, d_local, nullptr));
     const std::vector<u64> rnd(rand, rand + (air.aw ? (size_t)air.nr * ext : 0));
     const AuxBuildHost* bp = air.aw && aux_build ? &b : nullptr;
     TraceReport rep;
@@ -2759,8 +2776,7 @@ extern "C" int wf_trace_validate_sharded(wf_ctx* ctx, const wf_comm* comm, const
         default: r = validate_sharded<3>(ctx, comm, air, bp, aux_cols, local_cols, d_local, mont, rnd, log_n, check_degrees != 0, rep); break;
     }
     CKI(r);
-    const u32 n_tr = (u32)(air.degrees.size() + (air.aw ? air.aux_degrees.size() : 0));
-    write_validation(rep, n_tr, check_degrees, report, first_failing_step, expected_degrees, actual_degrees, msg, msg_cap);
+    write_validation(rep, air, check_degrees, report, first_failing_step, expected_degrees, actual_degrees, msg, msg_cap);
     return WF_OK;
 }
 
@@ -2977,12 +2993,15 @@ extern "C" int wf_deep_compose_polys(wf_ctx* ctx, uint32_t ext, const wf_mat* ma
     }
 }
 
-static int sharded_output(wf_ctx* ctx, int r, const std::vector<u8>& out, uint8_t* proof, size_t* proof_len) {
-    if (r != WF_OK) return r;
-    if (out.size() > *proof_len) return wf_fail(ctx, WF_ERR_INVALID, "proof buffer too small (%zu needed)", out.size());
-    memcpy(proof, out.data(), out.size());
-    *proof_len = out.size();
-    return WF_OK;
+// the proof bytes of one sharded proof, prove_sharded<D> for the extension degree of the options
+static int prove_sharded_bytes(wf_ctx* ctx, const wf_comm* comm, const AirHost& air, const AuxBuildHost* aux_build,
+                               wf_aux_assertions_fn aux_assertions, void* aux_user, const uint64_t* const* local_cols, const uint64_t* d_local,
+                               int mont, uint32_t log_n, const Options& o, std::vector<u8>& out, double* stats) {
+    switch (o.ext) {
+        case 1: return prove_sharded<1>(ctx, comm, air, aux_build, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats);
+        case 2: return prove_sharded<2>(ctx, comm, air, aux_build, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats);
+        default: return prove_sharded<3>(ctx, comm, air, aux_build, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats);
+    }
 }
 extern "C" int wf_prove_fib_sharded(wf_ctx* ctx, const wf_comm* comm, const uint64_t* const* local_cols, const uint64_t* d_local, int mont,
                                     uint32_t k, uint32_t log_n, const uint64_t* results, const uint32_t* opts, uint8_t* proof,
@@ -2994,13 +3013,8 @@ extern "C" int wf_prove_fib_sharded(wf_ctx* ctx, const wf_comm* comm, const uint
     CKI(parse_options(ctx, opts, o));
     const AirHost air = fib_air_host(k, (size_t)1 << log_n, results);
     std::vector<u8> out;
-    int r;
-    switch (o.ext) {
-        case 1: r = prove_sharded<1>(ctx, comm, air, nullptr, nullptr, nullptr, local_cols, d_local, mont, log_n, o, out, stats); break;
-        case 2: r = prove_sharded<2>(ctx, comm, air, nullptr, nullptr, nullptr, local_cols, d_local, mont, log_n, o, out, stats); break;
-        default: r = prove_sharded<3>(ctx, comm, air, nullptr, nullptr, nullptr, local_cols, d_local, mont, log_n, o, out, stats); break;
-    }
-    return sharded_output(ctx, r, out, proof, proof_len);
+    CKI(prove_sharded_bytes(ctx, comm, air, nullptr, nullptr, nullptr, local_cols, d_local, mont, log_n, o, out, stats));
+    return copy_proof_out(ctx, out, proof, proof_len);
 }
 extern "C" int wf_shard_columns(uint32_t width, uint32_t world, uint32_t rank, uint32_t* first, uint32_t* count) {
     if (!first || !count || width == 0 || width > 255 || world == 0 || (world & (world - 1)) || rank >= world) return WF_ERR_INVALID;
@@ -3026,37 +3040,18 @@ extern "C" int wf_prove_air_sharded(wf_ctx* ctx, const wf_comm* comm, const uint
     AuxBuildHost b;
     if (air.aw) {
         if (!aux_build) return wf_fail(ctx, WF_ERR_INVALID, "two-segment AIR: the sharded prover builds its aux segment from aux_build");
-        CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, b));
-        for (auto& col : b.cols)
-            for (u32 q = o.ext; q < 3; q++) if (col.init[q]) return wf_fail(ctx, WF_ERR_INVALID, "aux column init has non-zero words beyond the extension degree");
+        CKI(parse_aux_build(ctx, air, aux_build, aux_build_len, o.ext, b));
     } else if (aux_build || aux_assertions) {
         return wf_fail(ctx, WF_ERR_INVALID, "single-segment AIR: it has no aux segment");
     }
     const size_t rows_per = ((size_t)1 << (log_n + log2_ceil(o.blowup))) / (size_t)G, ce_per = ((size_t)1 << (log_n + air.log_ce_blowup())) / (size_t)G;
     if (log_n + log2_ceil(o.blowup) > 32 || rows_per < 64 * (size_t)o.blowup || ce_per < 64)
         return wf_fail(ctx, WF_ERR_UNSUPPORTED, "trace too short to shard over %d ranks", G);
-    // this rank's own arguments (its column block, its output buffer): every rank learns every rank's verdict in the first
-    // collective, and all of them return when one refuses
-    u32 first, count;
-    shard_columns(air.w, (u32)G, (u32)comm->rank, first, count);
-    int mine = WF_OK;
-    if (local_count != count)
-        mine = wf_fail(ctx, WF_ERR_INVALID, "rank %d owns %u columns of %u (wf_shard_columns), not %u", comm->rank, count, air.w, local_count);
-    else if ((count && !local_cols == !d_local) || !proof || !proof_len)
-        mine = wf_fail(ctx, WF_ERR_INVALID, "bad arguments: pass exactly one of local_cols and d_local, and an output buffer");
-    std::vector<int> verdicts(G);
-    if (comm->all_gather_host(comm->user, &mine, verdicts.data(), sizeof(int)) != 0) return wf_fail(ctx, WF_ERR_STATE, "all_gather_host callback failed");
-    if (mine != WF_OK) return mine;
-    for (int q = 0; q < G; q++)
-        if (verdicts[q] != WF_OK) return wf_fail(ctx, WF_ERR_INVALID, "rank %d refused its column block or output buffer", q);
+    const bool out_ok = proof && proof_len;
+    CKI(agree_on_columns(ctx, comm, air.w, local_count, local_cols, d_local, &out_ok));
     std::vector<u8> out;
-    int r;
-    switch (o.ext) {
-        case 1: r = prove_sharded<1>(ctx, comm, air, air.aw ? &b : nullptr, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats); break;
-        case 2: r = prove_sharded<2>(ctx, comm, air, air.aw ? &b : nullptr, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats); break;
-        default: r = prove_sharded<3>(ctx, comm, air, air.aw ? &b : nullptr, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats); break;
-    }
-    return sharded_output(ctx, r, out, proof, proof_len);
+    CKI(prove_sharded_bytes(ctx, comm, air, air.aw ? &b : nullptr, aux_assertions, aux_user, local_cols, d_local, mont, log_n, o, out, stats));
+    return copy_proof_out(ctx, out, proof, proof_len);
 }
 extern "C" int wf_prove_fib(wf_ctx* ctx, const uint64_t* const* trace_cols, int mont, uint32_t k, uint32_t log_n,
                             const uint64_t* results, const uint32_t* opts, uint8_t* proof, size_t* proof_len) {
